@@ -37,7 +37,7 @@ extern "C" {
 #define GSB_ERR_INVALID_ARG (-1)
 #define GSB_ERR_WORKSPACE (-2)
 #define GSB_ERR_UNSUPPORTED (-3)
-/* flags of gsb_rasterize_forward_packed_ex / gsb_rasterize_backward_ex */
+/* flags of gsb_rasterize_forward_packed / gsb_rasterize_backward */
 #define GSB_RASTER_CLAMP_MAX_ONE 1u
 
 typedef void *gsb_stream_t; /* cudaStream_t */
@@ -177,8 +177,8 @@ int gsb_gather_bin_edges(int m, int num_tiles, const int64_t *isect_ids_sorted,
 
 /* ---- Tile binning, fast path: two-level bucket sort fused with record packing ------------------
  * What RasterizeGaussians::forward needs between rasterize_gaussians.cpp:62 and :79 (cumsum, the M read-back,
- * emit, global sort, gather, bin edges, and the record packing of gsb_rasterize_forward) without a global sort and
- * without a host read-back in the middle of the frame.
+ * emit, global sort, gather, bin edges, and gsb_pack_records) without a global sort and without a host read-back in
+ * the middle of the frame.
  * cull = 0: tile_bins, cum_tiles_hit and the per-tile order (tile, then depth bits, ties by ascending unsorted
  *   slot) are bit-identical to gsb_cumsum_tiles_hit + gsb_map_gaussian_to_intersects + gsb_sort_intersects +
  *   gsb_gather_bin_edges.
@@ -198,12 +198,7 @@ int gsb_gather_bin_edges(int m, int num_tiles, const int64_t *isect_ids_sorted,
  *   gsb_rasterize_backward), tile_bins [tiles,2] (empty tiles (0,0)), stats.
  * gsb_bucket_sort_pack: fills `records`; optional outputs sorted_index [M] / gaussian_ids_sorted [M] (NULL to
  *   skip).  Returns GSB_ERR_UNSUPPORTED if len_capacity > gsb_bucket_max_tile_len() -- take the generic path.
- * gsb_rasterize_forward_packed: the blend kernel alone on an already packed record stream; m = the m_capacity
- *   the records buffer was sized with; bin_stats may be NULL.
- * tile_order (optional everywhere, [tiles] int32): a permutation of the tile ids, longest list first, written by
- *   gsb_bucket_tile_ranges and consumed by gsb_rasterize_forward_packed / gsb_rasterize_backward_ordered: the
- *   persistent blend warps take tiles in that order, so the tiles still running when the kernel drains are the
- *   cheapest ones.  No result depends on it (tiles are independent). */
+ * tile_order (optional, [tiles] int32): the longest-first tile order the blend calls take (see Rasterization). */
 int gsb_bucket_max_tile_len(void);
 size_t gsb_bucket_workspace_bytes(int n, int m_capacity, int num_tiles);
 int gsb_bucket_tile_ranges(int n, const float *xys, const int32_t *radii, const float *conics, const float *colors,
@@ -214,74 +209,59 @@ int gsb_bucket_sort_pack(int n, int m_capacity, int len_capacity, const float *d
                          const int32_t *cum_tiles_hit, int cull, int tiles_x, int tiles_y, const int32_t *tile_bins,
                          const int32_t *stats, void *workspace, size_t workspace_bytes, void *records,
                          int32_t *sorted_index, int32_t *gaussian_ids_sorted, gsb_stream_t stream);
-int gsb_rasterize_forward_packed(int img_h, int img_w, int tiles_x, int tiles_y, int m,
-                                 const int32_t *tile_bins, const int32_t *tile_order, const int32_t *bin_stats,
-                                 const float *background, void *records, float *out_img, float *final_Ts,
-                                 int32_t *final_idx, gsb_stream_t stream);
 
 /* ---- Rasterization ---------------------------------------------------------------------------
- * gsb_rasterize_forward replaces rasterize_forward_tensor (bindings.h:110-125, bindings.cu:338-410,
- *   kernel forward.cu:256-378).  Inputs as the reference (gaussian_ids_sorted [m], tile_bins
- *   [tiles,2], xys [n,2], conics [n,3], colors [n,3], opacities [n], background [3] on device) plus
- *   sorted_index [m] (the permutation from gsb_sort_intersects: sorted position -> unsorted
- *   intersection slot).  `records` is a caller-provided buffer of gsb_raster_records_bytes(m): the
- *   call packs the depth-sorted per-intersection stream (48 B/intersection + 256 B of scratch) that the
- *   blend kernel pulls with TMA bulk copies; keep it for the backward pass.  Outputs out_img [H,W,3],
- *   final_Ts [H,W], final_idx [H,W] i32, fully written.
- * gsb_rasterize_backward replaces rasterize_backward_tensor (bindings.h:174-189,
- *   bindings.cu:569-632, kernel backward.cu:161-355).  Consumes `records` from the forward call (its
- *   trailing scratch words are rewritten, hence non-const), conics [n,3] and opacities [n] (as the
- *   reference's signature), cum_tiles_hit [n] (gsb_cumsum_tiles_hit) and a scratch buffer grad_rows of
- *   gsb_raster_grad_rows_bytes(m).  v_output [H,W,3]; v_output_alpha [H,W] may be NULL (== zeros,
- *   rasterize_gaussians.cpp:108).  Writes v_xy [n,2], v_conic [n,3], v_colors [n,3], v_opacity [n]
- *   completely (no atomics, bit-reproducible run to run). */
+ * rasterize_forward_tensor (bindings.h:110-125, bindings.cu:338-410, kernel forward.cu:256-378) is gsb_pack_records
+ * followed by gsb_rasterize_forward_packed; rasterize_backward_tensor (bindings.h:174-189, bindings.cu:569-632,
+ * kernel backward.cu:161-355) is gsb_rasterize_backward.
+ * gsb_raster_records_bytes: size of the `records` buffer for m intersections: the depth-sorted 48-B
+ *   per-intersection records the blend kernels pull with TMA bulk copies, plus 256 B of scratch behind them that
+ *   every blend call rewrites (hence `records` is non-const in the backward too).
+ * gsb_raster_grad_rows_bytes: size of the backward's scratch buffer grad_rows for m intersections.
+ * gsb_pack_records: fills `records` from a sorted intersection list.  Inputs as the reference's
+ *   rasterize_forward_tensor (gaussian_ids_sorted [m], xys [n,2], conics [n,3], colors [n,3], opacities [n]) plus
+ *   sorted_index [m] (the permutation from gsb_sort_intersects: sorted position -> unsorted intersection slot).
+ *   gsb_bucket_sort_pack writes the same records on the fast path.
+ * gsb_rasterize_forward_packed: the blend kernel on a packed record stream; m = the count `records` was sized with
+ *   (the m_capacity on the fast path).  tile_bins [tiles,2], background [3]; writes out_img [H,W,3], final_Ts [H,W]
+ *   and final_idx [H,W] i32 completely.  Keep `records` for the backward pass.
+ * gsb_rasterize_forward_count: diagnostic twin of gsb_rasterize_forward_packed (same outputs, no tile order, no
+ *   flags) that also ACCUMULATES into pair_counts (device uint64[4]; zero it first) {records that pass the
+ *   per-record extent test, slot visits (x 32 lanes = pixel tests), pixel pairs evaluated (sigma inside the extent:
+ *   one ex2), pixel pairs blended} -- the work units SURVEY.md 8(d) asks the blend kernels' throughput to be quoted
+ *   in.  Never on a timed path.
+ * gsb_rasterize_backward: consumes `records`, tile_bins, tile_order, final_Ts and final_idx of the forward call,
+ *   conics [n,3] and opacities [n] (as the reference's signature), cum_tiles_hit [n] (the scan the records were
+ *   binned with) and grad_rows.  v_output [H,W,3]; v_output_alpha [H,W] may be NULL (== zeros,
+ *   rasterize_gaussians.cpp:108).  Writes v_xy [n,2], v_conic [n,3], v_colors [n,3], v_opacity [n] completely (no
+ *   atomics, bit-reproducible run to run).
+ * tile_order (optional, NULL = tile id order; [tiles] int32): a permutation of the tile ids, longest list first,
+ *   written by gsb_bucket_tile_ranges: the persistent blend warps take tiles in that order, so the tiles still
+ *   running when the kernel drains are the cheapest ones.  No result depends on it (tiles are independent).
+ * bin_stats (optional): the stats of gsb_bucket_tile_ranges; if they flag an overflow, the forward does nothing.
+ * flags: 0 or GSB_RASTER_CLAMP_MAX_ONE, which fuses the caller's `rgb = clamp_max(rgb, 1)` (model.cpp:222) into the
+ *   blend epilogue: out_img is written clamped, the channels that were cut are remembered in bits 28..30 of
+ *   final_idx (so m must stay below 2^28 and final_idx is private to the pair of calls), and the backward -- given
+ *   the same flag and the gradient of the CLAMPED image -- passes no gradient through them (torch's clamp_max mask
+ *   `x <= max`). */
 size_t gsb_raster_records_bytes(int m);
 size_t gsb_raster_grad_rows_bytes(int m);
-int gsb_rasterize_forward(int img_h, int img_w, int tiles_x, int tiles_y, int m,
-                          const int32_t *gaussian_ids_sorted, const int32_t *sorted_index,
-                          const int32_t *tile_bins, const float *xys, const float *conics,
-                          const float *colors, const float *opacities, const float *background,
-                          void *records, float *out_img, float *final_Ts, int32_t *final_idx,
-                          gsb_stream_t stream);
-int gsb_rasterize_backward_ordered(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
-                                   const int32_t *tile_bins, const int32_t *tile_order, const float *conics,
-                                   const float *opacities, void *records, const int32_t *cum_tiles_hit,
-                                   const float *background, const float *final_Ts, const int32_t *final_idx,
-                                   const float *v_output, const float *v_output_alpha, void *grad_rows, float *v_xy,
-                                   float *v_conic, float *v_colors, float *v_opacity, gsb_stream_t stream);
-/* gsb_pack_records: the packing half of gsb_rasterize_forward alone (sorted intersection list -> 48-B records).
- * gsb_rasterize_forward_packed_ex / gsb_rasterize_backward_ex: gsb_rasterize_forward_packed /
- *   gsb_rasterize_backward_ordered with `flags`.  GSB_RASTER_CLAMP_MAX_ONE fuses the caller's
- *   `rgb = clamp_max(rgb, 1)` (model.cpp:222) into the blend epilogue: out_img is written clamped, the channels that
- *   were cut are remembered in bits 28..30 of final_idx (so m must stay below 2^28 and final_idx is private to the
- *   pair of calls), and the backward call -- given the gradient of the CLAMPED image -- passes no gradient through
- *   them (torch's clamp_max mask `x <= max`). */
 int gsb_pack_records(int m, const int32_t *gaussian_ids_sorted, const int32_t *sorted_index, const float *xys,
                      const float *conics, const float *colors, const float *opacities, void *records,
                      gsb_stream_t stream);
-int gsb_rasterize_forward_packed_ex(int img_h, int img_w, int tiles_x, int tiles_y, int m, const int32_t *tile_bins,
-                                    const int32_t *tile_order, const int32_t *bin_stats, const float *background,
-                                    void *records, float *out_img, float *final_Ts, int32_t *final_idx,
-                                    unsigned flags, gsb_stream_t stream);
-int gsb_rasterize_backward_ex(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
-                              const int32_t *tile_bins, const int32_t *tile_order, const float *conics,
-                              const float *opacities, void *records, const int32_t *cum_tiles_hit,
-                              const float *background, const float *final_Ts, const int32_t *final_idx,
-                              const float *v_output, const float *v_output_alpha, void *grad_rows, float *v_xy,
-                              float *v_conic, float *v_colors, float *v_opacity, unsigned flags, gsb_stream_t stream);
-/* gsb_rasterize_forward_count: diagnostic twin of gsb_rasterize_forward_packed (same outputs) that also ACCUMULATES
- *   into pair_counts (device uint64[4]; zero it first) {records that pass the per-record extent test, slot visits
- *   (x 32 lanes = pixel tests), pixel pairs evaluated (sigma inside the extent: one ex2), pixel pairs blended} --
- *   the work units SURVEY.md 8(d) asks the blend kernels' throughput to be quoted in.  Never on a timed path. */
+int gsb_rasterize_forward_packed(int img_h, int img_w, int tiles_x, int tiles_y, int m, const int32_t *tile_bins,
+                                 const int32_t *tile_order, const int32_t *bin_stats, const float *background,
+                                 void *records, float *out_img, float *final_Ts, int32_t *final_idx,
+                                 unsigned flags, gsb_stream_t stream);
 int gsb_rasterize_forward_count(int img_h, int img_w, int tiles_x, int tiles_y, int m, const int32_t *tile_bins,
                                 const float *background, void *records, float *out_img, float *final_Ts,
                                 int32_t *final_idx, unsigned long long *pair_counts, gsb_stream_t stream);
-int gsb_rasterize_backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
-                           const int32_t *tile_bins, const float *conics, const float *opacities,
-                           void *records, const int32_t *cum_tiles_hit, const float *background,
-                           const float *final_Ts, const int32_t *final_idx, const float *v_output,
-                           const float *v_output_alpha, void *grad_rows, float *v_xy, float *v_conic,
-                           float *v_colors, float *v_opacity, gsb_stream_t stream);
+int gsb_rasterize_backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m, const int32_t *tile_bins,
+                           const int32_t *tile_order, const float *conics, const float *opacities, void *records,
+                           const int32_t *cum_tiles_hit, const float *background, const float *final_Ts,
+                           const int32_t *final_idx, const float *v_output, const float *v_output_alpha,
+                           void *grad_rows, float *v_xy, float *v_conic, float *v_colors, float *v_opacity,
+                           unsigned flags, gsb_stream_t stream);
 
 /* ---- Streaming helpers around the path (SURVEY.md 8f "next" rows) ------------------------------
  * gsb_mse_loss_grad: loss = mean((img-target)^2) written to *loss_out (device float; zeroed by the

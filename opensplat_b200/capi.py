@@ -46,22 +46,15 @@ _SIGS = {
     "gsb_gather_bin_edges": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_raster_records_bytes": (_sz, [_i]),
     "gsb_raster_grad_rows_bytes": (_sz, [_i]),
-    "gsb_rasterize_forward": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                                   _vp, _vp, _vp]),
+    "gsb_pack_records": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_rasterize_forward_packed": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint, _vp]),
+    "gsb_rasterize_forward_count": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_rasterize_backward": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                                    _vp, _vp, _vp, _vp, _vp, _vp]),
+                                    _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint, _vp]),
     "gsb_bucket_max_tile_len": (_i, []),
     "gsb_bucket_workspace_bytes": (_sz, [_i, _i, _i]),
     "gsb_bucket_tile_ranges": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
     "gsb_bucket_sort_pack": (_i, [_i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
-    "gsb_rasterize_forward_packed": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "gsb_rasterize_backward_ordered": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                                            _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "gsb_pack_records": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "gsb_rasterize_forward_packed_ex": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint, _vp]),
-    "gsb_rasterize_backward_ex": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                                       _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint, _vp]),
-    "gsb_rasterize_forward_count": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_activate_forward": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_activate_backward": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_densify_stats_update": (_i, [_i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),

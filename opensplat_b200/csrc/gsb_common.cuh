@@ -5,7 +5,7 @@
 #include <stdio.h>
 #include "../../include/gsplat_b200.h"
 
-#define GSB_VERSION 100
+#define GSB_VERSION 200
 
 // ---- error plumbing (thread-local message, C ABI returns the code) -------------------------
 void gsb_set_error(int code, const char *what, const char *file, int line);

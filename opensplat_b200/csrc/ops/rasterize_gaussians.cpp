@@ -159,11 +159,10 @@ torch::Tensor rasterizeForward(AutogradContext *ctx, unsigned flags, torch::Tens
                                             tileBins.data_ptr<int32_t>(), stats.data_ptr<int32_t>(), wp, wsBytes,
                                             records.data_ptr(), nullptr, nullptr, gsb::stream()),
                        "gsb_bucket_sort_pack");
-        gsb::check(gsb_rasterize_forward_packed_ex(imgHeight, imgWidth, tilesX, tilesY, mCap,
-                                                   tileBins.data_ptr<int32_t>(), tileOrder.data_ptr<int32_t>(),
-                                                   stats.data_ptr<int32_t>(), gsb::fp(bg), records.data_ptr(),
-                                                   gsb::fpw(outImg), gsb::fpw(finalTs),
-                                                   finalIdx.data_ptr<int32_t>(), flags, gsb::stream()),
+        gsb::check(gsb_rasterize_forward_packed(imgHeight, imgWidth, tilesX, tilesY, mCap, tileBins.data_ptr<int32_t>(),
+                                                tileOrder.data_ptr<int32_t>(), stats.data_ptr<int32_t>(), gsb::fp(bg),
+                                                records.data_ptr(), gsb::fpw(outImg), gsb::fpw(finalTs),
+                                                finalIdx.data_ptr<int32_t>(), flags, gsb::stream()),
                    "gsb_rasterize_forward_packed");
         // the path's single device->host read-back (rasterize_gaussians.cpp:63), waited for with the GPU busy
         statsReady.synchronize();
@@ -191,11 +190,11 @@ torch::Tensor rasterizeForward(AutogradContext *ctx, unsigned flags, torch::Tens
                                     gsb::fp(x), gsb::fp(con), gsb::fp(col), gsb::fp(op), records.data_ptr(),
                                     gsb::stream()),
                    "gsb_pack_records");
-        gsb::check(gsb_rasterize_forward_packed_ex(imgHeight, imgWidth, tilesX, tilesY, mRef,
-                                                   b.tileBins.data_ptr<int32_t>(), nullptr, nullptr, gsb::fp(bg),
-                                                   records.data_ptr(), gsb::fpw(outImg), gsb::fpw(finalTs),
-                                                   finalIdx.data_ptr<int32_t>(), flags, gsb::stream()),
-                   "gsb_rasterize_forward");
+        gsb::check(gsb_rasterize_forward_packed(imgHeight, imgWidth, tilesX, tilesY, mRef,
+                                                b.tileBins.data_ptr<int32_t>(), nullptr, nullptr, gsb::fp(bg),
+                                                records.data_ptr(), gsb::fpw(outImg), gsb::fpw(finalTs),
+                                                finalIdx.data_ptr<int32_t>(), flags, gsb::stream()),
+                   "gsb_rasterize_forward_packed");
         mRaster = mRef;
         ordered = false;
         break;
@@ -228,13 +227,13 @@ tensor_list rasterizeBackward(AutogradContext *ctx, tensor_list grad_outputs) {
     torch::Tensor v_colors = torch::empty({n, 3}, gsb::like(con, torch::kFloat32));
     torch::Tensor v_opacity = torch::empty({n, 1}, gsb::like(con, torch::kFloat32));
     // v_output_alpha is identically zero in the reference (rasterize_gaussians.cpp:108) -> NULL
-    gsb::check(gsb_rasterize_backward_ex(imgHeight, imgWidth, (imgWidth + BLOCK_X - 1) / BLOCK_X,
-                                         (imgHeight + BLOCK_Y - 1) / BLOCK_Y, n, m, tileBins.data_ptr<int32_t>(),
-                                         ordered ? tileOrder.data_ptr<int32_t>() : nullptr, gsb::fp(con), gsb::fp(op),
-                                         records.data_ptr(), cum.data_ptr<int32_t>(), gsb::fp(bg), gsb::fp(finalTs),
-                                         finalIdx.data_ptr<int32_t>(), gsb::fp(v_out), nullptr, rows.data_ptr(),
-                                         gsb::fpw(v_xy), gsb::fpw(v_conic), gsb::fpw(v_colors), gsb::fpw(v_opacity),
-                                         flags, gsb::stream()),
+    gsb::check(gsb_rasterize_backward(imgHeight, imgWidth, (imgWidth + BLOCK_X - 1) / BLOCK_X,
+                                      (imgHeight + BLOCK_Y - 1) / BLOCK_Y, n, m, tileBins.data_ptr<int32_t>(),
+                                      ordered ? tileOrder.data_ptr<int32_t>() : nullptr, gsb::fp(con), gsb::fp(op),
+                                      records.data_ptr(), cum.data_ptr<int32_t>(), gsb::fp(bg), gsb::fp(finalTs),
+                                      finalIdx.data_ptr<int32_t>(), gsb::fp(v_out), nullptr, rows.data_ptr(),
+                                      gsb::fpw(v_xy), gsb::fpw(v_conic), gsb::fpw(v_colors), gsb::fpw(v_opacity),
+                                      flags, gsb::stream()),
                "gsb_rasterize_backward");
     torch::Tensor none;
     return {v_xy, none, none, v_conic, none, v_colors, v_opacity, none, none, none};

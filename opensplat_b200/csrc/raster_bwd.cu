@@ -311,14 +311,13 @@ extern "C" size_t gsb_raster_grad_rows_bytes(int m) {
     return gsb_align_up((size_t)(m > 0 ? m : 0) * GSB_GRAD_ROW_FLOATS * 4 + 256, 256);
 }
 
-static int rasterize_backward_impl(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
-                                   const int32_t *tile_bins, const int32_t *tile_order, const float *conics,
-                                   const float *opacities, void *records,
-                                   const int32_t *cum_tiles_hit, const float *background,
-                                   const float *final_Ts, const int32_t *final_idx,
-                                   const float *v_output, const float *v_output_alpha,
-                                   void *grad_rows, float *v_xy, float *v_conic, float *v_colors,
-                                   float *v_opacity, unsigned flags, gsb_stream_t stream) {
+extern "C" int gsb_rasterize_backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
+                                      const int32_t *tile_bins, const int32_t *tile_order, const float *conics,
+                                      const float *opacities, void *records, const int32_t *cum_tiles_hit,
+                                      const float *background, const float *final_Ts, const int32_t *final_idx,
+                                      const float *v_output, const float *v_output_alpha, void *grad_rows,
+                                      float *v_xy, float *v_conic, float *v_colors, float *v_opacity, unsigned flags,
+                                      gsb_stream_t stream) {
     GSB_CHECK_ARG(img_h > 0 && img_w > 0 && n >= 0 && m >= 0);
     GSB_CHECK_ARG((flags & ~(unsigned)GSB_RASTER_CLAMP_MAX_ONE) == 0);
     const bool sat = (flags & GSB_RASTER_CLAMP_MAX_ONE) != 0;
@@ -348,46 +347,4 @@ static int rasterize_backward_impl(int img_h, int img_w, int tiles_x, int tiles_
         reinterpret_cast<float2 *>(v_xy), v_conic, v_colors, v_opacity);
     GSB_LAUNCH_CHECK();
     return 0;
-}
-
-extern "C" int gsb_rasterize_backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
-                                      const int32_t *tile_bins, const float *conics,
-                                      const float *opacities, void *records,
-                                      const int32_t *cum_tiles_hit, const float *background,
-                                      const float *final_Ts, const int32_t *final_idx,
-                                      const float *v_output, const float *v_output_alpha,
-                                      void *grad_rows, float *v_xy, float *v_conic, float *v_colors,
-                                      float *v_opacity, gsb_stream_t stream) {
-    return rasterize_backward_impl(img_h, img_w, tiles_x, tiles_y, n, m, tile_bins, nullptr, conics, opacities, records,
-                                   cum_tiles_hit, background, final_Ts, final_idx, v_output, v_output_alpha, grad_rows,
-                                   v_xy, v_conic, v_colors, v_opacity, 0u, stream);
-}
-
-// Same, with the tile order of gsb_bucket_tile_ranges (tiles handed to the persistent warps longest list first).
-extern "C" int gsb_rasterize_backward_ordered(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
-                                              const int32_t *tile_bins, const int32_t *tile_order,
-                                              const float *conics, const float *opacities, void *records,
-                                              const int32_t *cum_tiles_hit, const float *background,
-                                              const float *final_Ts, const int32_t *final_idx,
-                                              const float *v_output, const float *v_output_alpha,
-                                              void *grad_rows, float *v_xy, float *v_conic, float *v_colors,
-                                              float *v_opacity, gsb_stream_t stream) {
-    return rasterize_backward_impl(img_h, img_w, tiles_x, tiles_y, n, m, tile_bins, tile_order, conics, opacities,
-                                   records, cum_tiles_hit, background, final_Ts, final_idx, v_output, v_output_alpha,
-                                   grad_rows, v_xy, v_conic, v_colors, v_opacity, 0u, stream);
-}
-
-// gsb_rasterize_backward_ordered with `flags`: GSB_RASTER_CLAMP_MAX_ONE = final_idx carries the cut mask written by
-// gsb_rasterize_forward_packed_ex under the same flag and v_output is the gradient of the clamped image.
-extern "C" int gsb_rasterize_backward_ex(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
-                                         const int32_t *tile_bins, const int32_t *tile_order,
-                                         const float *conics, const float *opacities, void *records,
-                                         const int32_t *cum_tiles_hit, const float *background,
-                                         const float *final_Ts, const int32_t *final_idx,
-                                         const float *v_output, const float *v_output_alpha,
-                                         void *grad_rows, float *v_xy, float *v_conic, float *v_colors,
-                                         float *v_opacity, unsigned flags, gsb_stream_t stream) {
-    return rasterize_backward_impl(img_h, img_w, tiles_x, tiles_y, n, m, tile_bins, tile_order, conics, opacities,
-                                   records, cum_tiles_hit, background, final_Ts, final_idx, v_output, v_output_alpha,
-                                   grad_rows, v_xy, v_conic, v_colors, v_opacity, flags, stream);
 }

@@ -276,21 +276,33 @@ extern "C" int gsb_pack_records(int m, const int32_t *gaussian_ids_sorted, const
     return 0;
 }
 
-static int blend_forward(int img_h, int img_w, int tiles_x, int tiles_y, int m, const int32_t *tile_bins,
-                         const int32_t *tile_order, const int32_t *bin_stats, const float *background,
-                         void *records, float *out_img, float *final_Ts, int32_t *final_idx, unsigned flags,
-                         gsb_stream_t stream) {
+// Argument checks of the two blend entry points, then the persistent warps' tile counters (the 256 B of scratch
+// behind the records) are zeroed on `s` and returned in *counters.
+static int blend_setup(int img_h, int img_w, int tiles_x, int tiles_y, int m, const int32_t *tile_bins,
+                       const float *background, void *records, float *out_img, float *final_Ts, int32_t *final_idx,
+                       cudaStream_t s, unsigned **counters) {
     GSB_CHECK_ARG(img_h > 0 && img_w > 0 && m >= 0);
     GSB_CHECK_ARG(tiles_x == gsb_div_up(img_w, GSB_TILE) && tiles_y == gsb_div_up(img_h, GSB_TILE));
     GSB_CHECK_ARG(tile_bins && background && out_img && final_Ts && final_idx && records);
     GSB_CHECK_ARG(((uintptr_t)records % 16) == 0);
+    *counters = reinterpret_cast<unsigned *>(reinterpret_cast<char *>(records) + gsb_raster_records_bytes(m) - 256);
+    GSB_CUDA(cudaMemsetAsync(*counters, 0, 256, s));
+    return 0;
+}
+
+extern "C" int gsb_rasterize_forward_packed(int img_h, int img_w, int tiles_x, int tiles_y, int m,
+                                            const int32_t *tile_bins, const int32_t *tile_order,
+                                            const int32_t *bin_stats, const float *background, void *records,
+                                            float *out_img, float *final_Ts, int32_t *final_idx, unsigned flags,
+                                            gsb_stream_t stream) {
     GSB_CHECK_ARG((flags & ~(unsigned)GSB_RASTER_CLAMP_MAX_ONE) == 0);
     const bool sat = (flags & GSB_RASTER_CLAMP_MAX_ONE) != 0;
     GSB_CHECK_ARG(!sat || m < GSB_SAT_BIT0);
     cudaStream_t s = (cudaStream_t)stream;
-    unsigned *counters = reinterpret_cast<unsigned *>(
-        reinterpret_cast<char *>(records) + gsb_raster_records_bytes(m) - 256);
-    GSB_CUDA(cudaMemsetAsync(counters, 0, 256, s));
+    unsigned *counters = nullptr;
+    const int rc = blend_setup(img_h, img_w, tiles_x, tiles_y, m, tile_bins, background, records, out_img, final_Ts,
+                               final_idx, s, &counters);
+    if (rc) return rc;
     const int num_tiles = tiles_x * tiles_y;
 #define GSB_FWD_LAUNCH(S)                                                                                        \
     rasterize_forward_kernel<false, S><<<gsb_blend_grid((const void *)rasterize_forward_kernel<false, S>, num_tiles), \
@@ -304,40 +316,6 @@ static int blend_forward(int img_h, int img_w, int tiles_x, int tiles_y, int m, 
     return 0;
 }
 
-extern "C" int gsb_rasterize_forward(int img_h, int img_w, int tiles_x, int tiles_y, int m,
-                                     const int32_t *gaussian_ids_sorted, const int32_t *sorted_index,
-                                     const int32_t *tile_bins, const float *xys, const float *conics,
-                                     const float *colors, const float *opacities,
-                                     const float *background, void *records, float *out_img,
-                                     float *final_Ts, int32_t *final_idx, gsb_stream_t stream) {
-    GSB_CHECK_ARG(m >= 0 && records);
-    const int rc = gsb_pack_records(m, gaussian_ids_sorted, sorted_index, xys, conics, colors, opacities, records,
-                                    stream);
-    if (rc) return rc;
-    return blend_forward(img_h, img_w, tiles_x, tiles_y, m, tile_bins, nullptr, nullptr, background, records, out_img,
-                         final_Ts, final_idx, 0u, stream);
-}
-
-extern "C" int gsb_rasterize_forward_packed(int img_h, int img_w, int tiles_x, int tiles_y, int m,
-                                            const int32_t *tile_bins, const int32_t *tile_order,
-                                            const int32_t *bin_stats, const float *background, void *records,
-                                            float *out_img,
-                                            float *final_Ts, int32_t *final_idx, gsb_stream_t stream) {
-    return blend_forward(img_h, img_w, tiles_x, tiles_y, m, tile_bins, tile_order, bin_stats, background, records,
-                         out_img, final_Ts, final_idx, 0u, stream);
-}
-
-// gsb_rasterize_forward_packed with `flags` (GSB_RASTER_*): GSB_RASTER_CLAMP_MAX_ONE writes min(out, 1) and keeps
-// the per-channel cut mask in final_idx bits 28..30 (to be handed to gsb_rasterize_backward_ex with the same flag).
-extern "C" int gsb_rasterize_forward_packed_ex(int img_h, int img_w, int tiles_x, int tiles_y, int m,
-                                               const int32_t *tile_bins, const int32_t *tile_order,
-                                               const int32_t *bin_stats, const float *background, void *records,
-                                               float *out_img, float *final_Ts, int32_t *final_idx,
-                                               unsigned flags, gsb_stream_t stream) {
-    return blend_forward(img_h, img_w, tiles_x, tiles_y, m, tile_bins, tile_order, bin_stats, background, records,
-                         out_img, final_Ts, final_idx, flags, stream);
-}
-
 // Diagnostic twin of gsb_rasterize_forward_packed: same outputs, plus pair_counts (device uint64[4], accumulated --
 // zero it first) = {records passing the per-record test, slot visits (x 32 = pixel tests), pixel pairs evaluated
 // (sigma inside the extent), pixel pairs blended}.  Used by bench.py / the profiles for pairs-per-second figures;
@@ -346,13 +324,12 @@ extern "C" int gsb_rasterize_forward_count(int img_h, int img_w, int tiles_x, in
                                            const int32_t *tile_bins, const float *background, void *records,
                                            float *out_img, float *final_Ts, int32_t *final_idx,
                                            unsigned long long *pair_counts, gsb_stream_t stream) {
-    GSB_CHECK_ARG(img_h > 0 && img_w > 0 && m >= 0 && pair_counts);
-    GSB_CHECK_ARG(tiles_x == gsb_div_up(img_w, GSB_TILE) && tiles_y == gsb_div_up(img_h, GSB_TILE));
-    GSB_CHECK_ARG(tile_bins && background && out_img && final_Ts && final_idx && records);
+    GSB_CHECK_ARG(pair_counts);
     cudaStream_t s = (cudaStream_t)stream;
-    unsigned *counters = reinterpret_cast<unsigned *>(
-        reinterpret_cast<char *>(records) + gsb_raster_records_bytes(m) - 256);
-    GSB_CUDA(cudaMemsetAsync(counters, 0, 256, s));
+    unsigned *counters = nullptr;
+    const int rc = blend_setup(img_h, img_w, tiles_x, tiles_y, m, tile_bins, background, records, out_img, final_Ts,
+                               final_idx, s, &counters);
+    if (rc) return rc;
     const int num_tiles = tiles_x * tiles_y;
     const int grid = gsb_blend_grid((const void *)rasterize_forward_kernel<true, false>, num_tiles);
     rasterize_forward_kernel<true, false><<<grid, RK_THREADS, 0, s>>>(

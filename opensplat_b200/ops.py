@@ -286,7 +286,7 @@ def rasterize_forward_packed(tile_bounds_, img_size, m_capacity, tile_bins, reco
     fI = _empty((H, W), torch.int32, records)
     if tile_order is None:
         tile_order = getattr(tile_bins, "tile_order", None)
-    capi.check(capi.lib().gsb_rasterize_forward_packed_ex(
+    capi.check(capi.lib().gsb_rasterize_forward_packed(
         H, W, tile_bounds_[0], tile_bounds_[1], m_capacity, capi.ptr(tile_bins), capi.ptr(tile_order), capi.ptr(stats),
         capi.ptr(capi.f32(background)), capi.ptr(records), capi.ptr(out), capi.ptr(fT), capi.ptr(fI), int(flags),
         capi.stream()))
@@ -295,28 +295,17 @@ def rasterize_forward_packed(tile_bounds_, img_size, m_capacity, tile_bins, reco
 
 def rasterize_forward(tile_bounds_, img_size, gaussian_ids_sorted, sorted_index, tile_bins, xys, conics,
                       colors, opacities, background, flags=0):
-    W, H = img_size[0], img_size[1]
     m = gaussian_ids_sorted.shape[0]
     L = capi.lib()
     records = torch.empty(L.gsb_raster_records_bytes(m), dtype=torch.uint8, device=xys.device)
     if colors.shape[-1] != 3:
         raise ValueError("only 3-channel colors are supported")  # the N-D path is dead code in OpenSplat
-    if flags:
-        capi.check(L.gsb_pack_records(
-            m, capi.ptr(gaussian_ids_sorted), capi.ptr(sorted_index), capi.ptr(capi.f32(xys)),
-            capi.ptr(capi.f32(conics)), capi.ptr(capi.f32(colors)), capi.ptr(capi.f32(opacities)), capi.ptr(records),
-            capi.stream()))
-        return rasterize_forward_packed(tile_bounds_, img_size, m, tile_bins, records, background, None, None,
-                                        flags) + (records,)
-    out = _empty((H, W, 3), torch.float32, xys)
-    fT = _empty((H, W), torch.float32, xys)
-    fI = _empty((H, W), torch.int32, xys)
-    capi.check(L.gsb_rasterize_forward(
-        H, W, tile_bounds_[0], tile_bounds_[1], m, capi.ptr(gaussian_ids_sorted), capi.ptr(sorted_index),
-        capi.ptr(tile_bins), capi.ptr(capi.f32(xys)), capi.ptr(capi.f32(conics)), capi.ptr(capi.f32(colors)),
-        capi.ptr(capi.f32(opacities)), capi.ptr(capi.f32(background)), capi.ptr(records), capi.ptr(out),
-        capi.ptr(fT), capi.ptr(fI), capi.stream()))
-    return out, fT, fI, records
+    capi.check(L.gsb_pack_records(
+        m, capi.ptr(gaussian_ids_sorted), capi.ptr(sorted_index), capi.ptr(capi.f32(xys)),
+        capi.ptr(capi.f32(conics)), capi.ptr(capi.f32(colors)), capi.ptr(capi.f32(opacities)), capi.ptr(records),
+        capi.stream()))
+    return rasterize_forward_packed(tile_bounds_, img_size, m, tile_bins, records, background, None, None,
+                                    flags) + (records,)
 
 
 def rasterize_backward(img_height, img_width, n, m, tile_bins, conics, opacities, records, cum_tiles_hit,
@@ -330,7 +319,7 @@ def rasterize_backward(img_height, img_width, n, m, tile_bins, conics, opacities
     v_colors = _empty((n, 3), torch.float32, final_Ts)
     v_opacity = _empty((n, 1), torch.float32, final_Ts)
     v_output = capi.f32(v_output)
-    capi.check(L.gsb_rasterize_backward_ex(
+    capi.check(L.gsb_rasterize_backward(
         img_height, img_width, tb[0], tb[1], n, m, capi.ptr(tile_bins), capi.ptr(tile_order), capi.ptr(capi.f32(conics)),
         capi.ptr(capi.f32(opacities)), capi.ptr(records), capi.ptr(cum_tiles_hit),
         capi.ptr(capi.f32(background)), capi.ptr(final_Ts), capi.ptr(final_idx),

@@ -14,15 +14,13 @@ import os
 
 import torch
 
-from . import capi
+from . import capi, ops
 from .ops import tile_bounds, num_sh_bases, BinPlan
 from .parallel import flat_layout
 
 
 class SplatPipeline:
-    def __init__(self, n, W, H, sh_degree=3, device="cuda:0", m_capacity=None, stage_timing=False,
-                 binning="bucket"):
-        self.binning = binning  # "bucket" (two-level, fused pack) or "radix" (generic global sort)
+    def __init__(self, n, W, H, sh_degree=3, device="cuda:0", m_capacity=None, stage_timing=False):
         self.n, self.W, self.H, self.deg = int(n), int(W), int(H), int(sh_degree)
         self.K = num_sh_bases(sh_degree)
         self.dev = torch.device(device)
@@ -41,10 +39,8 @@ class SplatPipeline:
         self.loss = torch.zeros(1, dtype=f32, device=d)
         self.tile_bins = torch.empty((self.T, 2), dtype=i32, device=d)
         self.tile_order = torch.empty((self.T,), dtype=i32, device=d)   # longest-first tile order (fast path)
-        self.use_tile_order = os.environ.get("GSB_TILE_ORDER", "1") != "0"
         self.stats_dev = torch.zeros(4, dtype=i32, device=d)
         self.plan = BinPlan()   # capacities of the M-dependent buffers, carried from frame to frame
-        self.cull = True        # bin only (Gaussian, tile) pairs whose extent box touches the tile
         # ---- camera ----
         self.viewmat = torch.eye(4, dtype=f32, device=d)
         self.projmat = torch.eye(4, dtype=f32, device=d)
@@ -96,11 +92,8 @@ class SplatPipeline:
         self.v_xy = torch.empty((n, 2), dtype=f32, device=d)
         self.v_conic = torch.empty((n, 3), dtype=f32, device=d)
         self.v_rgbs = torch.empty((n, 3), dtype=f32, device=d)
-        self.scan_ws = torch.empty(self.L.gsb_cumsum_workspace_bytes(n), dtype=torch.uint8, device=d)
-        self.total_dev = torch.zeros(2, dtype=i32, device=d)
         self.max_len = 0
         self.m_cap = -1   # the M-sized buffers (and the n-sized bucket workspace) are (re)built by the next forward
-        self._generic_cap = 0
 
     def _alloc_grad_flat(self, numel):
         """The flat gradient buffer; multigpu.ViewParallelExchange re-binds it to symmetric (peer-mapped) memory."""
@@ -122,18 +115,6 @@ class SplatPipeline:
         self.bucket_ws = torch.empty(self.L.gsb_bucket_workspace_bytes(self.n, m_cap, self.T) + 256,
                                      dtype=torch.uint8, device=d)
         self.m_cap = m_cap
-
-    def _grow_generic(self, m):
-        """Buffers of the generic (global radix sort) path, allocated only when it is taken."""
-        cap = int(m * 1.25) + 1024
-        d = self.dev
-        self.isect = torch.empty(cap, dtype=torch.int64, device=d)
-        self.gids = torch.empty(cap, dtype=torch.int32, device=d)
-        self.isect_sorted = torch.empty(cap, dtype=torch.int64, device=d)
-        self.sorted_index = torch.empty(cap, dtype=torch.int32, device=d)
-        self.gids_sorted = torch.empty(cap, dtype=torch.int32, device=d)
-        self.sort_ws = torch.empty(self.L.gsb_sort_workspace_bytes(cap) + 256, dtype=torch.uint8, device=d)
-        self._generic_cap = cap
 
     def load_scene(self, sc):
         """sc: dict from opensplat_b200.scene.make_scene (numpy)."""
@@ -188,72 +169,60 @@ class SplatPipeline:
                                          P(self.projmat), fx, fy, cx, cy, H, W, self.tb[0], self.tb[1], 0.01,
                                          P(self.cov3d), P(self.xys), P(self.depths), P(self.radii), P(self.conics),
                                          P(self.nth), s))
-        if self.binning == "bucket":
-            limit = L.gsb_bucket_max_tile_len()
-            plan = self.plan
-            cull = 1 if self.cull else 0
-            # Everything below is sized by capacities planned from earlier frames and enqueued WITHOUT waiting for
-            # the path's one device->host read-back (M, rasterize_gaussians.cpp:63): the host looks at it after
-            # the blend kernel has been enqueued (the GPU never idles) and redoes a frame that outgrew the plan.
-            while True:
-                if plan.m_cap != self.m_cap:
-                    self._grow(plan.m_cap)
-                m_cap, len_cap = plan.m_cap, plan.len_cap
-                boff = (-self.bucket_ws.data_ptr()) % 256
-                wsp, wsb = self.bucket_ws.data_ptr() + boff, self.bucket_ws.numel() - boff
-                self._stage("scan")
-                capi.check(L.gsb_bucket_tile_ranges(n, P(self.xys), P(self.radii), P(self.conics), P(self.rgbs),
-                                                    P(p["opacities"]), cull, self.tb[0], self.tb[1], m_cap, len_cap,
-                                                    wsp, wsb, P(self.cum), P(self.tile_bins),
-                                                    P(self.tile_order) if self.use_tile_order else None,
-                                                    P(self.stats_dev), s))
-                plan.read_back(self.stats_dev)
-                if m_cap > 0:
-                    self._stage("bucket_sort_pack")
-                    capi.check(L.gsb_bucket_sort_pack(n, m_cap, len_cap, P(self.depths), P(self.radii), P(self.cum),
-                                                      cull, self.tb[0], self.tb[1], P(self.tile_bins),
-                                                      P(self.stats_dev), wsp, wsb, P(self.records), None, None, s))
-                self._stage("raster_fwd")
-                capi.check(L.gsb_rasterize_forward_packed(H, W, self.tb[0], self.tb[1], m_cap, P(self.tile_bins),
-                                                          P(self.tile_order) if self.use_tile_order else None,
-                                                          P(self.stats_dev), P(self.background), P(self.records),
-                                                          P(self.out_img), P(self.final_Ts), P(self.final_idx), s))
-                self._stage("end_fwd")
-                self.m, self.max_len, overflow = plan.wait()
-                if not overflow:
-                    self.m_raster = m_cap
-                    self._ordered = self.use_tile_order
-                    return self.out_img
-                self._ev = []            # the frame is redone: drop its stage events
-                if self.max_len > limit:
-                    break                # pathological tile lists: generic path below
-                plan.grow(self.m, self.max_len)
-        # ---- generic path: reference-exact global sort (binAndSortGaussians), with the M read-back in the middle
-        self._stage("scan")
-        capi.check(L.gsb_cumsum_tiles_hit(n, P(self.nth), P(self.cum), P(self.scan_ws), self.scan_ws.numel(),
-                                          P(self.total_dev), s))
-        m = self.m = int(self.total_dev[0])
-        if m > self._generic_cap:
-            self._grow_generic(m)
-        if self.m_cap < 0 or self.L.gsb_raster_records_bytes(m) > self.records.numel():
+        limit = L.gsb_bucket_max_tile_len()
+        plan = self.plan
+        # Everything below is sized by capacities planned from earlier frames and enqueued WITHOUT waiting for the
+        # path's one device->host read-back (M, rasterize_gaussians.cpp:63): the host looks at it after the blend
+        # kernel has been enqueued (the GPU never idles) and redoes a frame that outgrew the plan.
+        while True:
+            if plan.m_cap != self.m_cap:
+                self._grow(plan.m_cap)
+            m_cap, len_cap = plan.m_cap, plan.len_cap
+            boff = (-self.bucket_ws.data_ptr()) % 256
+            wsp, wsb = self.bucket_ws.data_ptr() + boff, self.bucket_ws.numel() - boff
+            self._stage("scan")
+            # cull = 1: bin only (Gaussian, tile) pairs whose extent box touches the tile
+            capi.check(L.gsb_bucket_tile_ranges(n, P(self.xys), P(self.radii), P(self.conics), P(self.rgbs),
+                                                P(p["opacities"]), 1, self.tb[0], self.tb[1], m_cap, len_cap, wsp, wsb,
+                                                P(self.cum), P(self.tile_bins), P(self.tile_order), P(self.stats_dev),
+                                                s))
+            plan.read_back(self.stats_dev)
+            if m_cap > 0:
+                self._stage("bucket_sort_pack")
+                capi.check(L.gsb_bucket_sort_pack(n, m_cap, len_cap, P(self.depths), P(self.radii), P(self.cum), 1,
+                                                  self.tb[0], self.tb[1], P(self.tile_bins), P(self.stats_dev), wsp,
+                                                  wsb, P(self.records), None, None, s))
+            self._stage("raster_fwd")
+            capi.check(L.gsb_rasterize_forward_packed(H, W, self.tb[0], self.tb[1], m_cap, P(self.tile_bins),
+                                                      P(self.tile_order), P(self.stats_dev), P(self.background),
+                                                      P(self.records), P(self.out_img), P(self.final_Ts),
+                                                      P(self.final_idx), 0, s))
+            self._stage("end_fwd")
+            self.m, self.max_len, overflow = plan.wait()
+            if not overflow:
+                self.m_raster = m_cap
+                self._ordered = True
+                return self.out_img
+            self._ev = []            # the frame is redone: drop its stage events
+            if self.max_len > limit:
+                break                # pathological tile lists: generic path below
+            plan.grow(self.m, self.max_len)
+        # ---- generic path: reference-exact global sort (binAndSortGaussians) of the unculled lists, with the M
+        # read-back in the middle
+        self._stage("generic_bin")
+        self.cum = ops.cumsum_tiles_hit(self.nth)
+        m = self.m = int(self.cum[-1])
+        if L.gsb_raster_records_bytes(m) > self.records.numel():
             self._grow(int(m * 1.25) + 1024)
             self.plan.m_cap = self.m_cap
-        self._stage("emit")
-        capi.check(L.gsb_map_gaussian_to_intersects(n, m, P(self.xys), P(self.depths), P(self.radii),
-                                                    P(self.cum), self.tb[0], self.tb[1], P(self.isect),
-                                                    P(self.gids), s))
-        self._stage("sort")
-        off = (-self.sort_ws.data_ptr()) % 256
-        capi.check(L.gsb_sort_intersects(m, self.T, P(self.isect), P(self.isect_sorted), P(self.sorted_index),
-                                         self.sort_ws.data_ptr() + off, self.sort_ws.numel() - off, s))
-        self._stage("bins")
-        capi.check(L.gsb_gather_bin_edges(m, self.T, P(self.isect_sorted), P(self.sorted_index), P(self.gids),
-                                          P(self.gids_sorted), P(self.tile_bins), s))
+        _, _, _, gids_sorted, self.tile_bins, sorted_index = ops.binAndSortGaussians(
+            n, m, self.xys, self.depths, self.radii, self.cum, self.tb, return_index=True)
         self._stage("raster_fwd")
-        capi.check(L.gsb_rasterize_forward(H, W, self.tb[0], self.tb[1], m, P(self.gids_sorted),
-                                           P(self.sorted_index), P(self.tile_bins), P(self.xys), P(self.conics),
-                                           P(self.rgbs), P(p["opacities"]), P(self.background), P(self.records),
-                                           P(self.out_img), P(self.final_Ts), P(self.final_idx), s))
+        capi.check(L.gsb_pack_records(m, P(gids_sorted), P(sorted_index), P(self.xys), P(self.conics), P(self.rgbs),
+                                      P(p["opacities"]), P(self.records), s))
+        capi.check(L.gsb_rasterize_forward_packed(H, W, self.tb[0], self.tb[1], m, P(self.tile_bins), None, None,
+                                                  P(self.background), P(self.records), P(self.out_img),
+                                                  P(self.final_Ts), P(self.final_idx), 0, s))
         self.m_raster = m
         self._ordered = False
         self._stage("end_fwd")
@@ -270,12 +239,12 @@ class SplatPipeline:
         capi.check(L.gsb_mse_loss_grad(cnt, P(self.out_img), P(self.target), P(self.v_img), P(self.loss), 1.0 / cnt, s))
         v_rgbs = self.exchange.v_rgbs_buffer() if self.exchange is not None else self.v_rgbs
         self._stage("raster_bwd")
-        capi.check(L.gsb_rasterize_backward_ordered(H, W, self.tb[0], self.tb[1], n, m, P(self.tile_bins),
-                                            P(self.tile_order) if self._ordered else None, P(self.conics),
-                                            P(p["opacities"]), P(self.records), P(self.cum), P(self.background),
-                                            P(self.final_Ts), P(self.final_idx),
-                                            P(self.v_img), None, P(self.grad_rows), P(self.v_xy), P(self.v_conic),
-                                            P(v_rgbs), P(g["opacities"]), s))
+        capi.check(L.gsb_rasterize_backward(H, W, self.tb[0], self.tb[1], n, m, P(self.tile_bins),
+                                    P(self.tile_order) if self._ordered else None, P(self.conics),
+                                    P(p["opacities"]), P(self.records), P(self.cum), P(self.background),
+                                    P(self.final_Ts), P(self.final_idx),
+                                    P(self.v_img), None, P(self.grad_rows), P(self.v_xy), P(self.v_conic),
+                                    P(v_rgbs), P(g["opacities"]), 0, s))
         if self.exchange is not None and self.exchange.overlap:
             self.exchange.start_colour(average=True)   # colour pulls + SH expansion start now, on a side stream
         self._stage("project_bwd")

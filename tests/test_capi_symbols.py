@@ -93,13 +93,13 @@ def _ctype_of(decl):
             "unsigned": C.c_uint, "unsigned int": C.c_uint, "gsb_stream_t": C.c_void_p}[base]
 
 
-def test_ctypes_signatures_match_the_header_prototypes():
+def test_ctypes_bindings_match_every_header_prototype():
     """Every binding in capi._SIGS has the arity and the scalar/pointer classes of its prototype in
     include/gsplat_b200.h (an int bound as a float, or a dropped argument, would otherwise only show as garbage on
     the GPU box)."""
     import ctypes as C
     protos = _prototypes()
-    assert len(protos) >= 50, len(protos)
+    assert len(protos) >= 45 and sorted(protos) == _declared(), len(protos)   # every declared name parsed
     sigs = dict(capi._SIGS)
     sigs.update(capi._OPT_SIGS)
     checked = 0

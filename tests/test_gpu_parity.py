@@ -268,7 +268,7 @@ def test_tile_order_is_a_longest_first_permutation_and_changes_nothing():
         assert torch.equal(x, y)
 
 
-def test_binning_capacity_overflow_is_flagged_and_harmless():
+def test_capacity_overflow_is_flagged_and_leaves_pack_and_blend_untouched():
     """Capacities smaller than the frame needs: stats[2] = 1 and neither the sort/pack nor the blend kernel touch
     their outputs; the operator redoes the frame with larger capacities and gives the same image."""
     n, W, H = 20000, 320, 200
@@ -294,7 +294,7 @@ def test_binning_capacity_overflow_is_flagged_and_harmless():
         fT, fI = torch.empty((H, W), device=DEV), torch.empty((H, W), dtype=torch.int32, device=DEV)
         capi.check(capi.lib().gsb_rasterize_forward_packed(H, W, tb[0], tb[1], m_cap, capi.ptr(b2), None, capi.ptr(st2),
                                                            capi.ptr(bg), capi.ptr(rec2), capi.ptr(out), capi.ptr(fT),
-                                                           capi.ptr(fI), capi.stream()))
+                                                           capi.ptr(fI), 0, capi.stream()))
         assert bool((out == -7.0).all())
     # operator level: plans start too small (fresh plan), the result must not depend on it
     ops._plans.clear()
@@ -602,8 +602,10 @@ def test_one_gaussian_covering_every_tile():
 @pytest.mark.parametrize("n,expect_path", [(7000, "radix"), (24000, "generic")])
 def test_very_long_tile_lists_take_radix_and_generic_paths(n, expect_path):
     """All Gaussians piled on one spot: a tile list longer than the bitonic (4096) / in-smem (16384) limits.
-    The operator must still match the oracle (CTA radix sort, resp. the generic global radix sort fallback)."""
+    The operator must still match the oracle (CTA radix sort, resp. the generic global radix sort fallback), and
+    SplatPipeline, which takes the same path, must match the operator chain bit for bit."""
     from opensplat_b200 import capi
+    from opensplat_b200.pipeline import SplatPipeline
     W, H = 64, 48
     sc = _scene(n, W, H, 0.5, opacity=(0.0045, 0.01), seed=n)
     # pile up around the centre of tile (2,1) (pixel 39.5, 23.5): every Gaussian lies inside that one tile, with a
@@ -633,6 +635,22 @@ def test_very_long_tile_lists_take_radix_and_generic_paths(n, expect_path):
     r = orc.rasterize_backward(H, W, b["gaussian_ids_sorted"], b["tile_bins"], o["xys"], o["conics"], colors,
                                sc["opacities"], [0.1, 0.2, 0.3], f["final_Ts"], f["final_idx"], wgt, exp_mode=1)
     assert rel_l2(npy(colt.grad), r["v_colors"]) <= 1e-3 and rel_l2(npy(opt.grad), r["v_opacity"]) <= 1e-3
+    # the same scene through SplatPipeline and through SphericalHarmonics -> ProjectGaussians -> RasterizeGaussians:
+    # same inputs, same kernels, so the image and the gradients are bit-identical
+    pipe = SplatPipeline(n, W, H, sh_degree=0)
+    pipe.load_scene(sc)
+    pipe.forward()
+    pipe.backward()
+    assert pipe._ordered == (expect_path == "radix")   # the generic fallback blends without the tile order
+    coeffs, opac = cu(sc["coeffs"]).requires_grad_(), cu(sc["opacities"]).requires_grad_()
+    rgbs = torch.clamp_min(ops.SphericalHarmonics.apply(0, cu(sc["viewdirs"]), coeffs) + 0.5, 0.0)
+    xys, depths, radii, conics, nth, _ = ops.ProjectGaussians.apply(
+        cu(sc["means"]), cu(sc["scales"]), 1.0, cu(sc["quats"]), cu(sc["viewmat"]), cu(sc["projmat"]), sc["fx"],
+        sc["fy"], sc["cx"], sc["cy"], H, W, tb)
+    img = ops.RasterizeGaussians.apply(xys, depths, radii, conics, nth, rgbs, opac, H, W, torch.zeros(3, device=DEV))
+    assert torch.equal(pipe.out_img, img)
+    img.backward(pipe.v_img)
+    assert torch.equal(opac.grad, pipe.g["opacities"]) and torch.equal(coeffs.grad, pipe.g["coeffs"])
 
 
 def test_long_tile_lists_at_realistic_tile_counts():

@@ -24,5 +24,5 @@ for _ in range(reps):
     pipe.forward_backward()
 e1.record()
 st = pipe.resolve_stage_times()
-print(os.environ.get("GSB_LIB", "default"), "tile_order=" + os.environ.get("GSB_TILE_ORDER", "1"), wl, f"step {e0.elapsed_time(e1)/reps:.4f} ms  M={pipe.m}",
+print(os.environ.get("GSB_LIB", "default"), wl, f"step {e0.elapsed_time(e1)/reps:.4f} ms  M={pipe.m}",
       " ".join(f"{k}={v:.4f}" for k, v in st.items()))
