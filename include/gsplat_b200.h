@@ -149,7 +149,8 @@ int gsb_project_backward_activated(int n, const float *means3d, const float *log
 /* ---- Tile binning ----------------------------------------------------------------------------
  * gsb_cumsum_tiles_hit replaces torch::cumsum(numTilesHit, 0, kInt32) (rasterize_gaussians.cpp:62).
  *   Inclusive scan; the caller reads M = cum_tiles_hit[n-1] back (rasterize_gaussians.cpp:63).
- *   If total_out != NULL the total is also written there (device or mapped-pinned int32).
+ *   In place when cum_tiles_hit == num_tiles_hit.  The workspace (gsb_cumsum_workspace_bytes(n)
+ *   bytes) must be 256-byte aligned; it is zeroed by the call.
  * gsb_map_gaussian_to_intersects replaces map_gaussian_to_intersects_tensor (bindings.h:95-103,
  *   bindings.cu:279-318, kernel forward.cu:107-143): isect_ids [m] i64 = (tile_id << 32) | depth bits,
  *   gaussian_ids [m] i32.
@@ -162,7 +163,7 @@ int gsb_project_backward_activated(int n, const float *means3d, const float *log
  *   y = last+1; empty tiles (0,0)), fully written. */
 size_t gsb_cumsum_workspace_bytes(int n);
 int gsb_cumsum_tiles_hit(int n, const int32_t *num_tiles_hit, int32_t *cum_tiles_hit, void *workspace,
-                         size_t workspace_bytes, int32_t *total_out, gsb_stream_t stream);
+                         size_t workspace_bytes, gsb_stream_t stream);
 int gsb_map_gaussian_to_intersects(int n, int m, const float *xys, const float *depths,
                                    const int32_t *radii, const int32_t *cum_tiles_hit, int tiles_x,
                                    int tiles_y, int64_t *isect_ids, int32_t *gaussian_ids,

@@ -41,21 +41,18 @@ def needs_build():
     return any(os.path.getmtime(p) > t for p in _deps() if os.path.exists(p))
 
 
-def build(force=False, verbose=False, defines=None, out=None):
-    """defines: extra -D flags (kernel variants for A/B runs); out: alternative output path."""
-    global LIB
-    variant = bool(defines or out)
-    if not variant and not force and not needs_build():
+def build(force=False, verbose=False):
+    if not force and not needs_build():
         return LIB
     os.makedirs(OUT_DIR, exist_ok=True)
-    obj_dir = os.path.join(HERE, "build") if not variant else os.path.join(HERE, "build", "v_" + os.path.basename(out or "x"))
+    obj_dir = os.path.join(HERE, "build")
     os.makedirs(obj_dir, exist_ok=True)
     srcs = {k: v for k, v in SOURCES.items() if os.path.exists(os.path.join(CSRC, k))}
 
     def compile_one(item):
         name, extra = item
         obj = os.path.join(obj_dir, name.replace(".cu", ".o"))
-        cmd = [NVCC] + ARCH + COMMON + extra + [f"-D{d}" for d in (defines or [])] + ["-c", os.path.join(CSRC, name), "-o", obj]
+        cmd = [NVCC] + ARCH + COMMON + extra + ["-c", os.path.join(CSRC, name), "-o", obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed for {name}:\n{r.stdout}\n{r.stderr}")
@@ -67,12 +64,11 @@ def build(force=False, verbose=False, defines=None, out=None):
 
     with ThreadPoolExecutor(max_workers=8) as ex:
         objs = list(ex.map(compile_one, srcs.items()))
-    target = out or LIB
-    cmd = [NVCC] + ARCH + ["-shared", "-o", target] + objs + ["-lcudart"]
+    cmd = [NVCC] + ARCH + ["-shared", "-o", LIB] + objs + ["-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
-    return target
+    return LIB
 
 
 if __name__ == "__main__":

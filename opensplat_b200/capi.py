@@ -9,7 +9,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# GSB_LIB overrides the library path (tools/bench_blend.py uses it to A/B kernel variants)
+# GSB_LIB overrides the library path (tools/bench_blend.py uses it to compare the builds of two commits)
 LIB_PATH = os.environ.get("GSB_LIB") or os.path.join(_HERE, "lib", "libgsplat_b200.so")
 _lib = None
 
@@ -39,7 +39,7 @@ _SIGS = {
     "gsb_project_backward_activated": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
                                             _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_cumsum_workspace_bytes": (_sz, [_i]),
-    "gsb_cumsum_tiles_hit": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "gsb_cumsum_tiles_hit": (_i, [_i, _vp, _vp, _vp, _sz, _vp]),
     "gsb_map_gaussian_to_intersects": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "gsb_sort_workspace_bytes": (_sz, [_i]),
     "gsb_sort_intersects": (_i, [_i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),

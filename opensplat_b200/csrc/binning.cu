@@ -1,9 +1,13 @@
-// binning.cu -- tile binning: scan (B1), intersection emit (B2), 64-bit key radix sort (B3),
+// binning.cu -- generic tile binning: scan (B1), intersection emit (B2), 64-bit key radix sort (B3),
 // gather + tile bin edges (B4).  SURVEY.md section 8a.
 //
 // Replaces, in the reference: torch::cumsum (rasterize_gaussians.cpp:62), map_gaussian_to_intersects
 // (forward.cu:107-143), torch::sort + torch::gather (rasterize_gaussians.cpp:25-32; CUB inside
 // libtorch) and get_tile_bin_edges (forward.cu:148-169).
+//
+// B1 is the fast path's single-pass chained scan (bucket.cu, K1b, launched through gsb_count_scan), so
+// both paths produce cum_tiles_hit with the same kernel.  Both also take each Gaussian's tile box from
+// gsb_tile_bbox (gsb_common.cuh), the function the projection computes num_tiles_hit with.
 //
 // The sort is a hand-written single-pass-per-digit LSD radix sort ("onesweep" organisation: one
 // up-front histogram of every digit, then per digit ONE kernel that ranks a tile of keys, publishes
@@ -15,113 +19,10 @@
 // (24 B x M) stays inside the 50 MB L2 up to M ~ 2M.
 #include "gsb_common.cuh"
 
+int gsb_count_scan_blocks(int n);
+void gsb_count_scan(int n, int *counts_then_cum, unsigned *ticket, unsigned long long *state, cudaStream_t s);
+
 namespace {
-
-// ------------------------------------------------------------------------------------------------
-// B1: inclusive scan of num_tiles_hit (int32)
-// ------------------------------------------------------------------------------------------------
-constexpr int SCAN_THREADS = 256;
-constexpr int SCAN_IPT = 8;
-constexpr int SCAN_TILE = SCAN_THREADS * SCAN_IPT;
-
-__device__ __forceinline__ int warp_incl_scan(int v) {
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        int t = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += t;
-    }
-    return v;
-}
-
-// block-wide exclusive scan of one value per thread; returns exclusive prefix, total in *total
-template <int THREADS>
-__device__ __forceinline__ int block_excl_scan(int v, int *total, int *smem /* >= THREADS/32 + 1 */) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    int inc = warp_incl_scan(v);
-    if (lane == 31) smem[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-        int x = (lane < THREADS / 32) ? smem[lane] : 0;
-        int xi = warp_incl_scan(x);
-        if (lane < THREADS / 32) smem[lane] = xi - x;
-        if (lane == 31) smem[THREADS / 32] = xi;
-    }
-    __syncthreads();
-    int res = smem[w] + inc - v;
-    *total = smem[THREADS / 32];
-    __syncthreads();
-    return res;
-}
-
-__device__ __forceinline__ void load_tile8(const int *__restrict__ in, int base, int n, int v[SCAN_IPT]) {
-    const int e0 = base + threadIdx.x * SCAN_IPT;
-    if (e0 + SCAN_IPT <= n && ((reinterpret_cast<uintptr_t>(in + e0) & 15) == 0)) {
-        int4 a = *reinterpret_cast<const int4 *>(in + e0);
-        int4 b = *reinterpret_cast<const int4 *>(in + e0 + 4);
-        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-    } else {
-#pragma unroll
-        for (int k = 0; k < SCAN_IPT; ++k) v[k] = (e0 + k < n) ? in[e0 + k] : 0;
-    }
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS)
-scan_block_sums_kernel(int n, const int *__restrict__ in, int *__restrict__ block_sums) {
-    __shared__ int sm[SCAN_THREADS / 32 + 1];
-    int v[SCAN_IPT];
-    load_tile8(in, blockIdx.x * SCAN_TILE, n, v);
-    int s = 0;
-#pragma unroll
-    for (int k = 0; k < SCAN_IPT; ++k) s += v[k];
-    int total;
-    block_excl_scan<SCAN_THREADS>(s, &total, sm);
-    if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
-}
-
-// single block: exclusive scan of block_sums in place; writes grand total
-__global__ void __launch_bounds__(1024)
-scan_block_offsets_kernel(int nb, int *__restrict__ block_sums, int *__restrict__ total_out) {
-    __shared__ int sm[1024 / 32 + 1];
-    int carry = 0;
-    for (int base = 0; base < nb; base += 1024) {
-        int i = base + threadIdx.x;
-        int v = (i < nb) ? block_sums[i] : 0;
-        int total;
-        int ex = block_excl_scan<1024>(v, &total, sm);
-        if (i < nb) block_sums[i] = carry + ex;
-        carry += total;
-    }
-    if (threadIdx.x == 0 && total_out) *total_out = carry;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS)
-scan_apply_kernel(int n, const int *__restrict__ in, const int *__restrict__ block_offsets,
-                  int *__restrict__ out) {
-    __shared__ int sm[SCAN_THREADS / 32 + 1];
-    int v[SCAN_IPT];
-    const int base = blockIdx.x * SCAN_TILE;
-    load_tile8(in, base, n, v);
-    int s = 0;
-#pragma unroll
-    for (int k = 0; k < SCAN_IPT; ++k) s += v[k];
-    int total;
-    int run = block_excl_scan<SCAN_THREADS>(s, &total, sm) + block_offsets[blockIdx.x];
-    const int e0 = base + threadIdx.x * SCAN_IPT;
-#pragma unroll
-    for (int k = 0; k < SCAN_IPT; ++k) {
-        run += v[k];
-        v[k] = run;
-    }
-    if (e0 + SCAN_IPT <= n && ((reinterpret_cast<uintptr_t>(out + e0) & 15) == 0)) {
-        *reinterpret_cast<int4 *>(out + e0) = make_int4(v[0], v[1], v[2], v[3]);
-        *reinterpret_cast<int4 *>(out + e0 + 4) = make_int4(v[4], v[5], v[6], v[7]);
-    } else {
-#pragma unroll
-        for (int k = 0; k < SCAN_IPT; ++k)
-            if (e0 + k < n) out[e0 + k] = v[k];
-    }
-}
 
 // ------------------------------------------------------------------------------------------------
 // B2: emit (tile|depth) keys
@@ -135,12 +36,8 @@ map_intersects_kernel(int n, const float2 *__restrict__ xys, const float *__rest
     const int r = radii[i];
     if (r <= 0) return;
     const float2 c = xys[i];
-    // get_tile_bbox (helpers.cuh:17-49) -- same arithmetic as project.cu
-    const float tcx = c.x / 16.f, tcy = c.y / 16.f, tr = (float)r / 16.f;
-    const int x0 = min(max(0, (int)(tcx - tr)), tiles_x);
-    const int x1 = min(max(0, (int)(tcx + tr + 1.f)), tiles_x);
-    const int y0 = min(max(0, (int)(tcy - tr)), tiles_y);
-    const int y1 = min(max(0, (int)(tcy + tr + 1.f)), tiles_y);
+    int x0, x1, y0, y1;
+    gsb_tile_bbox(c.x, c.y, (float)r, tiles_x, tiles_y, x0, x1, y0, y1);
     int cur = (i == 0) ? 0 : cum_tiles_hit[i - 1];
     const long long depth_id = (long long)__float_as_int(depths[i]);  // forward.cu:132
     for (int ty = y0; ty < y1; ++ty)
@@ -332,29 +229,29 @@ gather_bin_edges_kernel(int m, const long long *__restrict__ keys_sorted,
 }  // namespace
 
 // =================================================================================================
+// workspace: the block ticket (256 B), then the look-back state word of every block of the chained scan
 extern "C" size_t gsb_cumsum_workspace_bytes(int n) {
-    return gsb_align_up((size_t)(gsb_div_up(n > 0 ? n : 1, SCAN_TILE) + 1) * 4, 256);
+    return 256 + gsb_align_up((size_t)gsb_count_scan_blocks(n) * 8, 256);
 }
 
 extern "C" int gsb_cumsum_tiles_hit(int n, const int32_t *num_tiles_hit, int32_t *cum_tiles_hit,
-                                    void *workspace, size_t workspace_bytes, int32_t *total_out,
-                                    gsb_stream_t stream) {
+                                    void *workspace, size_t workspace_bytes, gsb_stream_t stream) {
     GSB_CHECK_ARG(n >= 0);
-    cudaStream_t s = (cudaStream_t)stream;
-    if (n == 0) {
-        if (total_out) GSB_CUDA(cudaMemsetAsync(total_out, 0, 4, s));
-        return 0;
-    }
+    if (n == 0) return 0;
     GSB_CHECK_ARG(num_tiles_hit && cum_tiles_hit && workspace);
-    if (workspace_bytes < gsb_cumsum_workspace_bytes(n)) {
+    GSB_CHECK_ARG(((uintptr_t)workspace % 256) == 0);
+    const size_t ws_bytes = gsb_cumsum_workspace_bytes(n);
+    if (workspace_bytes < ws_bytes) {
         gsb_set_error(GSB_ERR_WORKSPACE, "cumsum workspace too small", __FILE__, __LINE__);
         return GSB_ERR_WORKSPACE;
     }
-    const int nb = gsb_div_up(n, SCAN_TILE);
-    int *bs = (int *)workspace;
-    scan_block_sums_kernel<<<nb, SCAN_THREADS, 0, s>>>(n, num_tiles_hit, bs);
-    scan_block_offsets_kernel<<<1, 1024, 0, s>>>(nb, bs, total_out);
-    scan_apply_kernel<<<nb, SCAN_THREADS, 0, s>>>(n, num_tiles_hit, bs, cum_tiles_hit);
+    cudaStream_t s = (cudaStream_t)stream;
+    char *ws = (char *)workspace;
+    GSB_CUDA(cudaMemsetAsync(ws, 0, ws_bytes, s));
+    if (cum_tiles_hit != num_tiles_hit)
+        GSB_CUDA(cudaMemcpyAsync(cum_tiles_hit, num_tiles_hit, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToDevice,
+                                 s));
+    gsb_count_scan(n, cum_tiles_hit, (unsigned *)ws, (unsigned long long *)(ws + 256), s);
     GSB_LAUNCH_CHECK();
     return 0;
 }

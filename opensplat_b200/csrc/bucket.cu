@@ -7,7 +7,8 @@
 // host read-back in the middle:
 //   K1 bin_count      : per Gaussian, build its 48-B attribute record once and count the tiles it is binned to (one
 //                       atomic per tile -> tile sizes); K1b count_scan: single-pass chained scan (decoupled look-back)
-//                       of the per-Gaussian counts -> cum_tiles_hit (the gradient-row slots)
+//                       of the per-Gaussian counts -> cum_tiles_hit (the gradient-row slots).  The generic path's
+//                       gsb_cumsum_tiles_hit (binning.cu) is this same scan, launched through gsb_count_scan.
 //   K2 tile_scan      : exclusive scan over the T tiles (chained scan over <= 32 CTAs) -> tile_bins (first, last+1),
 //                       write cursors, stats = {M, longest list, overflow flag}
 //   K3 bucket_emit    : per Gaussian, write (depth bits << 32 | k) into its tiles' segments (atomic cursor;
@@ -53,46 +54,6 @@ static_assert(sizeof(BinHeader) == 1024, "header is 1 KB");
 __device__ __forceinline__ int len_bucket(int v, int len_capacity) {
     const long long b = (long long)v * LEN_BUCKETS / ((long long)max(len_capacity, 1) + 1);
     return (int)(b < LEN_BUCKETS - 1 ? b : LEN_BUCKETS - 1);
-}
-
-__device__ __forceinline__ void tile_bbox_of(float2 c, int r, int tiles_x, int tiles_y, int &x0, int &x1, int &y0,
-                                             int &y1) {
-    // get_tile_bbox (helpers.cuh:17-49) -- same arithmetic as project.cu / binning.cu
-    const float tcx = c.x / 16.f, tcy = c.y / 16.f, tr = (float)r / 16.f;
-    x0 = min(max(0, (int)(tcx - tr)), tiles_x);
-    x1 = min(max(0, (int)(tcx + tr + 1.f)), tiles_x);
-    y0 = min(max(0, (int)(tcy - tr)), tiles_y);
-    y1 = min(max(0, (int)(tcy + tr + 1.f)), tiles_y);
-}
-
-__device__ __forceinline__ int warp_incl_scan_i(int v) {
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += t;
-    }
-    return v;
-}
-
-// block-wide exclusive scan of one int per thread; *total = block sum.  smem: THREADS/32 + 1 ints.
-template <int THREADS>
-__device__ __forceinline__ int block_excl_scan_i(int v, int *total, int *smem) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const int inc = warp_incl_scan_i(v);
-    if (lane == 31) smem[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-        const int x = (lane < THREADS / 32) ? smem[lane] : 0;
-        const int xi = warp_incl_scan_i(x);
-        if (lane < THREADS / 32) smem[lane] = xi - x;
-        if (lane == 31) smem[THREADS / 32] = xi;
-    }
-    __syncthreads();
-    const int res = smem[w] + inc - v;
-    *total = smem[THREADS / 32];
-    __syncthreads();
-    return res;
 }
 
 // ---- single-pass chained scan across blocks (decoupled look-back) ------------------------------------------
@@ -160,7 +121,7 @@ bin_count_kernel(int n, const float2 *__restrict__ xys, const int *__restrict__ 
         float4 *dst = reinterpret_cast<float4 *>(gattr + i);
         dst[0] = rec.q0; dst[1] = rec.q1; dst[2] = rec.q2;
         int x0, x1, y0, y1;
-        tile_bbox_of(c, r, tiles_x, tiles_y, x0, x1, y0, y1);
+        gsb_tile_bbox(c.x, c.y, (float)r, tiles_x, tiles_y, x0, x1, y0, y1);
         for (int ty = y0; ty < y1; ++ty)
             for (int tx = x0; tx < x1; ++tx) {
                 if (cull && !extent_slot_mask(c.x, c.y, rec.q1.w, rec.q2.w, (float)(tx * GSB_TILE),
@@ -177,10 +138,10 @@ bin_count_kernel(int n, const float2 *__restrict__ xys, const int *__restrict__ 
 // 2048 counts per block, chained scan across blocks (decoupled look-back over ticket-ordered blocks).
 constexpr int GS_IPT = 8;
 __global__ void __launch_bounds__(BIN_THREADS)
-count_scan_kernel(int n, int *__restrict__ counts_then_cum, BinHeader *hdr, unsigned long long *state) {
+count_scan_kernel(int n, int *__restrict__ counts_then_cum, unsigned *ticket, unsigned long long *state) {
     __shared__ int sm[BIN_THREADS / 32 + 1];
     __shared__ int s_blk, s_prefix;
-    if (threadIdx.x == 0) s_blk = (int)atomicAdd(&hdr->ticket_n, 1u);
+    if (threadIdx.x == 0) s_blk = (int)atomicAdd(ticket, 1u);
     __syncthreads();
     const int blk = s_blk;
     const int e0 = (blk * BIN_THREADS + threadIdx.x) * GS_IPT;
@@ -198,7 +159,7 @@ count_scan_kernel(int n, int *__restrict__ counts_then_cum, BinHeader *hdr, unsi
 #pragma unroll
     for (int k = 0; k < GS_IPT; ++k) tsum += v[k];
     int total;
-    int run = block_excl_scan_i<BIN_THREADS>(tsum, &total, sm);
+    int run = block_excl_scan<BIN_THREADS>(tsum, &total, sm);
     if (threadIdx.x < 32) {
         const int p = chained_scan_prefix(state, blk, total);
         if (threadIdx.x == 0) s_prefix = p;
@@ -217,6 +178,18 @@ count_scan_kernel(int n, int *__restrict__ counts_then_cum, BinHeader *hdr, unsi
     }
 }
 
+}  // namespace
+
+// Host side of K1b, also called by gsb_cumsum_tiles_hit (binning.cu): in-place inclusive scan of n ints.  *ticket and
+// state[0 .. gsb_count_scan_blocks(n)) must be zero when the kernel starts.
+int gsb_count_scan_blocks(int n) { return gsb_div_up(n > 0 ? n : 1, BIN_THREADS * GS_IPT); }
+
+void gsb_count_scan(int n, int *counts_then_cum, unsigned *ticket, unsigned long long *state, cudaStream_t s) {
+    count_scan_kernel<<<gsb_count_scan_blocks(n), BIN_THREADS, 0, s>>>(n, counts_then_cum, ticket, state);
+}
+
+namespace {
+
 // K2: exclusive scan of the tile sizes -> tile_bins, write cursors, stats = {M, longest list, overflow, 0}
 __global__ void __launch_bounds__(TSCAN_THREADS)
 tile_scan_kernel(int T, int nblk, int m_capacity, int len_capacity, BinHeader *hdr, unsigned long long *state,
@@ -230,7 +203,7 @@ tile_scan_kernel(int T, int nblk, int m_capacity, int len_capacity, BinHeader *h
     const int v = (t < T) ? tile_count_then_cursor[(size_t)t * CUR_STRIDE] : 0;
     if (t < T) atomicAdd(&hdr->len_hist[len_bucket(v, len_capacity)], 1);
     int total;
-    const int excl = block_excl_scan_i<TSCAN_THREADS>(v, &total, sm);
+    const int excl = block_excl_scan<TSCAN_THREADS>(v, &total, sm);
     const int wmax = __reduce_max_sync(0xffffffffu, v);
     if ((threadIdx.x & 31) == 0 && wmax > 0) atomicMax(&s_max, wmax);
     if (threadIdx.x < 32) {
@@ -296,7 +269,7 @@ bucket_emit_kernel(int n, const GsbRecord *__restrict__ gattr, const float *__re
     const float4 q0 = src[0];
     const float hx = src[1].w, hy = src[2].w;
     int x0, x1, y0, y1;
-    tile_bbox_of(make_float2(q0.x, q0.y), r, tiles_x, tiles_y, x0, x1, y0, y1);
+    gsb_tile_bbox(q0.x, q0.y, (float)r, tiles_x, tiles_y, x0, x1, y0, y1);
     int k = (i == 0) ? 0 : cum_tiles_hit[i - 1];
     const unsigned long long hi = ((unsigned long long)(unsigned)__float_as_int(depths[i])) << 32;
     for (int ty = y0; ty < y1; ++ty)
@@ -315,17 +288,9 @@ typedef unsigned long long u64;
 
 // distribution sort of a tile's composites (tile_sort_pack_kernel)
 constexpr int DS_MIN_BINS = 64, DS_MAX_BINS = 2048;
-#ifndef GSB_DS_BIN_LIMIT
-#define GSB_DS_BIN_LIMIT 32     // a bin above this many entries (clustered depths) sends the tile to the comparison sorts
-#endif
-constexpr int DS_BIN_LIMIT = GSB_DS_BIN_LIMIT;
-#ifndef GSB_DSORT
-#define GSB_DSORT 1
-#endif
+constexpr int DS_BIN_LIMIT = 32;   // a bin above this many entries (clustered depths) sends the tile to the comparison sorts
 
-#ifndef GSB_BITONIC_MAX
-#define GSB_BITONIC_MAX 4096   // lists up to this (padded) length use the bitonic network (measured faster), longer ones the radix sort
-#endif
+constexpr int BITONIC_MAX = 4096;  // lists up to this (padded) length use the bitonic network (measured faster), longer ones the radix sort
 
 __device__ __forceinline__ u64 shfl_xor_u64(u64 v, int m) {
     unsigned lo = (unsigned)v, hi = (unsigned)(v >> 32);
@@ -596,7 +561,7 @@ tile_dsort_pack_kernel(int cap, const int2 *__restrict__ tile_bins, const unsign
             tsum += v[q]; tmax = max(tmax, v[q]);
         }
         int total;
-        int run = block_excl_scan_i<256>(tsum, &total, ds_scan);
+        int run = block_excl_scan<256>(tsum, &total, ds_scan);
         tmax = __reduce_max_sync(0xffffffffu, tmax);
         if (lane == 0) atomicMax(&ds_maxbin, tmax);
 #pragma unroll
@@ -652,7 +617,7 @@ tile_sort_pack_kernel(int cap, const int2 *__restrict__ tile_bins, const unsigne
     __shared__ unsigned s_flag;
     if (stats[2]) return;      // capacities exceeded: the host redoes the frame
     const int tile = blockIdx.x;
-    if (tile_done && tile_done[tile]) return;   // already ordered and packed by tile_dsort_pack_kernel
+    if (tile_done[tile]) return;   // already ordered and packed by tile_dsort_pack_kernel
     const int2 range = tile_bins[tile];
     const int L = range.y - range.x;
     if (L <= 0) return;
@@ -672,7 +637,7 @@ tile_sort_pack_kernel(int cap, const int2 *__restrict__ tile_bins, const unsigne
                 skey[lane] = a;
                 skey[32 + lane] = b;
             }
-        } else if (n2 <= GSB_BITONIC_MAX) {
+        } else if (n2 <= BITONIC_MAX) {
             // medium lists: bitonic network, <= 64-wide merges in registers / shuffles, wider strides in smem
             const int nwarps = blockDim.x >> 5, nblk = n2 >> 6;
             for (int blk = warp; blk < nblk; blk += nwarps) {
@@ -741,7 +706,7 @@ struct BucketLayout {
 };
 BucketLayout bucket_layout(int n, int m, int T) {
     BucketLayout L;
-    L.nblk_n = gsb_div_up(n > 0 ? n : 1, BIN_THREADS * GS_IPT);   // blocks of the count scan (K1b)
+    L.nblk_n = gsb_count_scan_blocks(n);
     L.nblk_t = gsb_div_up(T > 0 ? T : 1, TSCAN_THREADS);
     size_t o = 0;
     L.hdr = o; o += sizeof(BinHeader);
@@ -800,8 +765,7 @@ extern "C" int gsb_bucket_tile_ranges(int n, const float *xys, const int32_t *ra
         bin_count_kernel<<<gsb_div_up(n, BIN_THREADS), BIN_THREADS, 0, s>>>(
             n, reinterpret_cast<const float2 *>(xys), radii, conics, colors, opacities, cull, tiles_x, tiles_y, cursor,
             (GsbRecord *)(ws + L.gattr), cum_tiles_hit);
-        count_scan_kernel<<<L.nblk_n, BIN_THREADS, 0, s>>>(n, cum_tiles_hit, hdr,
-                                                          (unsigned long long *)(ws + L.state_n));
+        gsb_count_scan(n, cum_tiles_hit, &hdr->ticket_n, (unsigned long long *)(ws + L.state_n), s);
     }
     tile_scan_kernel<<<L.nblk_t, TSCAN_THREADS, 0, s>>>(T, L.nblk_t, m_capacity, len_capacity, hdr,
                                                        (unsigned long long *)(ws + L.state_t), cursor,
@@ -841,17 +805,15 @@ extern "C" int gsb_bucket_sort_pack(int n, int m_capacity, int len_capacity, con
     unsigned long long *comp = (unsigned long long *)(ws + L.comp);
     int *gids = (int *)(ws + L.gids);
     GsbRecord *gattr = (GsbRecord *)(ws + L.gattr);
-    const bool long_lists = GSB_DSORT && cap > 1024;   // K4a then carries the Gaussian ids as sort payload
+    const bool long_lists = cap > 1024;   // K4a then carries the Gaussian ids as sort payload
     bucket_emit_kernel<<<gsb_div_up(n, 256), 256, 0, s>>>(n, gattr, depths, radii, cum_tiles_hit, cull, tiles_x,
                                                          tiles_y, (int *)(ws + L.cursor), comp, gids,
                                                          long_lists ? (int *)(ws + L.gpos) : nullptr, stats);
     // K4a (distribution sort) stages the list twice in shared memory; lists beyond its capacity, and tiles whose
     // depths cluster, are left to K4b (comparison sorts)
-    unsigned char *tile_done = nullptr;
-    if (GSB_DSORT) {
-        const int dcap = cap < 8192 ? cap : 8192;
-        const size_t dsmem = (size_t)dcap * (long_lists ? 24 : 16);   // 2 x 8 B composites (+ 2 x 4 B Gaussian ids) per entry
-        tile_done = (unsigned char *)(ws + L.done);
+    const int dcap = cap < 8192 ? cap : 8192;
+    const size_t dsmem = (size_t)dcap * (long_lists ? 24 : 16);   // 2 x 8 B composites (+ 2 x 4 B Gaussian ids) per entry
+    unsigned char *tile_done = (unsigned char *)(ws + L.done);
 #define GSB_DSP(U, PAY)                                                                                         \
     do {                                                                                                        \
         if (dsmem > 32 * 1024)                                                                                  \
@@ -862,10 +824,9 @@ extern "C" int gsb_bucket_sort_pack(int n, int m_capacity, int len_capacity, con
                                                             reinterpret_cast<GsbRecord *>(records), sorted_index, \
                                                             gaussian_ids_sorted, stats, tile_done);             \
     } while (0)
-        if (long_lists) GSB_DSP(2, true);
-        else GSB_DSP(1, false);
+    if (long_lists) GSB_DSP(2, true);
+    else GSB_DSP(1, false);
 #undef GSB_DSP
-    }
     const size_t smem = (size_t)cap * 8;
 #define GSB_TSP(MAXI)                                                                                           \
     do {                                                                                                        \

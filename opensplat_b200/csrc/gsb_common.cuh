@@ -5,7 +5,7 @@
 #include <stdio.h>
 #include "../../include/gsplat_b200.h"
 
-#define GSB_VERSION 200
+#define GSB_VERSION 300
 
 // ---- error plumbing (thread-local message, C ABI returns the code) -------------------------
 void gsb_set_error(int code, const char *what, const char *file, int line);
@@ -82,5 +82,51 @@ __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
+}
+
+// ---- warp / block scans of one int per thread --------------------------------------------------
+__device__ __forceinline__ int warp_incl_scan(int v) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v += t;
+    }
+    return v;
+}
+
+// block-wide exclusive scan; returns the exclusive prefix and the block sum in *total.
+// smem: THREADS/32 + 1 ints.
+template <int THREADS>
+__device__ __forceinline__ int block_excl_scan(int v, int *total, int *smem) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int inc = warp_incl_scan(v);
+    if (lane == 31) smem[w] = inc;
+    __syncthreads();
+    if (w == 0) {
+        const int x = (lane < THREADS / 32) ? smem[lane] : 0;
+        const int xi = warp_incl_scan(x);
+        if (lane < THREADS / 32) smem[lane] = xi - x;
+        if (lane == 31) smem[THREADS / 32] = xi;
+    }
+    __syncthreads();
+    const int res = smem[w] + inc - v;
+    *total = smem[THREADS / 32];
+    __syncthreads();
+    return res;
+}
+
+// ---- tile bounding box of a projected Gaussian -------------------------------------------------
+// get_tile_bbox (helpers.cuh:17-49): tiles [x0, x1) x [y0, y1) touched by the square of half-width
+// `radius` around (cx, cy); (int) == cvt.rzi (saturating).  The projection (num_tiles_hit), both
+// binning paths (keys, bins) and the blend records must agree on it bit for bit, so every one of
+// them calls this; it contains no multiply-add, so --fmad does not change it.
+__device__ __forceinline__ void gsb_tile_bbox(float cx, float cy, float radius, int tiles_x, int tiles_y,
+                                              int &x0, int &x1, int &y0, int &y1) {
+    const float tcx = cx / 16.f, tcy = cy / 16.f, tr = radius / 16.f;
+    x0 = min(max(0, (int)(tcx - tr)), tiles_x);
+    x1 = min(max(0, (int)(tcx + tr + 1.f)), tiles_x);
+    y0 = min(max(0, (int)(tcy - tr)), tiles_y);
+    y1 = min(max(0, (int)(tcy + tr + 1.f)), tiles_y);
 }
 #endif  // __CUDACC__

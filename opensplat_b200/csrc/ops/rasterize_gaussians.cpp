@@ -178,9 +178,11 @@ torch::Tensor rasterizeForward(AutogradContext *ctx, unsigned flags, torch::Tens
         // pathological tile lists: generic global radix sort on the reference's own (unculled) intersection lists
         torch::Tensor nth = gsb::i32(numTilesHit);
         const size_t sb = gsb_cumsum_workspace_bytes(n);
-        torch::Tensor sws = torch::empty({(int64_t)sb}, gsb::like(x, torch::kUInt8));
-        gsb::check(gsb_cumsum_tiles_hit(n, nth.data_ptr<int32_t>(), cum.data_ptr<int32_t>(), sws.data_ptr(), sb,
-                                        nullptr, gsb::stream()),
+        torch::Tensor sws = torch::empty({(int64_t)sb + 256}, gsb::like(x, torch::kUInt8));
+        char *swsPtr = (char *)sws.data_ptr();
+        swsPtr += (256 - ((uintptr_t)swsPtr % 256)) % 256;
+        gsb::check(gsb_cumsum_tiles_hit(n, nth.data_ptr<int32_t>(), cum.data_ptr<int32_t>(), swsPtr, sb,
+                                        gsb::stream()),
                    "gsb_cumsum_tiles_hit");
         const int mRef = cum[n - 1].item<int>();
         Binned b = bin_and_sort(n, mRef, x, d, r, cum, tileBounds);

@@ -146,12 +146,8 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
             const float pxc = 0.5f * (float)img_w * ndcx + cx - 0.5f;
             const float pyc = 0.5f * (float)img_h * ndcy + cy - 0.5f;
 
-            // get_tile_bbox (helpers.cuh:17-49); (int) == cvt.rzi (saturating)
-            const float tcx = pxc / 16.f, tcy = pyc / 16.f, tr = radius / 16.f;
-            const int x0 = min(max(0, (int)(tcx - tr)), tiles_x);
-            const int x1 = min(max(0, (int)(tcx + tr + 1.f)), tiles_x);
-            const int y0 = min(max(0, (int)(tcy - tr)), tiles_y);
-            const int y1 = min(max(0, (int)(tcy + tr + 1.f)), tiles_y);
+            int x0, x1, y0, y1;
+            gsb_tile_bbox(pxc, pyc, radius, tiles_x, tiles_y, x0, x1, y0, y1);
             const int a = (x1 - x0) * (y1 - y0);
             if (a > 0) {
                 area = a;

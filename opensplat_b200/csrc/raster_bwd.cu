@@ -22,10 +22,6 @@
 // scheduling and two-level culling as the forward pass.
 #include "raster_common.cuh"
 
-#ifndef GSB_BWD_SLOT_SWITCH
-#define GSB_BWD_SLOT_SWITCH 1
-#endif
-
 int gsb_blend_grid(const void *kernel, int num_tiles);
 
 namespace {
@@ -42,14 +38,13 @@ __device__ __forceinline__ void zero_row(float *grad_rows, int k) {
     row[0] = z; row[1] = z; row[2] = z;
 }
 
-#ifndef GSB_BWD_MINB
-#define GSB_BWD_MINB 6   // 80 registers -> 6 CTAs per SM.  H100 SXM at 400 W, C2: 0.849 ms per launch against 0.885 ms
-                         // with 5 CTAs and 0.891 ms with 4
-#endif
+// 80 registers -> 6 CTAs per SM.  H100 SXM at 400 W, C2: 0.849 ms per launch against 0.885 ms with 5 CTAs and
+// 0.891 ms with 4
+constexpr int BWD_MIN_BLOCKS = 6;
 // SAT: v_output is the gradient w.r.t. the CLAMPED image of the forward kernel's SAT instantiation -- channels
 // marked as cut in final_idx bits 28..30 receive no gradient (clamp_max's mask, model.cpp:222).
 template <bool SAT>
-__global__ void __launch_bounds__(RK_THREADS, GSB_BWD_MINB)
+__global__ void __launch_bounds__(RK_THREADS, BWD_MIN_BLOCKS)
 rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                           const int2 *__restrict__ tile_bins, const GsbRecord *__restrict__ records,
                           const float *__restrict__ background, const float *__restrict__ final_Ts,
@@ -174,7 +169,9 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 float s0 = 0.f, s1 = 0.f, s2 = 0.f;  // sum w, sum w dy, sum w dy^2 over this lane's pixels
                 float a_r = 0.f, a_g = 0.f, a_b = 0.f;
                 bool any = false;
-                const int jlo = __ffs(rm) - 1, jhi = 31 - __clz(rm);   // slots inside the y-extent (contiguous)
+                // slots jlo..jhi inside the y-extent (contiguous); a computed jump to jlo that leaves after jhi (an
+                // A/B measurement chose it over the forward kernel's straight line of per-slot bit tests)
+                const int jlo = __ffs(rm) - 1, jhi = 31 - __clz(rm);
 #define GSB_BWD_SLOT(j)                                                                                   \
     {                                                                                                     \
         const float dy = dy0 - (float)(2 * j);  /* centre.y - pixel row */                                                                    \
@@ -203,7 +200,6 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
         }                                                                                                 \
         if (jhi == j) break;                                                                              \
     }
-#if GSB_BWD_SLOT_SWITCH
                 switch (jlo) {
                     case 0: GSB_BWD_SLOT(0)
                     case 1: GSB_BWD_SLOT(1)
@@ -214,19 +210,6 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                     case 6: GSB_BWD_SLOT(6)
                     default: GSB_BWD_SLOT(7)
                 }
-#else
-                (void)jlo;
-                do {
-                    if (rm & 1u) GSB_BWD_SLOT(0)
-                    if (rm & 2u) GSB_BWD_SLOT(1)
-                    if (rm & 4u) GSB_BWD_SLOT(2)
-                    if (rm & 8u) GSB_BWD_SLOT(3)
-                    if (rm & 16u) GSB_BWD_SLOT(4)
-                    if (rm & 32u) GSB_BWD_SLOT(5)
-                    if (rm & 64u) GSB_BWD_SLOT(6)
-                    if (rm & 128u) GSB_BWD_SLOT(7)
-                } while (0);
-#endif
 #undef GSB_BWD_SLOT
                 const int k = __float_as_int(q0.w);
                 float *row = grad_rows + (size_t)k * GSB_GRAD_ROW_FLOATS;

@@ -23,10 +23,7 @@ static_assert(sizeof(GsbRecord) == 48, "record must be 48 bytes");
 // Blend-kernel geometry: one WARP owns one 16x16 tile at a time (persistent warps pull tile ids from
 // a global counter); lane l owns column (l & 15) and the 8 rows 2*j + (l >> 4), j = 0..7 ("slot" j =
 // the two pixel rows 2j, 2j+1).  No block-level synchronisation anywhere in the blend loops.
-#ifndef GSB_RK_WARPS
-#define GSB_RK_WARPS 4
-#endif
-constexpr int RK_WARPS = GSB_RK_WARPS;   // warps per CTA
+constexpr int RK_WARPS = 4;            // warps per CTA
 constexpr int RK_THREADS = RK_WARPS * 32;
 constexpr int RK_PIX = 8;              // pixels per lane
 constexpr int RK_CHUNK = 32;           // records per TMA bulk copy (1536 B) == one record per lane

@@ -22,10 +22,6 @@
 //    sigma <= smax is tested before the exp.
 #include "raster_common.cuh"
 
-#ifndef GSB_FWD_SLOT_SWITCH
-#define GSB_FWD_SLOT_SWITCH 0
-#endif
-
 namespace {
 
 __global__ void __launch_bounds__(256)
@@ -46,10 +42,9 @@ pack_records_kernel(int m, const int *__restrict__ gaussian_ids_sorted,
     stg_stream4(dst + 2, r.q2);
 }
 
-#ifndef GSB_FWD_MINB
-#define GSB_FWD_MINB 8   // 64 registers -> 8 CTAs (32 warps) per SM.  H100 SXM at 400 W, C2: 0.416 ms per launch against
-                         // 0.445 ms with 7 CTAs and 0.464 ms with 6 (which needs no spill): occupancy wins
-#endif
+// 64 registers -> 8 CTAs (32 warps) per SM.  H100 SXM at 400 W, C2: 0.416 ms per launch against 0.445 ms with 7 CTAs
+// and 0.464 ms with 6 (which needs no spill): occupancy wins
+constexpr int FWD_MIN_BLOCKS = 8;
 // COUNT = true is a diagnostic instantiation (gsb_rasterize_forward_count): same arithmetic, plus per-launch
 // totals of {records that pass the per-record test, slot visits, pixel pairs whose sigma is inside the
 // extent (ex2 evaluated), pixel pairs blended} in pair_counts[0..3].  The production instantiation carries none
@@ -58,7 +53,7 @@ pack_records_kernel(int m, const int *__restrict__ gaussian_ids_sorted,
 // and, per pixel, which channels were cut (!(value <= 1), torch's clamp_max mask) goes into bits 28..30 of final_idx
 // for the SAT instantiation of the backward kernel (sorted indices stay below 2^28, checked by the entry point).
 template <bool COUNT, bool SAT>
-__global__ void __launch_bounds__(RK_THREADS, GSB_FWD_MINB)
+__global__ void __launch_bounds__(RK_THREADS, FWD_MIN_BLOCKS)
 rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                          const int2 *__restrict__ tile_bins, const GsbRecord *__restrict__ records,
                          const float *__restrict__ background, float *__restrict__ out_img,
@@ -150,10 +145,10 @@ rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 const float bdx = q1.y * dx;
                 const float dy0 = q0.y - py0;
                 const int idx = idx0 + t;   // sorted index of this record (final_idx of the pixels it is the last to blend)
-                // visit only the slots jlo..jhi (contiguous) inside the record's y-extent; warp-uniform control
-                // flow.  Two code shapes, chosen per kernel by A/B measurement: a computed jump into the slot
-                // sequence (GSB_*_SLOT_SWITCH=1), or a straight line of per-slot bit tests that leaves after jhi.
-                const int jlo = __ffs(rm) - 1, jhi = 31 - __clz(rm);
+                // visit only the slots inside the record's y-extent (contiguous); warp-uniform control flow: a
+                // straight line of per-slot bit tests that leaves after the last slot jhi (an A/B measurement
+                // chose it over a computed jump to the first slot, which the backward kernel uses)
+                const int jhi = 31 - __clz(rm);
 #define GSB_FWD_SLOT(j)                                                                                   \
     {                                                                                                     \
         const float dy = dy0 - (float)(2 * j);  /* centre.y - pixel row */                                                                    \
@@ -181,19 +176,6 @@ rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
         }                                                                                                 \
         if (jhi == j) break;                                                                              \
     }
-#if GSB_FWD_SLOT_SWITCH
-                switch (jlo) {
-                    case 0: GSB_FWD_SLOT(0)
-                    case 1: GSB_FWD_SLOT(1)
-                    case 2: GSB_FWD_SLOT(2)
-                    case 3: GSB_FWD_SLOT(3)
-                    case 4: GSB_FWD_SLOT(4)
-                    case 5: GSB_FWD_SLOT(5)
-                    case 6: GSB_FWD_SLOT(6)
-                    default: GSB_FWD_SLOT(7)
-                }
-#else
-                (void)jlo;
                 do {   // straight-line: one warp-uniform test per slot
                     if (rm & 1u) GSB_FWD_SLOT(0)
                     if (rm & 2u) GSB_FWD_SLOT(1)
@@ -204,7 +186,6 @@ rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                     if (rm & 64u) GSB_FWD_SLOT(6)
                     if (rm & 128u) GSB_FWD_SLOT(7)
                 } while (0);
-#endif
 #undef GSB_FWD_SLOT
             }
             if (__all_sync(0xffffffffu, done == 0xffu)) { ++c; break; }  // whole tile saturated

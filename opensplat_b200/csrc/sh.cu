@@ -7,15 +7,9 @@
 // moves its 128 Gaussians' coefficients as one contiguous span with 128-bit streaming accesses
 // (fully coalesced, L1 bypassed) through a padded shared-memory transpose; rows are padded to
 // 4*odd floats so the per-thread 128-bit row reads are bank-conflict free.
-#include <stdlib.h>
 #include "gsb_common.cuh"
 
-static int gsb_sm_count_sh() {
-    int dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return sms > 0 ? sms : 132;
-}
+int gsb_sm_count();
 
 namespace {
 
@@ -487,18 +481,6 @@ extern "C" int gsb_mask_rgb_grad(int n, const float *rgbs, float *v_rgbs, gsb_st
     return 0;
 }
 
-// CTAs per SM of the all-reduce role (GSB_GEOM_BLOCKS overrides the default for experiments)
-static int geom_blocks_per_sm() {
-    static int v = 0;
-    if (v == 0) {
-        const char *e = getenv("GSB_GEOM_BLOCKS");
-        v = e ? atoi(e) : 4;
-        if (v < 1) v = 1;
-        if (v > 32) v = 32;
-    }
-    return v;
-}
-
 static int launch_multiview(int n, int degree, int degrees_to_use, const float *means, int num_views,
                             const float *cam_positions, const float *const *v_rgbs_per_view, float scale,
                             float *v_coeffs, int rank, int world, long long geom_floats, float *const *geom_per_rank,
@@ -512,10 +494,9 @@ static int launch_multiview(int n, int degree, int degrees_to_use, const float *
         GSB_CHECK_ARG(((uintptr_t)geom_multicast % 16) == 0);
         // about two rounds of four 16-byte reductions per thread; between 1 and 8 CTAs per SM.  (The role is bound
         // by the switch, so fewer CTAs leave more slots to the colour half.)
-        const int sms = gsb_sm_count_sh();
+        const int sms = gsb_sm_count();
         const long long slice = (geom_floats / 4 + world - 1) / world;
-        long long want = (slice + 2 * 4 * SH_THREADS - 1) / (2 * 4 * SH_THREADS);
-        if (getenv("GSB_GEOM_BLOCKS")) want = (long long)geom_blocks_per_sm() * sms;
+        const long long want = (slice + 2 * 4 * SH_THREADS - 1) / (2 * 4 * SH_THREADS);
         geom_blocks = (int)(want < sms ? sms : (want > 8LL * sms ? 8LL * sms : want));
     }
     if (n == 0 && geom_blocks == 0) return 0;

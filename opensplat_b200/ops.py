@@ -128,9 +128,10 @@ def cumsum_tiles_hit(num_tiles_hit):
     cum = _empty((n,), torch.int32, num_tiles_hit)
     L = capi.lib()
     wsb = L.gsb_cumsum_workspace_bytes(n)
-    ws = _ws.get(num_tiles_hit.device, "cumsum", wsb)
-    capi.check(L.gsb_cumsum_tiles_hit(n, capi.ptr(num_tiles_hit), capi.ptr(cum), capi.ptr(ws), ws.numel(),
-                                      None, capi.stream()))
+    ws = _ws.get(num_tiles_hit.device, "cumsum", wsb + 256)
+    off = (-ws.data_ptr()) % 256
+    capi.check(L.gsb_cumsum_tiles_hit(n, capi.ptr(num_tiles_hit), capi.ptr(cum), ws.data_ptr() + off,
+                                      ws.numel() - off, capi.stream()))
     return cum
 
 

@@ -1,4 +1,5 @@
-"""Times the stages of one step for a given library variant (GSB_LIB=path) -- used to A/B kernel variants.
+"""Times the stages of one step with the library at GSB_LIB (default: the in-tree build) -- run it once with each of
+two commits' builds to compare them stage by stage.
 usage: GSB_LIB=... python tools/bench_blend.py [workload] [reps]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

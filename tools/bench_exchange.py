@@ -113,8 +113,7 @@ def main():
         # G-1 peers) + the other ranks' reduced slices
         recv = rgb_bytes + (geom_bytes if flavour == "multimem" else geom_bytes // world * (world - 1) * 2)
         r = {"step_ms_mask_barrier_launch_barrier": full, "launch_only_ms": k_only, "sh_half_only_ms": sh,
-             "geometry_half_only_ms": go, "two_streams_ms": ts, "geom_blocks_per_sm": os.environ.get("GSB_GEOM_BLOCKS", "4"),
-             "barrier_ms": bar, "bytes_received_per_rank_model": recv,
+             "geometry_half_only_ms": go, "two_streams_ms": ts, "barrier_ms": bar, "bytes_received_per_rank_model": recv,
              "nvlink_GBps_achieved_launch_only": recv / (k_only * 1e-3) / 1e9,
              "nvlink_GBps_colour_pull_only": rgb_bytes / (sh * 1e-3) / 1e9,
              "nvlink_reference_GBps": 450.0,   # H100 SXM data sheet: NVLink 4, 450 GB/s per direction
