@@ -39,6 +39,8 @@ extern "C" {
 #define GSB_ERR_UNSUPPORTED (-3)
 /* flags of gsb_rasterize_forward_packed / gsb_rasterize_backward */
 #define GSB_RASTER_CLAMP_MAX_ONE 1u
+/* or-ed into the `cull` argument of gsb_bucket_tile_ranges: report the visible count in stats[3] */
+#define GSB_BIN_COUNT_VISIBLE 2
 
 typedef void *gsb_stream_t; /* cudaStream_t */
 
@@ -78,6 +80,15 @@ int gsb_sh_forward_split(int n, int degree, int degrees_to_use, const float *mea
 int gsb_sh_backward_split(int n, int degree, int degrees_to_use, const float *means, const float *cam_pos,
                           const float *rgbs, const float *v_rgbs, float *v_features_dc, float *v_features_rest,
                           gsb_stream_t stream);
+/* Camera variants: the split variants' view directions (viewdirs = means - cam_pos, cam_pos a device float[3],
+ * normalised inside, no gradient) on a merged coeffs / v_coeffs [n,K,3] block, as the flat parameter layout stores
+ * it.  rgbs = clamp_min(SH + bias, 0); the backward masks v_rgbs with [rgbs > 0] and fully writes v_coeffs (bases above
+ * degrees_to_use get 0).  rgbs and the coefficient gradients are bit-identical to the split variants' on the same
+ * data. */
+int gsb_sh_forward_rgb_cam(int n, int degree, int degrees_to_use, const float *means, const float *cam_pos,
+                           const float *coeffs, float bias, float *rgbs, gsb_stream_t stream);
+int gsb_sh_backward_rgb_cam(int n, int degree, int degrees_to_use, const float *means, const float *cam_pos,
+                            const float *rgbs, const float *v_rgbs, float *v_coeffs, gsb_stream_t stream);
 
 /* Data-parallel training (SURVEY.md 8e): SH VJP fused with the cross-GPU gradient exchange.
  * gsb_mask_rgb_grad: v_rgbs *= [rgbs > 0] in place (gradient of the clamp, done before exposing v_rgbs).
@@ -189,8 +200,11 @@ int gsb_gather_bin_edges(int m, int num_tiles, const int64_t *isect_ids_sorted,
  *   lists (internal to the operator: the reference's RasterizeGaussians does not return them).
  * Capacities: the caller sizes `workspace` (gsb_bucket_workspace_bytes(n, m_capacity, tiles)), `records`
  *   (gsb_raster_records_bytes(m_capacity)) and the sort's shared memory (len_capacity <= gsb_bucket_max_tile_len())
- *   from earlier frames; stats (device int32[4]) = {M, longest tile list, overflow, 0} with overflow = 1 iff
- *   M > m_capacity or longest > len_capacity, in which case gsb_bucket_sort_pack and
+ *   from earlier frames; stats (device int32[4]) = {M, longest tile list, overflow, visible} with overflow = 1 iff
+ *   M > m_capacity or longest > len_capacity.  visible is 0 unless gsb_bucket_tile_ranges gets
+ *   cull | GSB_BIN_COUNT_VISIBLE; then it is the number of Gaussians with radii > 0 (counted from radii, not from the
+ *   lists: with the cull a visible Gaussian may sit in no tile list; visible == 0 is the `radii.sum() == 0` test of
+ *   model.cpp:173, here answered by the frame's one read-back).  On overflow gsb_bucket_sort_pack and
  *   gsb_rasterize_forward_packed (given the same stats pointer) do nothing: the host reads stats back AFTER
  *   enqueuing the whole forward pass and, on overflow, repeats the three calls with larger capacities.
  *   Exact-size use: m_capacity = M, len_capacity = longest list of a previous gsb_bucket_tile_ranges call.
@@ -275,6 +289,23 @@ int gsb_mse_loss_grad(long long n, const float *img, const float *target, float 
 int gsb_adam_step(long long n, float *param, const float *grad, float *exp_avg, float *exp_avg_sq, float lr,
                   float beta1, float beta2, float eps, float bias_correction1, float bias_correction2,
                   gsb_stream_t stream);
+/* gsb_adam_step_segments: gsb_adam_step with per-segment learning rates, in one launch (the six optimizers of
+ *   model.cpp:58-70 over one flat buffer).  `segments` is a HOST array of num_segments (<= GSB_ADAM_MAX_SEGMENTS)
+ *   entries; segment s covers floats [offset, offset + count) of all four buffers (offset a multiple of 4; the
+ *   buffers 16-byte aligned), and its element e takes lr_head if e % row_floats < head_floats, lr_rest otherwise
+ *   (a merged [n,K,3] SH block: row_floats = 3K, head_floats = 3 gives featuresDc / featuresRest their own rates).
+ *   Floats outside every segment are not touched.  Same update as gsb_adam_step, with one rounding for every float:
+ *   the parameter step's product is rounded before the subtraction.  gsb_adam_step's compiled kernel fuses that step
+ *   into one FMA on every fourth float and on its scalar tail, so those floats can differ in the last bit. */
+#define GSB_ADAM_MAX_SEGMENTS 8
+typedef struct gsb_adam_segment {
+    long long offset, count;
+    int row_floats, head_floats;
+    float lr_head, lr_rest;
+} gsb_adam_segment;
+int gsb_adam_step_segments(int num_segments, const gsb_adam_segment *segments, float *param, const float *grad,
+                           float *exp_avg, float *exp_avg_sq, float beta1, float beta2, float eps,
+                           float bias_correction1, float bias_correction2, gsb_stream_t stream);
 
 /* gsb_activate_forward / gsb_activate_backward: the parameter activations of Model::forward fused into one
  *   pass each way (model.cpp:148-150,176-177,200): scales = exp(log_scales), quats = raw_quats / |raw_quats|,

@@ -24,6 +24,8 @@ _SIGS = {
     "gsb_sh_backward_rgb": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "gsb_sh_forward_split": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
     "gsb_sh_backward_split": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_sh_forward_rgb_cam": (_i, [_i, _i, _i, _vp, _vp, _vp, _f, _vp, _vp]),
+    "gsb_sh_backward_rgb_cam": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_mask_rgb_grad": (_i, [_i, _vp, _vp, _vp]),
     "gsb_sh_backward_multiview": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _vp]),
     "gsb_exchange_gradients": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _i, _i, C.c_longlong, _vp, _vp, _vp]),
@@ -73,8 +75,18 @@ _SIGS = {
     "gsb_ssim_workspace_bytes": (_sz, [_i, _i]),
     "gsb_ssim_l1_loss": (_i, [_i, _i, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
     "gsb_adam_step": (_i, [C.c_longlong, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _vp]),
+    # num_segments, segments (host AdamSegment array), param, grad, exp_avg, exp_avg_sq, b1, b2, eps, bc1, bc2, stream
+    "gsb_adam_step_segments": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _vp]),
     "gsb_mse_loss_grad": (_i, [C.c_longlong, _vp, _vp, _vp, _vp, _f, _vp]),
 }
+
+ADAM_MAX_SEGMENTS = 8   # GSB_ADAM_MAX_SEGMENTS
+
+
+class AdamSegment(C.Structure):
+    """gsb_adam_segment (include/gsplat_b200.h)."""
+    _fields_ = [("offset", C.c_longlong), ("count", C.c_longlong), ("row_floats", C.c_int),
+                ("head_floats", C.c_int), ("lr_head", C.c_float), ("lr_rest", C.c_float)]
 # optional symbols (experimental entry points) are bound when present
 _OPT_SIGS = {}
 

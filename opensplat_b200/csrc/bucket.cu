@@ -10,7 +10,7 @@
 //                       of the per-Gaussian counts -> cum_tiles_hit (the gradient-row slots).  The generic path's
 //                       gsb_cumsum_tiles_hit (binning.cu) is this same scan, launched through gsb_count_scan.
 //   K2 tile_scan      : exclusive scan over the T tiles (chained scan over <= 32 CTAs) -> tile_bins (first, last+1),
-//                       write cursors, stats = {M, longest list, overflow flag}
+//                       write cursors, stats = {M, longest list, overflow flag, visible count of K1}
 //   K3 bucket_emit    : per Gaussian, write (depth bits << 32 | k) into its tiles' segments (atomic cursor;
 //                       arrival order is arbitrary, the composite key makes the final order unique)
 //   K4 tile_sort_pack : one CTA per tile sorts its segment in shared memory (64-bit composites), then gathers the
@@ -43,7 +43,8 @@ struct BinHeader {          // 1 KB at the start of the workspace, zeroed by the
     unsigned done_t;        // K2 blocks finished
     int max_len;            // longest tile list (atomicMax)
     int total;              // M
-    int pad0[3];
+    int visible;            // Gaussians with radii > 0 (K1: one atomic per CTA)
+    int pad0[2];
     int len_hist[LEN_BUCKETS];   // tiles per list-length bucket (K2), for the longest-first tile order (K2b)
     int len_cur[LEN_BUCKETS];    // K2b write cursors
     int pad[120];
@@ -102,16 +103,23 @@ __device__ __forceinline__ int chained_scan_prefix(unsigned long long *state, in
     return excl;
 }
 
-// K1: attribute record + tile counting; writes the per-Gaussian count of binned tiles (scanned by K1b)
+// K1: attribute record + tile counting; writes the per-Gaussian count of binned tiles (scanned by K1b).  With
+// `visible` given, adds the CTA's count of visible Gaussians (radii > 0, whether or not the cull leaves them in any
+// tile list: the test of model.cpp:173 is radii.sum() == 0) to *visible with one atomic.
 __global__ void __launch_bounds__(BIN_THREADS)
 bin_count_kernel(int n, const float2 *__restrict__ xys, const int *__restrict__ radii,
                  const float *__restrict__ conics, const float *__restrict__ colors,
                  const float *__restrict__ opacities, int cull, int tiles_x, int tiles_y,
-                 int *__restrict__ tile_count, GsbRecord *__restrict__ gattr, int *__restrict__ count_out) {
+                 int *__restrict__ tile_count, GsbRecord *__restrict__ gattr, int *__restrict__ count_out,
+                 int *__restrict__ visible) {
     const int i = blockIdx.x * BIN_THREADS + threadIdx.x;
+    const int r = (i < n) ? radii[i] : 0;
+    if (visible) {   // uniform over the grid: the barrier is reached by every thread or by none
+        const int nvis = __syncthreads_count(r > 0);
+        if (threadIdx.x == 0 && nvis > 0) atomicAdd(visible, nvis);
+    }
     if (i >= n) return;
     int cnt = 0;
-    const int r = radii[i];
     if (r > 0) {
         const float2 c = xys[i];
         // the record of this Gaussian is built ONCE here (log2 / sqrt / extents) and only copied per intersection
@@ -190,7 +198,7 @@ void gsb_count_scan(int n, int *counts_then_cum, unsigned *ticket, unsigned long
 
 namespace {
 
-// K2: exclusive scan of the tile sizes -> tile_bins, write cursors, stats = {M, longest list, overflow, 0}
+// K2: exclusive scan of the tile sizes -> tile_bins, write cursors, stats = {M, longest list, overflow, visible}
 __global__ void __launch_bounds__(TSCAN_THREADS)
 tile_scan_kernel(int T, int nblk, int m_capacity, int len_capacity, BinHeader *hdr, unsigned long long *state,
                  int *__restrict__ tile_count_then_cursor, int2 *__restrict__ tile_bins, int *__restrict__ stats) {
@@ -228,7 +236,7 @@ tile_scan_kernel(int T, int nblk, int m_capacity, int len_capacity, BinHeader *h
             stats[0] = M;
             stats[1] = mx;
             stats[2] = (M > m_capacity || mx > len_capacity) ? 1 : 0;
-            stats[3] = 0;
+            stats[3] = hdr->visible;   // complete (K1 ran before this kernel); 0 unless counted
         }
     }
 }
@@ -741,7 +749,8 @@ extern "C" size_t gsb_bucket_workspace_bytes(int n, int m_capacity, int num_tile
 }
 
 // Phase 1: attribute records, tile sizes -> tile_bins + write cursors (inside the workspace), the scan of the
-// per-Gaussian tile counts and stats = {M, longest list, overflow, 0} (device int32[4]).
+// per-Gaussian tile counts and stats = {M, longest list, overflow, visible Gaussians or 0} (device int32[4]).
+// cull: bit 0 culls by the extent box; GSB_BIN_COUNT_VISIBLE asks for the visible count in stats[3].
 extern "C" int gsb_bucket_tile_ranges(int n, const float *xys, const int32_t *radii, const float *conics,
                                       const float *colors, const float *opacities, int cull, int tiles_x,
                                       int tiles_y, int m_capacity, int len_capacity, void *workspace,
@@ -749,6 +758,9 @@ extern "C" int gsb_bucket_tile_ranges(int n, const float *xys, const int32_t *ra
                                       int32_t *tile_order, int32_t *stats, gsb_stream_t stream) {
     GSB_CHECK_ARG(n >= 0 && tiles_x > 0 && tiles_y > 0 && m_capacity >= 0 && len_capacity >= 0);
     GSB_CHECK_ARG(tile_bins && stats && workspace && ((uintptr_t)workspace % 256) == 0);
+    GSB_CHECK_ARG((cull & ~(1 | GSB_BIN_COUNT_VISIBLE)) == 0);
+    const bool count_visible = (cull & GSB_BIN_COUNT_VISIBLE) != 0;
+    cull &= 1;
     const int T = tiles_x * tiles_y;
     const BucketLayout L = bucket_layout(n, m_capacity, T);
     if (workspace_bytes < L.total) {
@@ -764,7 +776,7 @@ extern "C" int gsb_bucket_tile_ranges(int n, const float *xys, const int32_t *ra
         GSB_CHECK_ARG(xys && radii && conics && colors && opacities && cum_tiles_hit && ((uintptr_t)xys % 8) == 0);
         bin_count_kernel<<<gsb_div_up(n, BIN_THREADS), BIN_THREADS, 0, s>>>(
             n, reinterpret_cast<const float2 *>(xys), radii, conics, colors, opacities, cull, tiles_x, tiles_y, cursor,
-            (GsbRecord *)(ws + L.gattr), cum_tiles_hit);
+            (GsbRecord *)(ws + L.gattr), cum_tiles_hit, count_visible ? &hdr->visible : nullptr);
         gsb_count_scan(n, cum_tiles_hit, &hdr->ticket_n, (unsigned long long *)(ws + L.state_n), s);
     }
     tile_scan_kernel<<<L.nblk_t, TSCAN_THREADS, 0, s>>>(T, L.nblk_t, m_capacity, len_capacity, hdr,

@@ -3,6 +3,8 @@
 //                       (simple_trainer.cpp:199-201 does this with torch::nn::MSELoss + autograd)
 //   gsb_adam_step     : one fused Adam update over a flat parameter buffer
 //                       (simple_trainer.cpp:146,202 torch::optim::Adam; model.cpp:236-243 runs six of them)
+//   gsb_adam_step_segments : the same update with a learning rate per segment (and per row position inside it),
+//                       i.e. the six optimizers of model.cpp:58-70 over one flat buffer in one launch
 // Both are HBM-bound elementwise passes: 128-bit accesses, grid = multiple of the SM count.
 #include "gsb_common.cuh"
 
@@ -79,6 +81,66 @@ adam_kernel(long long n4, long long n, float *__restrict__ p, const float *__res
     }
     for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
         upd(p[i], g[i], m[i], v[i]);
+}
+
+// adam_kernel's update of one element with its roundings spelled out: FFMA for m, v and the denominator, the
+// parameter step as FMUL + FADD.  Left to the compiler, the contraction depends on the surrounding code: adam_kernel's
+// SASS rounds the parameter step like this in lanes x-z of its float4 path but fuses it into one FFMA in lane w and in
+// its scalar tail, so those floats of a gsb_adam_step call can differ from this in the last bit.  Both paths of the
+// segmented kernel call this one function, so its result does not depend on where a float falls.
+__device__ __forceinline__ void adam_update(float &pp, float gg, float &mm, float &vv, float lr, float b1, float b2,
+                                            float eps, float inv_bc1, float inv_sqrt_bc2) {
+    mm = __fmaf_rn(1.f - b1, gg, b1 * mm);
+    vv = __fmaf_rn(gg, (1.f - b2) * gg, b2 * vv);
+    // torch.optim.Adam: p -= lr/bc1 * m / (sqrt(v)/sqrt(bc2) + eps)
+    pp = __fsub_rn(pp, __fmul_rn(lr * inv_bc1, __fdividef(mm, __fmaf_rn(sqrtf(vv), inv_sqrt_bc2, eps))));
+}
+
+// The segment table travels by value in the kernel's parameter space (8 x 32 B).
+struct AdamSegments {
+    gsb_adam_segment s[GSB_ADAM_MAX_SEGMENTS];
+    int count;
+};
+
+// Adam over the segments of a flat buffer in one launch: element e of segment s takes lr_head when
+// e % row_floats < head_floats and lr_rest otherwise.  Segments start on 16-byte boundaries; the floats between
+// them (padding) are never touched.
+__global__ void __launch_bounds__(256)
+adam_segments_kernel(AdamSegments segs, float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m,
+                     float *__restrict__ v, float b1, float b2, float eps, float inv_bc1, float inv_sqrt_bc2) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (int k = 0; k < segs.count; ++k) {
+        const gsb_adam_segment sg = segs.s[k];
+        float *ps = p + sg.offset, *ms = m + sg.offset, *vs = v + sg.offset;
+        const float *gs = g + sg.offset;
+        const long long n4 = sg.count / 4;
+        for (long long i = t0; i < n4; i += stride) {
+            float4 P = reinterpret_cast<float4 *>(ps)[i];
+            const float4 G = ldg_stream4(reinterpret_cast<const float4 *>(gs) + i);
+            float4 M = reinterpret_cast<float4 *>(ms)[i];
+            float4 V = reinterpret_cast<float4 *>(vs)[i];
+            // a float4 may straddle a head / rest boundary: the rate is chosen per component
+            int j = (int)((4 * i) % sg.row_floats);
+            float lr[4];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                lr[c] = j < sg.head_floats ? sg.lr_head : sg.lr_rest;
+                if (++j == sg.row_floats) j = 0;
+            }
+            adam_update(P.x, G.x, M.x, V.x, lr[0], b1, b2, eps, inv_bc1, inv_sqrt_bc2);
+            adam_update(P.y, G.y, M.y, V.y, lr[1], b1, b2, eps, inv_bc1, inv_sqrt_bc2);
+            adam_update(P.z, G.z, M.z, V.z, lr[2], b1, b2, eps, inv_bc1, inv_sqrt_bc2);
+            adam_update(P.w, G.w, M.w, V.w, lr[3], b1, b2, eps, inv_bc1, inv_sqrt_bc2);
+            reinterpret_cast<float4 *>(ps)[i] = P;
+            reinterpret_cast<float4 *>(ms)[i] = M;
+            reinterpret_cast<float4 *>(vs)[i] = V;
+        }
+        for (long long e = 4 * n4 + t0; e < sg.count; e += stride) {
+            const float lr = (int)(e % sg.row_floats) < sg.head_floats ? sg.lr_head : sg.lr_rest;
+            adam_update(ps[e], gs[e], ms[e], vs[e], lr, b1, b2, eps, inv_bc1, inv_sqrt_bc2);
+        }
+    }
 }
 
 // ---- parameter activations of Model::forward (model.cpp:114,148-150,176-177,200), one pass each way ----
@@ -195,6 +257,35 @@ extern "C" int gsb_adam_step(long long n, float *param, const float *grad, float
     adam_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n4, n, param, grad, exp_avg, exp_avg_sq, lr, beta1,
                                                                beta2, eps, 1.f / bias_correction1,
                                                                1.f / sqrtf(bias_correction2));
+    GSB_LAUNCH_CHECK();
+    return 0;
+}
+
+// The six optimizers of Model::setupOptimizers (model.cpp:58-70) over one flat buffer in one launch: one segment
+// per parameter slice, the merged SH block as one segment with two rates (featuresDc on the first 3 floats of
+// every 3K-float row, featuresRest on the rest).  Same update as gsb_adam_step.
+extern "C" int gsb_adam_step_segments(int num_segments, const gsb_adam_segment *segments, float *param,
+                                      const float *grad, float *exp_avg, float *exp_avg_sq, float beta1, float beta2,
+                                      float eps, float bias_correction1, float bias_correction2,
+                                      gsb_stream_t stream) {
+    GSB_CHECK_ARG(num_segments >= 0 && num_segments <= GSB_ADAM_MAX_SEGMENTS && (num_segments == 0 || segments));
+    GSB_CHECK_ARG(bias_correction1 > 0.f && bias_correction2 > 0.f);
+    AdamSegments segs = {};
+    long long total = 0;
+    for (int k = 0; k < num_segments; ++k) {
+        const gsb_adam_segment &sg = segments[k];
+        GSB_CHECK_ARG(sg.offset >= 0 && sg.offset % 4 == 0 && sg.count >= 0);
+        GSB_CHECK_ARG(sg.row_floats > 0 && sg.head_floats >= 0 && sg.head_floats <= sg.row_floats);
+        segs.s[k] = sg;
+        total += sg.count;
+    }
+    segs.count = num_segments;
+    if (total == 0) return 0;
+    GSB_CHECK_ARG(param && grad && exp_avg && exp_avg_sq);
+    GSB_CHECK_ARG((((uintptr_t)param | (uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) % 16) == 0);
+    adam_segments_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(
+        segs, param, grad, exp_avg, exp_avg_sq, beta1, beta2, eps, 1.f / bias_correction1,
+        1.f / sqrtf(bias_correction2));
     GSB_LAUNCH_CHECK();
     return 0;
 }

@@ -469,6 +469,22 @@ extern "C" int gsb_sh_backward_split(int n, int degree, int degrees_to_use, cons
                               v_features_rest, cam_pos);
 }
 
+// Camera variants: the split variants' view directions (means - cam_pos, formed in the kernel) on the merged
+// [n,K,3] coefficient block of the flat parameter layout.  Same kernels and arithmetic as the split variants; only
+// the coefficient rows are moved as one span instead of two.
+extern "C" int gsb_sh_forward_rgb_cam(int n, int degree, int degrees_to_use, const float *means, const float *cam_pos,
+                                      const float *coeffs, float bias, float *rgbs, gsb_stream_t stream) {
+    GSB_CHECK_ARG(n == 0 || cam_pos);
+    return launch_sh_forward(n, degree, degrees_to_use, means, coeffs, rgbs, 1, bias, stream, 0, nullptr, cam_pos);
+}
+
+extern "C" int gsb_sh_backward_rgb_cam(int n, int degree, int degrees_to_use, const float *means,
+                                       const float *cam_pos, const float *rgbs, const float *v_rgbs, float *v_coeffs,
+                                       gsb_stream_t stream) {
+    GSB_CHECK_ARG(n == 0 || (cam_pos && rgbs));
+    return launch_sh_backward(n, degree, degrees_to_use, means, v_rgbs, v_coeffs, rgbs, stream, 0, nullptr, cam_pos);
+}
+
 // In-place gradient of clamp_min(. , 0): v_rgbs *= [rgbs > 0]  (what gsb_sh_backward_rgb does internally;
 // needed separately when the SH VJP runs in the fused multi-view kernel).
 extern "C" int gsb_mask_rgb_grad(int n, const float *rgbs, float *v_rgbs, gsb_stream_t stream) {

@@ -43,7 +43,41 @@ class Camera:
 LEARNING_RATES = {"means": 0.00016, "scales": 0.005, "quats": 0.001, "featuresDc": 0.0025, "featuresRest": 0.000125,
                   "opacities": 0.05}
 MEANS_LR_FINAL = 0.0000016
+MEANS_LR_INIT = float(torch.tensor(LEARNING_RATES["means"], dtype=torch.float64).float())   # the float lrInit
 PARAM_NAMES = ("means", "scales", "quats", "featuresDc", "featuresRest", "opacities")
+
+
+def downscale_factor(step, num_downscales, resolution_schedule):
+    """Model::getDownscaleFactor (model.cpp:227-229)."""
+    return int(2 ** max(num_downscales - step // resolution_schedule, 0))
+
+
+def means_learning_rate(step, max_steps, lr_init):
+    """OptimScheduler::step for the means (optim_scheduler.cpp:4-12): log-linear decay from lr_init (the float
+    learning rate the optimizer was built with) to 1.6e-6 at max_steps."""
+    t = max(min(float(step) / float(max_steps), 1.0), 0.0)
+    return math.exp(math.log(lr_init) * (1.0 - t) + math.log(MEANS_LR_FINAL) * t)
+
+
+def camera_setup(cam, downscale):
+    """The camera block of Model::forward (model.cpp:120-142) at a downscale factor: returns (height, width,
+    (fx, fy, cx, cy), view [4,4], proj [4,4], cam_pos [3]), the three tensors on the host.  The caller forms the
+    full projection as `proj @ view` on the device."""
+    sf = float(downscale)
+    fx, fy, cx, cy = cam.fx / sf, cam.fy / sf, cam.cx / sf, cam.cy / sf
+    height, width = int(float(cam.height) / sf), int(float(cam.width) / sf)
+    c2w = cam.camToWorld
+    R = c2w[:3, :3] @ torch.diag(torch.tensor([1.0, -1.0, -1.0]))     # flip y/z to gsplat conventions
+    T = c2w[:3, 3:4]
+    Rinv = R.t()
+    Tinv = (-Rinv) @ T
+    view = torch.eye(4)
+    view[:3, :3] = Rinv
+    view[:3, 3:4] = Tinv
+    fov_x = 2.0 * math.atan(width / (2.0 * fx))
+    fov_y = 2.0 * math.atan(height / (2.0 * fy))
+    proj = projection_matrix(0.001, 1000.0, fov_x, fov_y, "cpu")
+    return height, width, (fx, fy, cx, cy), view, proj, T.reshape(3)
 
 
 class GaussianModel:
@@ -72,7 +106,7 @@ class GaussianModel:
     # ---- optimizers: six Adam instances with the reference's learning rates, fused kernel per tensor ----------
     def setup_optimizers(self):
         self.lr = dict(LEARNING_RATES)
-        self.lr_init_means = float(torch.tensor(LEARNING_RATES["means"], dtype=torch.float64).float())  # float lrInit
+        self.lr_init_means = MEANS_LR_INIT
         self.adam_m = {k: torch.zeros_like(getattr(self, k)) for k in PARAM_NAMES}
         self.adam_v = {k: torch.zeros_like(getattr(self, k)) for k in PARAM_NAMES}
         self.adam_t = 0
@@ -105,32 +139,17 @@ class GaussianModel:
 
     def schedulers_step(self, step):
         """OptimScheduler::step for the means (optim_scheduler.cpp:4-12): log-linear decay to 1.6e-6 at maxSteps."""
-        t = max(min(float(step) / float(self.cfg.max_steps), 1.0), 0.0)
-        self.lr["means"] = math.exp(math.log(self.lr_init_means) * (1.0 - t) + math.log(MEANS_LR_FINAL) * t)
+        self.lr["means"] = means_learning_rate(step, self.cfg.max_steps, self.lr_init_means)
 
     def get_downscale_factor(self, step):
-        return int(2 ** max(self.numDownscales - step // self.resolutionSchedule, 0))
+        return downscale_factor(step, self.numDownscales, self.resolutionSchedule)
 
     # ---- Model::forward (model.cpp:83-225) ------------------------------------------------------------------
     def forward(self, cam, step):
         dev = self.device
-        sf = float(self.get_downscale_factor(step))
-        fx, fy, cx, cy = cam.fx / sf, cam.fy / sf, cam.cx / sf, cam.cy / sf
-        height, width = int(float(cam.height) / sf), int(float(cam.width) / sf)
-        c2w = cam.camToWorld
-        R = c2w[:3, :3] @ torch.diag(torch.tensor([1.0, -1.0, -1.0]))     # flip y/z to gsplat conventions
-        T = c2w[:3, 3:4]
-        Rinv = R.t()
-        Tinv = (-Rinv) @ T
+        height, width, (fx, fy, cx, cy), view, proj, cam_pos = camera_setup(cam, self.get_downscale_factor(step))
         self.lastHeight, self.lastWidth = height, width
-        view = torch.eye(4)
-        view[:3, :3] = Rinv
-        view[:3, 3:4] = Tinv
-        view = view.to(dev)
-        fov_x = 2.0 * math.atan(width / (2.0 * fx))
-        fov_y = 2.0 * math.atan(height / (2.0 * fy))
-        proj = projection_matrix(0.001, 1000.0, fov_x, fov_y, dev)
-        cam_pos = T.reshape(3).to(dev)
+        view, proj, cam_pos = view.to(dev), proj.to(dev), cam_pos.to(dev)
         tb = ops.tile_bounds(width, height)
         # model.cpp:148-150,200 inside the projection: exp(scales), quaternion normalisation, sigmoid(opacities)
         xys, depths, radii, conics, num_tiles_hit, _, opac = ops.ProjectGaussiansActivated.apply(

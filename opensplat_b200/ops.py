@@ -187,11 +187,13 @@ class BinPlan:
     high-water marks with headroom) so that a frame needs no host read-back before its kernels are enqueued:
     the kernels are sized by these capacities, raise stats[2] if a frame outgrows them, and the host checks the
     (asynchronous) read-back after enqueuing the whole forward pass.  One instance per device (operator layer) or
-    per pipeline."""
+    per pipeline.  After wait(), `visible` holds stats[3]: the frame's count of Gaussians with radii > 0 when the
+    binning was asked for it (GSB_BIN_COUNT_VISIBLE), else 0."""
 
     def __init__(self):
         self.m_cap = 0
         self.len_cap = 0
+        self.visible = 0
         self.host = None   # pinned int32[4]
         self.event = None
 
@@ -218,7 +220,7 @@ class BinPlan:
 
     def wait(self):
         self.event.synchronize()
-        m, max_len, overflow, _ = (int(v) for v in self.host.tolist())
+        m, max_len, overflow, self.visible = (int(v) for v in self.host.tolist())
         return m, max_len, bool(overflow)
 
 
@@ -233,10 +235,14 @@ def _plan_for(device):
     return p
 
 
+BIN_COUNT_VISIBLE = 2   # GSB_BIN_COUNT_VISIBLE (include/gsplat_b200.h)
+
+
 def bucket_tile_ranges(xys, radii, conics, colors, opacities, tile_bounds_, m_capacity, len_capacity, cull=True,
-                       workspace=None):
+                       workspace=None, count_visible=False):
     """Fast-path phase 1: per-Gaussian attribute records (kept in the workspace), cum_tiles_hit [n], tile_bins
-    [T,2] and the device stats {M, longest tile list, overflow, 0}, without sorting and without a read-back."""
+    [T,2] and the device stats {M, longest tile list, overflow, visible}, without sorting and without a read-back.
+    visible (the count of radii > 0) is 0 unless count_visible."""
     n = xys.shape[0]
     T = tile_bounds_[0] * tile_bounds_[1]
     L = capi.lib()
@@ -252,7 +258,8 @@ def bucket_tile_ranges(xys, radii, conics, colors, opacities, tile_bounds_, m_ca
     stats = _empty((4,), torch.int32, xys)
     capi.check(L.gsb_bucket_tile_ranges(
         n, capi.ptr(capi.f32(xys)), capi.ptr(radii.contiguous()), capi.ptr(capi.f32(conics)),
-        capi.ptr(capi.f32(colors)), capi.ptr(capi.f32(opacities)), 1 if cull else 0, tile_bounds_[0],
+        capi.ptr(capi.f32(colors)), capi.ptr(capi.f32(opacities)),
+        (1 if cull else 0) | (BIN_COUNT_VISIBLE if count_visible else 0), tile_bounds_[0],
         tile_bounds_[1], m_capacity, len_capacity, workspace.data_ptr() + off, workspace.numel() - off,
         capi.ptr(cum), capi.ptr(bins), capi.ptr(order), capi.ptr(stats), capi.stream()))
     bins.tile_order = order

@@ -21,24 +21,15 @@ from .parallel import flat_layout
 
 class SplatPipeline:
     def __init__(self, n, W, H, sh_degree=3, device="cuda:0", m_capacity=None, stage_timing=False):
-        self.n, self.W, self.H, self.deg = int(n), int(W), int(H), int(sh_degree)
+        self.n, self.deg = int(n), int(sh_degree)
         self.K = num_sh_bases(sh_degree)
         self.dev = torch.device(device)
-        self.tb = tile_bounds(W, H)
-        self.T = self.tb[0] * self.tb[1]
         self.L = capi.lib()
         d, f32, i32 = self.dev, torch.float32, torch.int32
         self._alloc_gaussians(self.n)
-        # ---- per-pixel ----
-        self.out_img = torch.empty((H, W, 3), dtype=f32, device=d)
-        self.final_Ts = torch.empty((H, W), dtype=f32, device=d)
-        self.final_idx = torch.empty((H, W), dtype=i32, device=d)
-        self.v_img = torch.empty((H, W, 3), dtype=f32, device=d)
-        self.target = torch.zeros((H, W, 3), dtype=f32, device=d)
+        self._alloc_pixels(W, H)
         self.background = torch.zeros(3, dtype=f32, device=d)
         self.loss = torch.zeros(1, dtype=f32, device=d)
-        self.tile_bins = torch.empty((self.T, 2), dtype=i32, device=d)
-        self.tile_order = torch.empty((self.T,), dtype=i32, device=d)   # longest-first tile order (fast path)
         self.stats_dev = torch.zeros(4, dtype=i32, device=d)
         self.plan = BinPlan()   # capacities of the M-dependent buffers, carried from frame to frame
         # ---- camera ----
@@ -94,6 +85,23 @@ class SplatPipeline:
         self.v_rgbs = torch.empty((n, 3), dtype=f32, device=d)
         self.max_len = 0
         self.m_cap = -1   # the M-sized buffers (and the n-sized bucket workspace) are (re)built by the next forward
+
+    def _alloc_pixels(self, W, H):
+        """(Re)allocates everything sized by the image: the per-pixel buffers and the per-tile bins.  Called by
+        __init__ and when a trainer's downscale schedule changes the render resolution."""
+        self.W, self.H = int(W), int(H)
+        self.tb = tile_bounds(self.W, self.H)
+        self.T = self.tb[0] * self.tb[1]
+        d, f32, i32 = self.dev, torch.float32, torch.int32
+        H, W = self.H, self.W
+        self.out_img = torch.empty((H, W, 3), dtype=f32, device=d)
+        self.final_Ts = torch.empty((H, W), dtype=f32, device=d)
+        self.final_idx = torch.empty((H, W), dtype=i32, device=d)
+        self.v_img = torch.empty((H, W, 3), dtype=f32, device=d)
+        self.target = torch.zeros((H, W, 3), dtype=f32, device=d)
+        self.tile_bins = torch.empty((self.T, 2), dtype=i32, device=d)
+        self.tile_order = torch.empty((self.T,), dtype=i32, device=d)   # longest-first tile order (fast path)
+        self.m_cap = -1   # the bucket workspace is sized by the tile count: rebuilt by the next frame
 
     def _alloc_grad_flat(self, numel):
         """The flat gradient buffer; multigpu.ViewParallelExchange re-binds it to symmetric (peer-mapped) memory."""
@@ -169,6 +177,15 @@ class SplatPipeline:
                                          P(self.projmat), fx, fy, cx, cy, H, W, self.tb[0], self.tb[1], 0.01,
                                          P(self.cov3d), P(self.xys), P(self.depths), P(self.radii), P(self.conics),
                                          P(self.nth), s))
+        return self._bin_blend(p["opacities"], 0)
+
+    def _bin_blend(self, opacities, flags, count_visible=False):
+        """Binning, packing and the blend kernel of one frame (after SH colour and projection), with the frame's one
+        host wait.  opacities: the [n] opacities the blend uses; flags: gsb_rasterize_forward_packed's;
+        count_visible: have the binning count the Gaussians with radii > 0 into self.plan.visible."""
+        L, P, s = self.L, capi.ptr, capi.stream()
+        n, W, H = self.n, self.W, self.H
+        bin_flags = 1 | (ops.BIN_COUNT_VISIBLE if count_visible else 0)
         limit = L.gsb_bucket_max_tile_len()
         plan = self.plan
         # Everything below is sized by capacities planned from earlier frames and enqueued WITHOUT waiting for the
@@ -183,7 +200,8 @@ class SplatPipeline:
             self._stage("scan")
             # cull = 1: bin only (Gaussian, tile) pairs whose extent box touches the tile
             capi.check(L.gsb_bucket_tile_ranges(n, P(self.xys), P(self.radii), P(self.conics), P(self.rgbs),
-                                                P(p["opacities"]), 1, self.tb[0], self.tb[1], m_cap, len_cap, wsp, wsb,
+                                                P(opacities), bin_flags, self.tb[0], self.tb[1], m_cap, len_cap, wsp,
+                                                wsb,
                                                 P(self.cum), P(self.tile_bins), P(self.tile_order), P(self.stats_dev),
                                                 s))
             plan.read_back(self.stats_dev)
@@ -196,7 +214,7 @@ class SplatPipeline:
             capi.check(L.gsb_rasterize_forward_packed(H, W, self.tb[0], self.tb[1], m_cap, P(self.tile_bins),
                                                       P(self.tile_order), P(self.stats_dev), P(self.background),
                                                       P(self.records), P(self.out_img), P(self.final_Ts),
-                                                      P(self.final_idx), 0, s))
+                                                      P(self.final_idx), flags, s))
             self._stage("end_fwd")
             self.m, self.max_len, overflow = plan.wait()
             if not overflow:
@@ -219,10 +237,10 @@ class SplatPipeline:
             n, m, self.xys, self.depths, self.radii, self.cum, self.tb, return_index=True)
         self._stage("raster_fwd")
         capi.check(L.gsb_pack_records(m, P(gids_sorted), P(sorted_index), P(self.xys), P(self.conics), P(self.rgbs),
-                                      P(p["opacities"]), P(self.records), s))
+                                      P(opacities), P(self.records), s))
         capi.check(L.gsb_rasterize_forward_packed(H, W, self.tb[0], self.tb[1], m, P(self.tile_bins), None, None,
                                                   P(self.background), P(self.records), P(self.out_img),
-                                                  P(self.final_Ts), P(self.final_idx), 0, s))
+                                                  P(self.final_Ts), P(self.final_idx), flags, s))
         self.m_raster = m
         self._ordered = False
         self._stage("end_fwd")

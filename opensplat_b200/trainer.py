@@ -1,0 +1,203 @@
+"""One step of the reference's training loop (opensplat.cpp:151-170: Model::forward, mainLoss, backward,
+optimizersStep, schedulersStep, afterTrain) over the flat parameter / gradient / Adam-moment buffers of
+pipeline.SplatPipeline, without autograd:
+
+    trainer = SplatTrainer(params, cfg)        # the arguments of model.GaussianModel
+    for step in range(1, steps + 1):
+        loss = trainer.step(cam, gt, step)     # device tensor {total, L1, SSIM}; never read on the host here
+
+It runs the kernels model.GaussianModel runs, in the same order, with the same camera and learning-rate code, so the
+two follow the same trajectory (same Gaussian counts, losses to rounding; the segmented Adam rounds the parameter
+step of some floats differently from gsb_adam_step, see include/gsplat_b200.h).  What changes is the bookkeeping
+around them: one segmented Adam launch instead of six, no autograd nodes, and one host wait per step (the binning read-back, whose stats[3] visible count replaces the
+`radii.sum() == 0` test of model.cpp:173).  Between refinements a step allocates no device memory; a refinement
+(densify.Densifier, unchanged) re-creates the flat layout through SplatPipeline.resize_gaussians.
+Single process only."""
+import ctypes as C
+
+import torch
+
+from . import capi, ops
+from .densify import Densifier, RefineConfig
+from .export import SceneWriter
+from .model import LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, camera_setup, downscale_factor, means_learning_rate
+from .parallel import flat_views
+from .pipeline import SplatPipeline
+
+
+def adam_segments(offs, lr):
+    """Segment table of gsb_adam_step_segments for the flat layout `offs` (parallel.flat_layout) and the reference's
+    six learning rates `lr` (keyed like model.LEARNING_RATES): one (offset, count, row_floats, head_floats, lr_head,
+    lr_rest) per slice.  The merged SH block [n,K,3] gives featuresDc the first 3 floats of every 3K-float row and
+    featuresRest the rest."""
+    segs = []
+    for name, (o, c, shp) in offs.items():
+        row = 1
+        for d in shp[1:]:
+            row *= d
+        if name == "coeffs":
+            segs.append((o, c, row, 3, lr["featuresDc"], lr["featuresRest"]))
+        else:
+            segs.append((o, c, row, row, lr[name], lr[name]))
+    return segs
+
+
+def _split_coeffs(views):
+    """Copies of the reference's six tensors from flat-layout views (featuresDc / featuresRest cut out of coeffs)."""
+    c = views["coeffs"]
+    out = {k: views[k].clone() for k in ("means", "scales", "quats", "opacities")}
+    out["featuresDc"] = c[:, 0, :].clone(memory_format=torch.contiguous_format)
+    out["featuresRest"] = c[:, 1:, :].clone(memory_format=torch.contiguous_format)
+    return {k: out[k] for k in PARAM_NAMES}
+
+
+class SplatTrainer:
+    def __init__(self, params, cfg=None, sh_degree=None, sh_degree_interval=1000, num_downscales=0,
+                 resolution_schedule=3000, background=(0.6130, 0.0101, 0.3984), device="cuda:0", generator=None,
+                 ssim_weight=0.2, m_capacity=None):
+        """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
+        featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
+        m_capacity: initial intersection capacity of the binning buffers (grown on demand)."""
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            raise RuntimeError("SplatTrainer runs in one process: data-parallel training needs the SH degree schedule "
+                               "passed through multigpu.ViewParallelExchange first; use model.GaussianModel under a "
+                               "process group")
+        self.device = torch.device(device)
+        self.cfg = cfg or RefineConfig()
+        t = {k: torch.as_tensor(params[k]).to(device=self.device, dtype=torch.float32) for k in PARAM_NAMES}
+        n, k_bases = t["means"].shape[0], t["featuresRest"].shape[1] + 1
+        self.sh_degree = ops.deg_from_sh(k_bases) if sh_degree is None else int(sh_degree)
+        self.sh_degree_interval = int(sh_degree_interval)
+        self.num_downscales, self.resolution_schedule = int(num_downscales), int(resolution_schedule)
+        self.ssim_weight = float(ssim_weight)
+        # the image size is known from the first camera: the pipeline starts with one-tile placeholder buffers
+        self.pipe = pp = SplatPipeline(n, 16, 16, sh_degree=ops.deg_from_sh(k_bases), device=self.device,
+                                       m_capacity=m_capacity)
+        for k in ("means", "scales", "quats"):
+            pp.p[k].copy_(t[k])
+        pp.p["opacities"].copy_(t["opacities"].reshape(n, 1))
+        pp.p["coeffs"][:, 0, :].copy_(t["featuresDc"])
+        pp.p["coeffs"][:, 1:, :].copy_(t["featuresRest"])
+        pp.adam_m = torch.zeros_like(pp.param_flat)
+        pp.adam_v = torch.zeros_like(pp.param_flat)
+        pp.background.copy_(torch.tensor(background, dtype=torch.float32))
+        self.L = capi.lib()
+        self.lr = dict(LEARNING_RATES)
+        self.densifier = Densifier(self.cfg, generator=generator)
+        # camera: view [16], proj [16], cam_pos [3], uploaded from one pinned staging buffer per step
+        self.cam_host = torch.zeros(35, dtype=torch.float32).pin_memory()
+        self.cam_dev = torch.zeros(35, dtype=torch.float32, device=self.device)
+        self.viewmat = self.cam_dev[:16].view(4, 4)
+        self.proj = self.cam_dev[16:32].view(4, 4)
+        self.cam_pos = self.cam_dev[32:35]
+        self.projmat = torch.zeros((4, 4), dtype=torch.float32, device=self.device)
+        self.loss = torch.zeros(3, dtype=torch.float32, device=self.device)
+        self.resolution = None
+        self.pixel_reallocs = 0   # resolution changes after the first step (the downscale schedule)
+        self.writer = None
+        self.last_info = {"refined": False}
+        self._alloc_gaussian_scratch()
+
+    def _alloc_gaussian_scratch(self):
+        n = self.pipe.n
+        self.opac = torch.empty(n, dtype=torch.float32, device=self.device)     # sigmoid(logits) for the blend
+        self.v_opac = torch.empty(n, dtype=torch.float32, device=self.device)   # blend gradient w.r.t. it
+
+    def _set_resolution(self, W, H):
+        if self.resolution is not None:
+            self.pixel_reallocs += 1
+        self.resolution = (W, H)
+        self.pipe._alloc_pixels(W, H)
+        self.ssim_ws = torch.empty(self.L.gsb_ssim_workspace_bytes(H, W) + 256, dtype=torch.uint8, device=self.device)
+
+    @property
+    def n(self):
+        return self.pipe.n
+
+    @property
+    def image(self):
+        """The image of the last step ([H,W,3], clamped to 1; the background where nothing was visible)."""
+        return self.pipe.out_img
+
+    def params(self):
+        """Copies of the reference's six tensors."""
+        return _split_coeffs(self.pipe.p)
+
+    def adam_state(self):
+        """(exp_avg, exp_avg_sq): copies keyed like params()."""
+        pp = self.pipe
+        return _split_coeffs(flat_views(pp.adam_m, pp.offs)), _split_coeffs(flat_views(pp.adam_v, pp.offs))
+
+    def step(self, cam, gt, step):
+        """One training step at `step` (1-based, as opensplat.cpp counts).  cam: model.Camera; gt: [H,W,3] fp32 CUDA
+        image at this step's render resolution.  Returns the device tensor {total, L1, SSIM}, which the next step
+        overwrites."""
+        pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
+        H, W, (fx, fy, cx, cy), view, proj, cam_pos = camera_setup(
+            cam, downscale_factor(step, self.num_downscales, self.resolution_schedule))
+        if (W, H) != self.resolution:
+            self._set_resolution(W, H)
+        if gt.dtype != torch.float32 or tuple(gt.shape) != (H, W, 3):
+            raise ValueError(f"gt must be a float32 [{H},{W},3] image (this step's render resolution)")
+        # The previous step's host wait came after this buffer's last upload, so it can be rewritten.
+        self.cam_host[:16].copy_(view.reshape(16))
+        self.cam_host[16:32].copy_(proj.reshape(16))
+        self.cam_host[32:35].copy_(cam_pos)
+        self.cam_dev.copy_(self.cam_host, non_blocking=True)
+        torch.matmul(self.proj, self.viewmat, out=self.projmat)   # `proj @ view`, on the device like GaussianModel
+        n, p, g = pp.n, pp.p, pp.g
+        tb = pp.tb
+        use = min(step // self.sh_degree_interval, self.sh_degree)
+        # ---- forward, enqueued without a host wait until the binning read-back ----
+        capi.check(L.gsb_sh_forward_rgb_cam(n, pp.deg, use, P(p["means"]), P(self.cam_pos), P(p["coeffs"]), 0.5,
+                                            P(pp.rgbs), s))
+        capi.check(L.gsb_project_forward_activated(
+            n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmat),
+            P(self.projmat), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
+            P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac), s))
+        pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True)
+        off = (-self.ssim_ws.data_ptr()) % 256
+        capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(self.loss),
+                                      self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off, s))
+        info = {"refined": False}
+        if pp.plan.visible > 0:   # model.cpp:173-174: a view that hits nothing trains nothing
+            # ---- backward ----
+            capi.check(L.gsb_rasterize_backward(
+                H, W, tb[0], tb[1], n, pp.m_raster, P(pp.tile_bins), P(pp.tile_order) if pp._ordered else None,
+                P(pp.conics), P(self.opac), P(pp.records), P(pp.cum), P(pp.background), P(pp.final_Ts),
+                P(pp.final_idx), P(pp.v_img), None, P(pp.grad_rows), P(pp.v_xy), P(pp.v_conic), P(pp.v_rgbs),
+                P(self.v_opac), ops.CLAMP_MAX_ONE, s))
+            capi.check(L.gsb_project_backward_activated(
+                n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(self.opac), P(self.viewmat), P(self.projmat),
+                fx, fy, H, W, P(pp.radii), P(pp.conics), P(pp.v_xy), None, P(pp.v_conic), P(self.v_opac),
+                P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]), s))
+            capi.check(L.gsb_sh_backward_rgb_cam(n, pp.deg, use, P(p["means"]), P(self.cam_pos), P(pp.rgbs),
+                                                 P(pp.v_rgbs), P(g["coeffs"]), s))
+            # ---- the six optimizers in one launch (torch.optim.Adam defaults, as GaussianModel.optimizers_step) ----
+            pp.adam_t += 1
+            t = pp.adam_t
+            segs = adam_segments(pp.offs, self.lr)
+            table = (capi.AdamSegment * len(segs))(*[capi.AdamSegment(*sg) for sg in segs])
+            capi.check(L.gsb_adam_step_segments(len(segs), C.addressof(table), P(pp.param_flat), P(pp.grad_flat),
+                                                P(pp.adam_m), P(pp.adam_v), 0.9, 0.999, 1e-8, 1.0 - 0.9 ** t,
+                                                1.0 - 0.999 ** t, s))
+        self.lr["means"] = means_learning_rate(step, self.cfg.max_steps, MEANS_LR_INIT)
+        if pp.plan.visible > 0:
+            # ---- Model::afterTrain on views into the flat buffers ----
+            new_p, new_m, new_v, info = self.densifier.after_train(
+                step, pp.p, flat_views(pp.adam_m, pp.offs), flat_views(pp.adam_v, pp.offs), pp.v_xy, pp.radii, H, W)
+            if new_p is not pp.p:   # the Gaussian set changed: the only allocations of a step
+                pp.resize_gaussians(new_p, new_m, new_v)
+                self._alloc_gaussian_scratch()
+        self.last_info = info
+        return self.loss
+
+    # ---- Model::save (model.cpp:496-594) -----------------------------------------------------------------------
+    def save(self, filename, step=0, keep_crs=False, scale=1.0, translation=(0.0, 0.0, 0.0), wait=True):
+        """Writes the scene as GaussianModel.save does, packing the rows straight from the flat buffer."""
+        if self.writer is None:
+            self.writer = SceneWriter(self.device)
+        self.writer.save(filename, dict(self.pipe.p), step, keep_crs, scale, translation)
+        if wait:
+            self.writer.wait()
