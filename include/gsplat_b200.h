@@ -113,6 +113,19 @@ int gsb_exchange_gradients(int n, int degree, int degrees_to_use, const float *m
                            const float *cam_positions, const float *const *v_rgbs_per_view, float scale,
                            float *v_coeffs, int rank, int world, long long geom_floats,
                            float *const *geom_per_rank, float *geom_multicast, gsb_stream_t stream);
+/* Per-step camera centres: gsb_sh_backward_multiview / gsb_exchange_gradients with view r's centre read from
+ *   cam_pos_per_view[r] instead of cam_positions[r].  cam_pos_per_view is a DEVICE array of num_views device pointers
+ *   to 3 floats each; like v_rgbs_per_view, entries may be peer-mapped, so a data-parallel trainer whose ranks render
+ *   a different camera every step exposes each step's centre next to its colour gradient (written before the
+ *   caller's first barrier) instead of gathering the centres with a collective.  Same arguments, checks and results
+ *   otherwise: given the same centres the coefficient gradients are bit-identical to the two entry points above. */
+int gsb_sh_backward_multiview_cams(int n, int degree, int degrees_to_use, const float *means, int num_views,
+                                   const float *const *cam_pos_per_view, const float *const *v_rgbs_per_view,
+                                   float scale, float *v_coeffs, gsb_stream_t stream);
+int gsb_exchange_gradients_cams(int n, int degree, int degrees_to_use, const float *means, int num_views,
+                                const float *const *cam_pos_per_view, const float *const *v_rgbs_per_view,
+                                float scale, float *v_coeffs, int rank, int world, long long geom_floats,
+                                float *const *geom_per_rank, float *geom_multicast, gsb_stream_t stream);
 
 /* ---- Projection ------------------------------------------------------------------------------
  * gsb_project_forward replaces project_gaussians_forward_tensor (bindings.h:42-65,

@@ -29,6 +29,9 @@ _SIGS = {
     "gsb_mask_rgb_grad": (_i, [_i, _vp, _vp, _vp]),
     "gsb_sh_backward_multiview": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _vp]),
     "gsb_exchange_gradients": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _i, _i, C.c_longlong, _vp, _vp, _vp]),
+    "gsb_sh_backward_multiview_cams": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _vp]),
+    "gsb_exchange_gradients_cams": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _i, _i, C.c_longlong, _vp, _vp,
+                                         _vp]),
     "gsb_project_forward": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i, _i, _i, _f,
                                  _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_project_backward": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i,

@@ -7,6 +7,8 @@
 // moves its 128 Gaussians' coefficients as one contiguous span with 128-bit streaming accesses
 // (fully coalesced, L1 bypassed) through a padded shared-memory transpose; rows are padded to
 // 4*odd floats so the per-thread 128-bit row reads are bank-conflict free.
+#include <type_traits>
+
 #include "gsb_common.cuh"
 
 int gsb_sm_count();
@@ -220,6 +222,18 @@ sh_backward_kernel(int n, int degrees_to_use, const float *__restrict__ viewdirs
 // multimem.ld_reduce pulls the sum of all ranks' copies through the switch and one multimem.st broadcasts the
 // result to every rank; without multicast the slice is summed from / written to the peers' mapped pointers.
 // The caller brackets the launch with two cross-rank barriers (inputs complete / results visible).
+//
+// Camera centres: PEER_CAMS = false reads view r's centre from a device [num_views,3] array (fixed when the exchange
+// is built); PEER_CAMS = true from cam_pos[r], a device array of num_views pointers to 3 floats each that may be
+// peer-mapped like v_rgb_views -- a trainer renders a different camera on every rank at every step, and each rank
+// exposes this step's centre next to its colour gradient instead of gathering the centres with a collective.  Role A
+// stages a batch's VB centres in shared memory once per CTA (3 x VB threads, one float each) so that the 128 threads
+// of a CTA do not all load the same peer address, and every thread reads them into registers before the expansion:
+// read inside the expansion loop instead, ptxas contracts three of the K = 16 basis' multiply-subtract pairs into
+// FMAs differently from the PEER_CAMS = false kernel, and the gradients are no longer bit-identical to it.
+template <bool PEER_CAMS>
+using MvCamPos = typename std::conditional<PEER_CAMS, const float *const *, const float *>::type;
+
 __device__ __forceinline__ float4 multimem_ld_reduce_add(const float *mc_ptr) {
     float4 v;
     asm volatile("multimem.ld_reduce.relaxed.sys.global.add.v4.f32 {%0,%1,%2,%3}, [%4];"
@@ -233,10 +247,10 @@ __device__ __forceinline__ void multimem_st(float *mc_ptr, float4 v) {
 
 constexpr int MV_MAX_RANKS = 16;   // peers the non-multicast all-reduce role can address
 
-template <int K>
+template <int K, bool PEER_CAMS>
 __global__ void __launch_bounds__(SH_THREADS)
 sh_backward_multiview_kernel(int n, int degrees_to_use, const float *__restrict__ means, int num_views,
-                             const float *__restrict__ cam_pos, const float *const *__restrict__ v_rgb_views,
+                             MvCamPos<PEER_CAMS> __restrict__ cam_pos, const float *const *__restrict__ v_rgb_views,
                              float scale, float *__restrict__ v_coeffs, int vec_ok,
                              // ---- all-reduce role (geom_blocks == 0: none) ----
                              int geom_blocks, int rank, int world, long long geom_vec4,
@@ -285,6 +299,7 @@ sh_backward_multiview_kernel(int n, int degrees_to_use, const float *__restrict_
     // ---- role A: multi-view SH VJP with peer pulls ----
     __shared__ __align__(16) float tile[SH_THREADS * S];
     __shared__ float stage[VB][3 * SH_THREADS];
+    __shared__ float cam_stage[3 * VB];          // PEER_CAMS: this batch's camera centres
     const int blk = (int)blockIdx.x - geom_blocks;
     const int g0 = blk * SH_THREADS;
     const int ng = min(SH_THREADS, n - g0);
@@ -311,12 +326,26 @@ sh_backward_multiview_kernel(int n, int degrees_to_use, const float *__restrict_
                     if (t + q * SH_THREADS < span) pull[u][q] = vr[t + q * SH_THREADS];
             }
         }
+        float cam_pull = 0.f;
+        if constexpr (PEER_CAMS) {
+            if (t < 3 * VB && r0 + t / 3 < num_views) cam_pull = cam_pos[r0 + t / 3][t % 3];   // local or peer-mapped
+        }
         __syncthreads();   // the previous batch has been consumed
 #pragma unroll
         for (int u = 0; u < VB; ++u)
 #pragma unroll
             for (int q = 0; q < 3; ++q) stage[u][t + q * SH_THREADS] = pull[u][q];
+        if constexpr (PEER_CAMS) {
+            if (t < 3 * VB) cam_stage[t] = cam_pull;
+        }
         __syncthreads();
+        float cam_x[VB], cam_y[VB], cam_z[VB];   // PEER_CAMS: the batch's centres, read from shared memory once
+        if constexpr (PEER_CAMS) {
+#pragma unroll
+            for (int u = 0; u < VB; ++u) {
+                cam_x[u] = cam_stage[3 * u]; cam_y[u] = cam_stage[3 * u + 1]; cam_z[u] = cam_stage[3 * u + 2];
+            }
+        }
         if (t < ng) {
 #pragma unroll
             for (int u = 0; u < VB; ++u) {
@@ -325,8 +354,11 @@ sh_backward_multiview_kernel(int n, int degrees_to_use, const float *__restrict_
                 if (v0 == 0.f && v1 == 0.f && v2 == 0.f) continue;  // not visible in this view
                 const int r = r0 + u;
                 float Y[K];
-                sh_basis(nb, mx - __ldg(cam_pos + 3 * r), my - __ldg(cam_pos + 3 * r + 1),
-                         mz - __ldg(cam_pos + 3 * r + 2), Y);
+                if constexpr (PEER_CAMS)
+                    sh_basis(nb, mx - cam_x[u], my - cam_y[u], mz - cam_z[u], Y);
+                else
+                    sh_basis(nb, mx - __ldg(cam_pos + 3 * r), my - __ldg(cam_pos + 3 * r + 1),
+                             mz - __ldg(cam_pos + 3 * r + 2), Y);
 #pragma unroll
                 for (int b = 0; b < K; ++b) {
                     if (b < nb) {
@@ -497,8 +529,9 @@ extern "C" int gsb_mask_rgb_grad(int n, const float *rgbs, float *v_rgbs, gsb_st
     return 0;
 }
 
+template <bool PEER_CAMS>
 static int launch_multiview(int n, int degree, int degrees_to_use, const float *means, int num_views,
-                            const float *cam_positions, const float *const *v_rgbs_per_view, float scale,
+                            MvCamPos<PEER_CAMS> cam_positions, const float *const *v_rgbs_per_view, float scale,
                             float *v_coeffs, int rank, int world, long long geom_floats, float *const *geom_per_rank,
                             float *geom_multicast, gsb_stream_t stream) {
     GSB_CHECK_ARG(n >= 0 && bases_of_degree(degree) > 0 && degrees_to_use >= 0 && degrees_to_use <= degree);
@@ -520,7 +553,7 @@ static int launch_multiview(int n, int degree, int degrees_to_use, const float *
     cudaStream_t s = (cudaStream_t)stream;
     int grid = geom_blocks + gsb_div_up(n, SH_THREADS);
     int vec_ok = ((uintptr_t)v_coeffs % 16) == 0;
-#define GSB_SH_M(K) sh_backward_multiview_kernel<K><<<grid, SH_THREADS, 0, s>>>(n, degrees_to_use, means, num_views, cam_positions, v_rgbs_per_view, scale, v_coeffs, vec_ok, geom_blocks, rank, world, geom_floats / 4, geom_per_rank, geom_multicast)
+#define GSB_SH_M(K) sh_backward_multiview_kernel<K, PEER_CAMS><<<grid, SH_THREADS, 0, s>>>(n, degrees_to_use, means, num_views, cam_positions, v_rgbs_per_view, scale, v_coeffs, vec_ok, geom_blocks, rank, world, geom_floats / 4, geom_per_rank, geom_multicast)
     switch (degree) {
         case 0: GSB_SH_M(1); break;
         case 1: GSB_SH_M(4); break;
@@ -537,14 +570,33 @@ extern "C" int gsb_sh_backward_multiview(int n, int degree, int degrees_to_use, 
                                          int num_views, const float *cam_positions,
                                          const float *const *v_rgbs_per_view, float scale, float *v_coeffs,
                                          gsb_stream_t stream) {
-    return launch_multiview(n, degree, degrees_to_use, means, num_views, cam_positions, v_rgbs_per_view, scale,
-                            v_coeffs, 0, 1, 0, nullptr, nullptr, stream);
+    return launch_multiview<false>(n, degree, degrees_to_use, means, num_views, cam_positions, v_rgbs_per_view,
+                                   scale, v_coeffs, 0, 1, 0, nullptr, nullptr, stream);
 }
 
 extern "C" int gsb_exchange_gradients(int n, int degree, int degrees_to_use, const float *means, int num_views,
                                       const float *cam_positions, const float *const *v_rgbs_per_view, float scale,
                                       float *v_coeffs, int rank, int world, long long geom_floats,
                                       float *const *geom_per_rank, float *geom_multicast, gsb_stream_t stream) {
-    return launch_multiview(n, degree, degrees_to_use, means, num_views, cam_positions, v_rgbs_per_view, scale,
-                            v_coeffs, rank, world, geom_floats, geom_per_rank, geom_multicast, stream);
+    return launch_multiview<false>(n, degree, degrees_to_use, means, num_views, cam_positions, v_rgbs_per_view,
+                                   scale, v_coeffs, rank, world, geom_floats, geom_per_rank, geom_multicast, stream);
+}
+
+// Per-step camera centres: the two entry points above with view r's centre read from cam_pos_per_view[r] (a device
+// array of num_views device pointers to 3 floats, local or peer-mapped) instead of a [num_views,3] array.
+extern "C" int gsb_sh_backward_multiview_cams(int n, int degree, int degrees_to_use, const float *means,
+                                              int num_views, const float *const *cam_pos_per_view,
+                                              const float *const *v_rgbs_per_view, float scale, float *v_coeffs,
+                                              gsb_stream_t stream) {
+    return launch_multiview<true>(n, degree, degrees_to_use, means, num_views, cam_pos_per_view, v_rgbs_per_view,
+                                  scale, v_coeffs, 0, 1, 0, nullptr, nullptr, stream);
+}
+
+extern "C" int gsb_exchange_gradients_cams(int n, int degree, int degrees_to_use, const float *means, int num_views,
+                                           const float *const *cam_pos_per_view,
+                                           const float *const *v_rgbs_per_view, float scale, float *v_coeffs,
+                                           int rank, int world, long long geom_floats, float *const *geom_per_rank,
+                                           float *geom_multicast, gsb_stream_t stream) {
+    return launch_multiview<true>(n, degree, degrees_to_use, means, num_views, cam_pos_per_view, v_rgbs_per_view,
+                                  scale, v_coeffs, rank, world, geom_floats, geom_per_rank, geom_multicast, stream);
 }

@@ -19,6 +19,13 @@ overlap project_backward and the geometry all-reduce:
 NVLink bytes per rank per step at G ranks (N Gaussians): received (G-1) x 12 N (colour gradients) + 44 N
 (reduced slice + broadcasts), sent the same -- against 2(G-1)/G x 236 N each way for the flat all-reduce
 (G = 8: 128 MB instead of 413 MB at 1M Gaussians), and no separate sh_backward / NCCL kernels.
+
+Camera centres: by default every rank's centre is gathered once, when the exchange is built (a caller that renders
+the same view on every step, bench.py).  A trainer renders a different camera on every rank at every step: it calls
+`set_camera()` before each backward pass, which copies the step's centre into a 16-byte trailer of this rank's
+symmetric allocation, and from then on the launches use the `_cams` entry points, whose kernel reads every peer's
+centre through the peer mapping, as it reads the colour gradients -- no collective on the step.  `degrees_to_use`
+(the SH degree schedule) is passed through to the kernel; it defaults to the pipeline's full degree.
 """
 import os
 
@@ -29,17 +36,22 @@ from . import capi
 
 
 class ViewParallelExchange:
-    def __init__(self, pipe, cam_pos, group=None):
+    def __init__(self, pipe, cam_pos=None, group=None):
+        """cam_pos: this rank's fixed camera centre, gathered from every rank once here; None when the caller passes
+        each step's centre to set_camera() instead (a collective either way: every rank passes one or none)."""
         self.pipe = pipe
         self.group = group if group is not None else dist.group.WORLD
         self.world = dist.get_world_size(self.group)
         self.rank = dist.get_rank(self.group)
         dev = pipe.dev
-        # every rank's camera centre (tiny, exchanged once)
-        cp = torch.as_tensor(cam_pos, dtype=torch.float32, device=dev).reshape(1, 3)
-        allcp = [torch.zeros_like(cp) for _ in range(self.world)]
-        dist.all_gather(allcp, cp, group=self.group)
-        self.cam_positions = torch.cat(allcp, 0).contiguous()
+        self.cam_positions = None
+        if cam_pos is not None:
+            # every rank's camera centre (tiny, exchanged once)
+            cp = torch.as_tensor(cam_pos, dtype=torch.float32, device=dev).reshape(1, 3)
+            allcp = [torch.zeros_like(cp) for _ in range(self.world)]
+            dist.all_gather(allcp, cp, group=self.group)
+            self.cam_positions = torch.cat(allcp, 0).contiguous()
+        self.per_step_cams = False   # set_camera() switches the launches to the peers' per-step centres
         self.use_multicast = os.environ.get("GSB_EXCHANGE_MULTICAST", "1") != "0"
         self.overlap = os.environ.get("GSB_EXCHANGE_OVERLAP", "1") != "0"
         self.side = torch.cuda.Stream(device=dev)
@@ -49,19 +61,23 @@ class ViewParallelExchange:
     def _alloc_symmetric(self, pipe):
         import torch.distributed._symmetric_memory as symm_mem
         dev, n = pipe.dev, pipe.n
-        # ONE symmetric allocation: [flat gradient buffer | this view's colour gradient v_rgb [n,3]]
+        # ONE symmetric allocation: [flat gradient buffer | this view's colour gradient v_rgb [n,3] | this step's
+        # camera centre (3 floats of a 16-byte trailer, read by the peers once set_camera() is used)]
         rgb_off = (pipe.numel + 3) // 4 * 4
-        total = rgb_off + (3 * n + 3) // 4 * 4
+        cam_off = rgb_off + (3 * n + 3) // 4 * 4
+        total = cam_off + 4
         t = symm_mem.empty(total, dtype=torch.float32, device=dev)
         t.zero_()
         hdl = symm_mem.rendezvous(t, self.group.group_name)
         self.buf, self.hdl = t, hdl
         pipe.rebind_grad_flat(t[:pipe.numel])
         self.v_rgb = t[rgb_off:rgb_off + 3 * n].view(n, 3)
+        self.cam = t[cam_off:cam_off + 3]
         base_off = int(getattr(hdl, "offset", 0) or 0)      # the tensor's offset inside its symmetric allocation block
         ptrs = [int(p) + base_off for p in hdl.buffer_ptrs]
         self.geom_ptrs = torch.tensor(ptrs, dtype=torch.int64, device=dev)              # peers' flat buffers
         self.rgb_ptrs = torch.tensor([p + 4 * rgb_off for p in ptrs], dtype=torch.int64, device=dev)
+        self.cam_ptrs = torch.tensor([p + 4 * cam_off for p in ptrs], dtype=torch.int64, device=dev)   # peers' centres
         mc = int(getattr(hdl, "multicast_ptr", 0) or 0) if self.use_multicast else 0
         mc = mc + base_off if mc else 0
         assert ptrs[self.rank] == t.data_ptr(), "symmetric-memory handle does not describe this tensor"
@@ -80,52 +96,76 @@ class ViewParallelExchange:
         """Where this step's rasterize-backward must write its colour gradient."""
         return self.v_rgb
 
-    def start_colour(self, average=True):
+    def set_camera(self, cam_pos_dev):
+        """This step's camera centre (a device float[3]): a stream-ordered device-to-device copy into this rank's
+        trailer, no host wait, no collective.  Call it before every backward pass once it is used (a resize()
+        leaves a new, zeroed trailer).  Safe to overwrite: the previous step closed with barrier(channel=2), which
+        every rank passes only after its multi-view kernel -- the last reader of the peers' trailers -- finished."""
+        self.cam.copy_(cam_pos_dev)
+        self.per_step_cams = True
+
+    def _entry_points(self):
+        """(multi-view SH backward, fused exchange, camera-centre argument): the `_cams` entry points with the peers'
+        per-step centres once set_camera() has been called, otherwise the fixed centres gathered at construction
+        (the two pairs take the same arguments)."""
+        L = capi.lib()
+        if self.per_step_cams:
+            return L.gsb_sh_backward_multiview_cams, L.gsb_exchange_gradients_cams, self.cam_ptrs.data_ptr()
+        if self.cam_positions is None:
+            raise RuntimeError("ViewParallelExchange built without cam_pos: call set_camera() before the backward pass")
+        return L.gsb_sh_backward_multiview, L.gsb_exchange_gradients, capi.ptr(self.cam_positions)
+
+    def start_colour(self, average=True, degrees_to_use=None):
         """Call right after rasterize-backward (v_rgb is final, the geometry gradients are not yet): masks v_rgb with
         the clamp's gradient and starts the multi-view SH backward -- the part of the exchange that moves most bytes,
         (G-1) x 12 B per Gaussian -- on a side stream, so that it overlaps project_backward and, afterwards, the
-        all-reduce of the geometry gradients."""
+        all-reduce of the geometry gradients.  degrees_to_use: the SH degree schedule's (default: the full degree)."""
         p = self.pipe
         L = capi.lib()
+        multiview, _, cams = self._entry_points()
+        use = p.deg if degrees_to_use is None else int(degrees_to_use)
         self._scale = 1.0 / self.world if average else 1.0
         cur = torch.cuda.current_stream()
         capi.check(L.gsb_mask_rgb_grad(p.n, capi.ptr(p.rgbs), capi.ptr(self.v_rgb), capi.stream()))
         self._rgb_ready.record(cur)
         with torch.cuda.stream(self.side):
             self.side.wait_event(self._rgb_ready)
-            self.hdl.barrier(channel=0)          # every rank's v_rgb is complete
-            capi.check(L.gsb_sh_backward_multiview(
-                p.n, p.deg, p.deg, capi.ptr(p.p["means"]), self.world, capi.ptr(self.cam_positions),
+            self.hdl.barrier(channel=0)          # every rank's v_rgb (and camera centre) is complete
+            capi.check(multiview(
+                p.n, p.deg, use, capi.ptr(p.p["means"]), self.world, cams,
                 self.rgb_ptrs.data_ptr(), self._scale, capi.ptr(p.g["coeffs"]), self.side.cuda_stream))
             self._colour_done.record(self.side)
 
-    def finish(self):
+    def finish(self, degrees_to_use=None):
         """Call after project_backward: all-reduces the geometry gradients (two-shot; NVSwitch multimem when mapped),
         joins the colour half and closes the step with the barrier that lets every rank overwrite its buffers."""
         p = self.pipe
-        L = capi.lib()
+        _, exchange, cams = self._entry_points()
+        use = p.deg if degrees_to_use is None else int(degrees_to_use)
         self.hdl.barrier(channel=1)              # every rank's geometry gradients are complete
-        capi.check(L.gsb_exchange_gradients(
-            0, p.deg, p.deg, None, 1, capi.ptr(self.cam_positions), None, self._scale, None, self.rank, self.world,
+        capi.check(exchange(
+            0, p.deg, use, None, 1, cams, None, self._scale, None, self.rank, self.world,
             self.geom_numel, self.geom_ptrs.data_ptr(), self.multicast_ptr if self.multicast_ptr else None,
             capi.stream()))
         torch.cuda.current_stream().wait_event(self._colour_done)
         # every rank's slice of the reduced geometry gradients has landed everywhere, and nobody still reads the v_rgb /
-        # geometry buffers of this step (so the next backward pass may overwrite them)
+        # geometry buffers / camera trailers of this step (so the next step may overwrite them)
         self.hdl.barrier(channel=2)
 
-    def exchange(self, average=True):
+    def exchange(self, average=True, degrees_to_use=None):
         """The whole exchange after project_backward, as ONE fused launch (gsb_exchange_gradients: both CTA roles in one
         grid) between two barriers -- no overlap with the backward kernels; what callers use that cannot split the
         step (bench.py's operator-level e2e arm)."""
         p = self.pipe
         L = capi.lib()
+        _, exchange, cams = self._entry_points()
+        use = p.deg if degrees_to_use is None else int(degrees_to_use)
         scale = 1.0 / self.world if average else 1.0
         capi.check(L.gsb_mask_rgb_grad(p.n, capi.ptr(p.rgbs), capi.ptr(self.v_rgb), capi.stream()))
-        # every rank has finished writing this step's v_rgb and geometry gradients
+        # every rank has finished writing this step's v_rgb, camera centre and geometry gradients
         self.hdl.barrier(channel=0)
-        capi.check(L.gsb_exchange_gradients(
-            p.n, p.deg, p.deg, capi.ptr(p.p["means"]), self.world, capi.ptr(self.cam_positions),
+        capi.check(exchange(
+            p.n, p.deg, use, capi.ptr(p.p["means"]), self.world, cams,
             self.rgb_ptrs.data_ptr(), scale, capi.ptr(p.g["coeffs"]), self.rank, self.world, self.geom_numel,
             self.geom_ptrs.data_ptr(), self.multicast_ptr if self.multicast_ptr else None, capi.stream()))
         self.hdl.barrier(channel=2)
