@@ -89,6 +89,13 @@ int gsb_sh_forward_rgb_cam(int n, int degree, int degrees_to_use, const float *m
                            const float *coeffs, float bias, float *rgbs, gsb_stream_t stream);
 int gsb_sh_backward_rgb_cam(int n, int degree, int degrees_to_use, const float *means, const float *cam_pos,
                             const float *rgbs, const float *v_rgbs, float *v_coeffs, gsb_stream_t stream);
+/* Several camera views at once (a trainer's B views of one step): gsb_sh_forward_rgb_cam for every centre of
+ * cam_positions (device [num_views,3]) into rgbs (device [num_views,n,3], view v at rgbs + 3*n*v).  The coefficient
+ * block is read once for all views; every view's rgbs are bit-identical to a gsb_sh_forward_rgb_cam call with its
+ * centre.  num_views >= 1. */
+int gsb_sh_forward_rgb_cam_multiview(int n, int degree, int degrees_to_use, const float *means, int num_views,
+                                     const float *cam_positions, const float *coeffs, float bias, float *rgbs,
+                                     gsb_stream_t stream);
 
 /* Data-parallel training (SURVEY.md 8e): SH VJP fused with the cross-GPU gradient exchange.
  * gsb_mask_rgb_grad: v_rgbs *= [rgbs > 0] in place (gradient of the clamp, done before exposing v_rgbs).
@@ -169,6 +176,16 @@ int gsb_project_backward_activated(int n, const float *means3d, const float *log
                                    const float *v_depth, const float *v_conic, const float *v_opacity,
                                    float *v_mean3d, float *v_log_scales, float *v_raw_quats,
                                    float *v_opacity_logits, gsb_stream_t stream);
+/* gsb_project_backward_activated_acc: the same arguments and VJP, ADDED into v_mean3d, v_log_scales, v_raw_quats
+ *   and v_opacity_logits (out = out + vjp, one rounding per element; the outputs must hold valid floats) -- the sum of
+ *   the geometry gradients over a trainer's views of one step, in view order, without a separate add pass. */
+int gsb_project_backward_activated_acc(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                       const float *raw_quats, const float *opacities, const float *viewmat,
+                                       const float *projmat, float fx, float fy, int img_h, int img_w,
+                                       const int32_t *radii, const float *conics, const float *v_xy,
+                                       const float *v_depth, const float *v_conic, const float *v_opacity,
+                                       float *v_mean3d, float *v_log_scales, float *v_raw_quats,
+                                       float *v_opacity_logits, gsb_stream_t stream);
 
 /* ---- Tile binning ----------------------------------------------------------------------------
  * gsb_cumsum_tiles_hit replaces torch::cumsum(numTilesHit, 0, kInt32) (rasterize_gaussians.cpp:62).

@@ -26,6 +26,7 @@ _SIGS = {
     "gsb_sh_backward_split": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_sh_forward_rgb_cam": (_i, [_i, _i, _i, _vp, _vp, _vp, _f, _vp, _vp]),
     "gsb_sh_backward_rgb_cam": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_sh_forward_rgb_cam_multiview": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _vp]),
     "gsb_mask_rgb_grad": (_i, [_i, _vp, _vp, _vp]),
     "gsb_sh_backward_multiview": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _vp]),
     "gsb_exchange_gradients": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _f, _vp, _i, _i, C.c_longlong, _vp, _vp, _vp]),
@@ -43,6 +44,8 @@ _SIGS = {
     # v_opacity, v_means, v_log_scales, v_raw_quats, v_logits, stream
     "gsb_project_backward_activated": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
                                             _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_project_backward_activated_acc": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
+                                                _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_cumsum_workspace_bytes": (_sz, [_i]),
     "gsb_cumsum_tiles_hit": (_i, [_i, _vp, _vp, _vp, _sz, _vp]),
     "gsb_map_gaussian_to_intersects": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),

@@ -173,7 +173,9 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
 // ACT: VJP of the activating forward -- v_scale comes out w.r.t. the LOG-scales (x exp), the quaternion gradient
 // is w.r.t. the raw quaternion as always (the normalisation is inside quat_to_rotmat), and the rasterizer's opacity
 // gradient is taken through the sigmoid (x o (1 - o), from the saved activated opacity).
-template <bool ACT>
+// ACC: add this view's VJP to the four outputs (prev + vjp, one rounding each) instead of writing it -- the sum
+// over a trainer's views of one step, in view order.
+template <bool ACT, bool ACC>
 __global__ void __launch_bounds__(PJ_THREADS)
 project_backward_kernel(int n, const float *__restrict__ means3d, const float *__restrict__ scales,
                         float glob_scale, const float *__restrict__ quats,
@@ -189,7 +191,10 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
     if (i >= n) return;
     if (ACT) {
         const float o = opacities[i];
-        v_opacity_logits[i] = v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f;
+        if constexpr (ACC)
+            v_opacity_logits[i] = v_opacity_logits[i] + (v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f);
+        else
+            v_opacity_logits[i] = v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f;
     }
     float vm[3] = {0.f, 0.f, 0.f}, vs[3] = {0.f, 0.f, 0.f};
     float4 vq = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -317,9 +322,16 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
         vq = make_float4((gw - w * dot) * inv, (gx - x * dot) * inv, (gy - y * dot) * inv,
                          (gz - z * dot) * inv);
     }
-    v_mean3d[3 * i] = vm[0]; v_mean3d[3 * i + 1] = vm[1]; v_mean3d[3 * i + 2] = vm[2];
-    v_scale[3 * i] = vs[0]; v_scale[3 * i + 1] = vs[1]; v_scale[3 * i + 2] = vs[2];
-    v_quat[i] = vq;
+    if constexpr (ACC) {
+        const float4 pq = v_quat[i];
+        v_mean3d[3 * i] += vm[0]; v_mean3d[3 * i + 1] += vm[1]; v_mean3d[3 * i + 2] += vm[2];
+        v_scale[3 * i] += vs[0]; v_scale[3 * i + 1] += vs[1]; v_scale[3 * i + 2] += vs[2];
+        v_quat[i] = make_float4(pq.x + vq.x, pq.y + vq.y, pq.z + vq.z, pq.w + vq.w);
+    } else {
+        v_mean3d[3 * i] = vm[0]; v_mean3d[3 * i + 1] = vm[1]; v_mean3d[3 * i + 2] = vm[2];
+        v_scale[3 * i] = vs[0]; v_scale[3 * i + 1] = vs[1]; v_scale[3 * i + 2] = vs[2];
+        v_quat[i] = vq;
+    }
 }
 
 }  // namespace
@@ -372,7 +384,7 @@ extern "C" int gsb_project_forward_activated(int n, const float *means3d, const 
                                 conics, num_tiles_hit, opacities, stream);
 }
 
-static int project_backward_impl(bool act, int n, const float *means3d, const float *scales, float glob_scale,
+static int project_backward_impl(bool act, bool acc, int n, const float *means3d, const float *scales, float glob_scale,
                                  const float *quats, const float *opacities, const float *viewmat,
                                  const float *projmat, float fx, float fy, int img_h, int img_w,
                                  const int32_t *radii, const float *conics, const float *v_xy, const float *v_depth,
@@ -386,11 +398,11 @@ static int project_backward_impl(bool act, int n, const float *means3d, const fl
     GSB_CHECK_ARG(((uintptr_t)quats % 16) == 0 && ((uintptr_t)v_quat % 16) == 0 && ((uintptr_t)v_xy % 8) == 0);
     const float tan_fovx = (float)(0.5 * (double)img_w / (double)fx);
     const float tan_fovy = (float)(0.5 * (double)img_h / (double)fy);
-#define GSB_PJ_B(A) project_backward_kernel<A><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
+#define GSB_PJ_B(A, ACC) project_backward_kernel<A, ACC><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
         n, means3d, scales, glob_scale, quats, viewmat, projmat, fx, fy, tan_fovx, tan_fovy, img_h, img_w, radii,     \
         conics, reinterpret_cast<const float2 *>(v_xy), v_depth, v_conic, v_mean3d, v_scale,                          \
         reinterpret_cast<float4 *>(v_quat), opacities, v_opacity, v_opacity_logits)
-    if (act) GSB_PJ_B(true); else GSB_PJ_B(false);
+    if (acc) GSB_PJ_B(true, true); else if (act) GSB_PJ_B(true, false); else GSB_PJ_B(false, false);
 #undef GSB_PJ_B
     GSB_LAUNCH_CHECK();
     return 0;
@@ -403,8 +415,8 @@ extern "C" int gsb_project_backward(int n, const float *means3d, const float *sc
                                     const float *v_xy, const float *v_depth, const float *v_conic,
                                     float *v_mean3d, float *v_scale, float *v_quat, gsb_stream_t stream) {
     (void)cov3d; (void)cx; (void)cy;
-    return project_backward_impl(false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx, fy,
-                                 img_h, img_w, radii, conics, v_xy, v_depth, v_conic, nullptr, v_mean3d, v_scale,
+    return project_backward_impl(false, false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx,
+                                 fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, nullptr, v_mean3d, v_scale,
                                  v_quat, nullptr, stream);
 }
 
@@ -415,7 +427,20 @@ extern "C" int gsb_project_backward_activated(int n, const float *means3d, const
                                               const float *v_depth, const float *v_conic, const float *v_opacity,
                                               float *v_mean3d, float *v_log_scales, float *v_raw_quats,
                                               float *v_opacity_logits, gsb_stream_t stream) {
-    return project_backward_impl(true, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat, projmat, fx,
-                                 fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity, v_mean3d,
-                                 v_log_scales, v_raw_quats, v_opacity_logits, stream);
+    return project_backward_impl(true, false, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
+                                 projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
+                                 v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
+}
+
+// The same VJP added into the four outputs (v += vjp): a trainer's several views of one step summed in place.
+extern "C" int gsb_project_backward_activated_acc(int n, const float *means3d, const float *log_scales,
+                                                  float glob_scale, const float *raw_quats, const float *opacities,
+                                                  const float *viewmat, const float *projmat, float fx, float fy,
+                                                  int img_h, int img_w, const int32_t *radii, const float *conics,
+                                                  const float *v_xy, const float *v_depth, const float *v_conic,
+                                                  const float *v_opacity, float *v_mean3d, float *v_log_scales,
+                                                  float *v_raw_quats, float *v_opacity_logits, gsb_stream_t stream) {
+    return project_backward_impl(true, true, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
+                                 projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
+                                 v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
 }

@@ -6,7 +6,8 @@
 // coefficient block with one thread per Gaussian (192-B stride between lanes at K=16).  Here a CTA
 // moves its 128 Gaussians' coefficients as one contiguous span with 128-bit streaming accesses
 // (fully coalesced, L1 bypassed) through a padded shared-memory transpose; rows are padded to
-// 4*odd floats so the per-thread 128-bit row reads are bank-conflict free.
+// 4*odd floats so the per-thread 128-bit row reads are bank-conflict free.  The multi-view forward stages the span
+// once and evaluates it for several camera centres (a trainer's views of one step).
 #include <type_traits>
 
 #include "gsb_common.cuh"
@@ -22,14 +23,25 @@ __host__ __device__ constexpr int sh_row_stride(int K) {
     return 4 * ((q & 1) ? q : q + 1);
 }
 
-// SH constants, sh.cuh:12-37
+// SH constants, sh.cuh:12-37.  ROUNDED_PRODUCTS: form the six second-order products with __fmul_rn, which the compiler
+// never contracts into an FMA.  The single-view kernels compute them as separate multiplies; in the loop over views of
+// sh_forward_multiview_kernel at K >= 16 the compiler would otherwise fold x * x into the subtractions of the degree-2
+// and degree-3 bases, and its colours would no longer be bit-identical to gsb_sh_forward_rgb_cam's.  (At K = 9 the
+// plain products contract as in the single-view kernel, and the rounded ones would not.)
+template <bool ROUNDED_PRODUCTS = false>
 __device__ __forceinline__ void sh_basis(int nb, float vx, float vy, float vz, float *Y) {
     Y[0] = 0.28209479177387814f;
     if (nb <= 1) return;
     // sh.cuh:67-72 normalises the direction inside the kernel
     float norm = sqrtf(vx * vx + vy * vy + vz * vz);
     float x = vx / norm, y = vy / norm, z = vz / norm;
-    float xx = x * x, xy = x * y, xz = x * z, yy = y * y, yz = y * z, zz = z * z;
+    float xx, xy, xz, yy, yz, zz;
+    if constexpr (ROUNDED_PRODUCTS) {
+        xx = __fmul_rn(x, x); xy = __fmul_rn(x, y); xz = __fmul_rn(x, z);
+        yy = __fmul_rn(y, y); yz = __fmul_rn(y, z); zz = __fmul_rn(z, z);
+    } else {
+        xx = x * x; xy = x * y; xz = x * z; yy = y * y; yz = y * z; zz = z * z;
+    }
     Y[1] = -0.4886025119029199f * y;
     Y[2] = 0.4886025119029199f * z;
     Y[3] = -0.4886025119029199f * x;
@@ -135,6 +147,74 @@ sh_forward_kernel(int n, int degrees_to_use, const float *__restrict__ viewdirs,
     colors[3 * g] = c0;
     colors[3 * g + 1] = c1;
     colors[3 * g + 2] = c2;
+}
+
+// Multi-view forward (a trainer's B camera views of one step): rgbs[v] = clamp_min(SH(means - cam_pos[v]) + bias, 0)
+// for v < num_views.  The coefficient span of the CTA's 128 Gaussians is staged once through the same padded
+// transpose as sh_forward_kernel and held in registers across the views, so the [n,K,3] block is read once per step
+// instead of once per view.  Per view the arithmetic is sh_forward_kernel's with cam_pos (the same view direction,
+// basis and accumulation order), so every view's rgbs are bit-identical to a gsb_sh_forward_rgb_cam call.
+template <int K>
+__global__ void __launch_bounds__(SH_THREADS)
+sh_forward_multiview_kernel(int n, int degrees_to_use, const float *__restrict__ means, int num_views,
+                            const float *__restrict__ cam_pos, const float *__restrict__ coeffs, float bias,
+                            float *__restrict__ rgbs, int vec_ok) {
+    constexpr int C = 3 * K;
+    constexpr int S = sh_row_stride(K);
+    __shared__ __align__(16) float tile[SH_THREADS * S];
+    const int g0 = blockIdx.x * SH_THREADS;
+    const int ng = min(SH_THREADS, n - g0);
+    const int nb = min(nb_of(degrees_to_use), K);
+    const float *src = coeffs + (size_t)g0 * C;
+    const int total = ng * C;
+    if (vec_ok && (C % 4 == 0)) {
+        const float4 *src4 = reinterpret_cast<const float4 *>(src);
+        for (int f = threadIdx.x; f < total / 4; f += SH_THREADS) {
+            float4 v = ldg_stream4(src4 + f);
+            int e = 4 * f, g = e / C, j = e - g * C;
+            *reinterpret_cast<float4 *>(&tile[g * S + j]) = v;
+        }
+    } else {
+        for (int e = threadIdx.x; e < total; e += SH_THREADS) {
+            int g = e / C, j = e - g * C;
+            tile[g * S + j] = __ldg(src + e);
+        }
+    }
+    __syncthreads();
+    const int t = threadIdx.x;
+    if (t >= ng) return;
+    const int g = g0 + t;
+    const float mx = means[3 * g], my = means[3 * g + 1], mz = means[3 * g + 2];
+    float row[S];
+#pragma unroll
+    for (int j = 0; j < S; j += 4) {
+        float4 v = *reinterpret_cast<const float4 *>(&tile[t * S + j]);
+        row[j] = v.x; row[j + 1] = v.y; row[j + 2] = v.z; row[j + 3] = v.w;
+    }
+    for (int view = 0; view < num_views; ++view) {
+        float Y[K];
+        {
+            float vx = mx, vy = my, vz = mz;
+            vx -= __ldg(cam_pos + 3 * view); vy -= __ldg(cam_pos + 3 * view + 1); vz -= __ldg(cam_pos + 3 * view + 2);
+            sh_basis<(K >= 16)>(nb, vx, vy, vz, Y);
+        }
+        float c0 = 0.f, c1 = 0.f, c2 = 0.f;
+#pragma unroll
+        for (int b = 0; b < K; ++b) {
+            if (b < nb) {
+                c0 += Y[b] * row[3 * b];
+                c1 += Y[b] * row[3 * b + 1];
+                c2 += Y[b] * row[3 * b + 2];
+            }
+        }
+        c0 = fmaxf(c0 + bias, 0.f);
+        c1 = fmaxf(c1 + bias, 0.f);
+        c2 = fmaxf(c2 + bias, 0.f);
+        float *out = rgbs + (size_t)view * 3 * n;
+        out[3 * g] = c0;
+        out[3 * g + 1] = c1;
+        out[3 * g + 2] = c2;
+    }
 }
 
 template <int K>
@@ -515,6 +595,31 @@ extern "C" int gsb_sh_backward_rgb_cam(int n, int degree, int degrees_to_use, co
                                        gsb_stream_t stream) {
     GSB_CHECK_ARG(n == 0 || (cam_pos && rgbs));
     return launch_sh_backward(n, degree, degrees_to_use, means, v_rgbs, v_coeffs, rgbs, stream, 0, nullptr, cam_pos);
+}
+
+// Several camera views at once: gsb_sh_forward_rgb_cam for each of the num_views centres of cam_positions [V,3],
+// into rgbs [V,n,3], with one read of the coefficient block.
+extern "C" int gsb_sh_forward_rgb_cam_multiview(int n, int degree, int degrees_to_use, const float *means,
+                                                int num_views, const float *cam_positions, const float *coeffs,
+                                                float bias, float *rgbs, gsb_stream_t stream) {
+    GSB_CHECK_ARG(n >= 0 && num_views >= 1 && bases_of_degree(degree) > 0 && degrees_to_use >= 0 &&
+                  degrees_to_use <= degree);
+    if (n == 0) return 0;
+    GSB_CHECK_ARG(means && cam_positions && coeffs && rgbs);
+    cudaStream_t s = (cudaStream_t)stream;
+    int grid = gsb_div_up(n, SH_THREADS);
+    int vec_ok = ((uintptr_t)coeffs % 16) == 0;
+#define GSB_SH_FM(K) sh_forward_multiview_kernel<K><<<grid, SH_THREADS, 0, s>>>(n, degrees_to_use, means, num_views, cam_positions, coeffs, bias, rgbs, vec_ok)
+    switch (degree) {
+        case 0: GSB_SH_FM(1); break;
+        case 1: GSB_SH_FM(4); break;
+        case 2: GSB_SH_FM(9); break;
+        case 3: GSB_SH_FM(16); break;
+        default: GSB_SH_FM(25); break;
+    }
+#undef GSB_SH_FM
+    GSB_LAUNCH_CHECK();
+    return 0;
 }
 
 // In-place gradient of clamp_min(. , 0): v_rgbs *= [rgbs > 0]  (what gsb_sh_backward_rgb does internally;

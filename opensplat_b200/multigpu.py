@@ -26,6 +26,11 @@ the same view on every step, bench.py).  A trainer renders a different camera on
 symmetric allocation, and from then on the launches use the `_cams` entry points, whose kernel reads every peer's
 centre through the peer mapping, as it reads the colour gradients -- no collective on the step.  `degrees_to_use`
 (the SH degree schedule) is passed through to the kernel; it defaults to the pipeline's full degree.
+
+Several views per rank (`views_per_rank=B`, a trainer's B views of one step): the allocation holds B colour slots and
+B centre trailers, and the launches expand all B x G views, ordered rank-major (view r*B + b), so that every replica
+sums the same views in the same order; gradients are averaged over the B x G views.  `symmetric_layout` and
+`view_pointers` hold the offset and pointer arithmetic.
 """
 import os
 
@@ -35,19 +40,50 @@ import torch.distributed as dist
 from . import capi
 
 
+def symmetric_layout(numel, n, views_per_rank=1):
+    """Float offsets of the symmetric allocation [flat gradients (numel) | B colour slots v_rgb [n,3] | B 16-byte
+    centre trailers]: (rgb_off, cam_off, total).  The B slots are one contiguous [B,n,3] block (slot b at
+    rgb_off + 3 n b), so that one gsb_mask_rgb_grad over n B floats triples masks them all; the block and every
+    trailer start on a 16-byte boundary.  At B = 1 this is the single-view layout."""
+    if numel < 0 or n < 0 or views_per_rank < 1:
+        raise ValueError("symmetric_layout: numel >= 0, n >= 0 and views_per_rank >= 1")
+    rgb_off = (numel + 3) // 4 * 4
+    cam_off = rgb_off + (3 * n * views_per_rank + 3) // 4 * 4
+    return rgb_off, cam_off, cam_off + 4 * views_per_rank
+
+
+def view_pointers(bases, n, views_per_rank, rgb_off, cam_off):
+    """Device addresses of every rank's B colour slots and B centre trailers, given each rank's base address of the
+    allocation (`bases`, in rank order): two lists of G x B entries, rank-major (entry r B + b is rank r's view b)."""
+    rgb = [base + 4 * (rgb_off + 3 * n * b) for base in bases for b in range(views_per_rank)]
+    cam = [base + 4 * (cam_off + 4 * b) for base in bases for b in range(views_per_rank)]
+    return rgb, cam
+
+
 class ViewParallelExchange:
-    def __init__(self, pipe, cam_pos=None, group=None):
-        """cam_pos: this rank's fixed camera centre, gathered from every rank once here; None when the caller passes
-        each step's centre to set_camera() instead (a collective either way: every rank passes one or none)."""
+    def __init__(self, pipe, cam_pos=None, group=None, views_per_rank=1):
+        """cam_pos: this rank's fixed camera centre(s) ([B,3], or [3] at B = 1), gathered from every rank once here;
+        None when the caller passes each step's centres to set_camera() instead (a collective either way: every rank
+        passes one or none).  views_per_rank: the B views every rank contributes per step; every rank must pass the
+        same B (checked here, with one small all-gather)."""
         self.pipe = pipe
         self.group = group if group is not None else dist.group.WORLD
         self.world = dist.get_world_size(self.group)
         self.rank = dist.get_rank(self.group)
+        self.views = int(views_per_rank)
+        if self.views < 1:
+            raise ValueError("views_per_rank must be >= 1")
         dev = pipe.dev
+        mine = torch.tensor([self.views], dtype=torch.int64, device=dev)
+        every = torch.empty(self.world, dtype=torch.int64, device=dev)
+        dist.all_gather_into_tensor(every, mine, group=self.group)
+        if bool((every != mine).any()):
+            raise ValueError(f"ViewParallelExchange: the ranks disagree on views_per_rank ({every.tolist()})")
+        self.num_views = self.world * self.views      # views expanded per step, rank-major
         self.cam_positions = None
         if cam_pos is not None:
-            # every rank's camera centre (tiny, exchanged once)
-            cp = torch.as_tensor(cam_pos, dtype=torch.float32, device=dev).reshape(1, 3)
+            # every rank's camera centres (tiny, exchanged once)
+            cp = torch.as_tensor(cam_pos, dtype=torch.float32, device=dev).reshape(self.views, 3)
             allcp = [torch.zeros_like(cp) for _ in range(self.world)]
             dist.all_gather(allcp, cp, group=self.group)
             self.cam_positions = torch.cat(allcp, 0).contiguous()
@@ -61,23 +97,24 @@ class ViewParallelExchange:
     def _alloc_symmetric(self, pipe):
         import torch.distributed._symmetric_memory as symm_mem
         dev, n = pipe.dev, pipe.n
-        # ONE symmetric allocation: [flat gradient buffer | this view's colour gradient v_rgb [n,3] | this step's
-        # camera centre (3 floats of a 16-byte trailer, read by the peers once set_camera() is used)]
-        rgb_off = (pipe.numel + 3) // 4 * 4
-        cam_off = rgb_off + (3 * n + 3) // 4 * 4
-        total = cam_off + 4
+        # ONE symmetric allocation: [flat gradient buffer | this rank's B colour gradients v_rgb [B,n,3] | this
+        # step's B camera centres (3 floats of a 16-byte trailer each, read by the peers once set_camera() is used)]
+        B = self.views
+        rgb_off, cam_off, total = symmetric_layout(pipe.numel, n, B)
         t = symm_mem.empty(total, dtype=torch.float32, device=dev)
         t.zero_()
         hdl = symm_mem.rendezvous(t, self.group.group_name)
         self.buf, self.hdl = t, hdl
         pipe.rebind_grad_flat(t[:pipe.numel])
-        self.v_rgb = t[rgb_off:rgb_off + 3 * n].view(n, 3)
-        self.cam = t[cam_off:cam_off + 3]
+        self.v_rgb_views = t[rgb_off:rgb_off + 3 * n * B].view(B, n, 3)
+        self.v_rgb = self.v_rgb_views[0]
+        self.cams = t[cam_off:cam_off + 4 * B].view(B, 4)[:, :3]
         base_off = int(getattr(hdl, "offset", 0) or 0)      # the tensor's offset inside its symmetric allocation block
         ptrs = [int(p) + base_off for p in hdl.buffer_ptrs]
         self.geom_ptrs = torch.tensor(ptrs, dtype=torch.int64, device=dev)              # peers' flat buffers
-        self.rgb_ptrs = torch.tensor([p + 4 * rgb_off for p in ptrs], dtype=torch.int64, device=dev)
-        self.cam_ptrs = torch.tensor([p + 4 * cam_off for p in ptrs], dtype=torch.int64, device=dev)   # peers' centres
+        rgb_ptrs, cam_ptrs = view_pointers(ptrs, n, B, rgb_off, cam_off)
+        self.rgb_ptrs = torch.tensor(rgb_ptrs, dtype=torch.int64, device=dev)
+        self.cam_ptrs = torch.tensor(cam_ptrs, dtype=torch.int64, device=dev)   # peers' centres
         mc = int(getattr(hdl, "multicast_ptr", 0) or 0) if self.use_multicast else 0
         mc = mc + base_off if mc else 0
         assert ptrs[self.rank] == t.data_ptr(), "symmetric-memory handle does not describe this tensor"
@@ -92,16 +129,17 @@ class ViewParallelExchange:
         dist.barrier(group=self.group)
         self._alloc_symmetric(pipe)
 
-    def v_rgbs_buffer(self):
-        """Where this step's rasterize-backward must write its colour gradient."""
-        return self.v_rgb
+    def v_rgbs_buffer(self, b=0):
+        """Where this step's rasterize-backward of view b must write its colour gradient."""
+        return self.v_rgb_views[b]
 
-    def set_camera(self, cam_pos_dev):
-        """This step's camera centre (a device float[3]): a stream-ordered device-to-device copy into this rank's
-        trailer, no host wait, no collective.  Call it before every backward pass once it is used (a resize()
-        leaves a new, zeroed trailer).  Safe to overwrite: the previous step closed with barrier(channel=2), which
-        every rank passes only after its multi-view kernel -- the last reader of the peers' trailers -- finished."""
-        self.cam.copy_(cam_pos_dev)
+    def set_camera(self, cam_pos_dev, b=0):
+        """This step's camera centre of view b (a device float[3]): a stream-ordered device-to-device copy into this
+        rank's trailer b, no host wait, no collective.  Call it for every view before every backward pass once it is
+        used (a resize() leaves new, zeroed trailers).  Safe to overwrite: the previous step closed with
+        barrier(channel=2), which every rank passes only after its multi-view kernel -- the last reader of the peers'
+        trailers -- finished."""
+        self.cams[b].copy_(cam_pos_dev)
         self.per_step_cams = True
 
     def _entry_points(self):
@@ -115,24 +153,34 @@ class ViewParallelExchange:
             raise RuntimeError("ViewParallelExchange built without cam_pos: call set_camera() before the backward pass")
         return L.gsb_sh_backward_multiview, L.gsb_exchange_gradients, capi.ptr(self.cam_positions)
 
-    def start_colour(self, average=True, degrees_to_use=None):
+    def _mask(self, rgbs):
+        """The clamp's gradient on all B colour slots, one launch: rgbs are the forward colours of this rank's B views
+        (one contiguous [B,n,3] block; default the pipeline's [n,3] rgbs, B = 1)."""
+        p = self.pipe
+        rgbs = p.rgbs if rgbs is None else rgbs
+        if rgbs.numel() != 3 * p.n * self.views or not rgbs.is_contiguous():
+            raise ValueError(f"rgbs must be one contiguous [{self.views},{p.n},3] block")
+        capi.check(capi.lib().gsb_mask_rgb_grad(p.n * self.views, capi.ptr(rgbs), capi.ptr(self.v_rgb_views),
+                                                capi.stream()))
+
+    def start_colour(self, average=True, degrees_to_use=None, rgbs=None):
         """Call right after rasterize-backward (v_rgb is final, the geometry gradients are not yet): masks v_rgb with
         the clamp's gradient and starts the multi-view SH backward -- the part of the exchange that moves most bytes,
         (G-1) x 12 B per Gaussian -- on a side stream, so that it overlaps project_backward and, afterwards, the
-        all-reduce of the geometry gradients.  degrees_to_use: the SH degree schedule's (default: the full degree)."""
+        all-reduce of the geometry gradients.  degrees_to_use: the SH degree schedule's (default: the full degree).
+        average: scale both halves by 1/(B G), the mean over every view of the step.  rgbs: see _mask."""
         p = self.pipe
-        L = capi.lib()
         multiview, _, cams = self._entry_points()
         use = p.deg if degrees_to_use is None else int(degrees_to_use)
-        self._scale = 1.0 / self.world if average else 1.0
+        self._scale = 1.0 / self.num_views if average else 1.0
         cur = torch.cuda.current_stream()
-        capi.check(L.gsb_mask_rgb_grad(p.n, capi.ptr(p.rgbs), capi.ptr(self.v_rgb), capi.stream()))
+        self._mask(rgbs)
         self._rgb_ready.record(cur)
         with torch.cuda.stream(self.side):
             self.side.wait_event(self._rgb_ready)
-            self.hdl.barrier(channel=0)          # every rank's v_rgb (and camera centre) is complete
+            self.hdl.barrier(channel=0)          # every rank's v_rgb (and camera centres) are complete
             capi.check(multiview(
-                p.n, p.deg, use, capi.ptr(p.p["means"]), self.world, cams,
+                p.n, p.deg, use, capi.ptr(p.p["means"]), self.num_views, cams,
                 self.rgb_ptrs.data_ptr(), self._scale, capi.ptr(p.g["coeffs"]), self.side.cuda_stream))
             self._colour_done.record(self.side)
 
@@ -152,20 +200,19 @@ class ViewParallelExchange:
         # geometry buffers / camera trailers of this step (so the next step may overwrite them)
         self.hdl.barrier(channel=2)
 
-    def exchange(self, average=True, degrees_to_use=None):
+    def exchange(self, average=True, degrees_to_use=None, rgbs=None):
         """The whole exchange after project_backward, as ONE fused launch (gsb_exchange_gradients: both CTA roles in one
         grid) between two barriers -- no overlap with the backward kernels; what callers use that cannot split the
-        step (bench.py's operator-level e2e arm)."""
+        step (bench.py's operator-level e2e arm).  Arguments as start_colour."""
         p = self.pipe
-        L = capi.lib()
         _, exchange, cams = self._entry_points()
         use = p.deg if degrees_to_use is None else int(degrees_to_use)
-        scale = 1.0 / self.world if average else 1.0
-        capi.check(L.gsb_mask_rgb_grad(p.n, capi.ptr(p.rgbs), capi.ptr(self.v_rgb), capi.stream()))
-        # every rank has finished writing this step's v_rgb, camera centre and geometry gradients
+        scale = 1.0 / self.num_views if average else 1.0
+        self._mask(rgbs)
+        # every rank has finished writing this step's v_rgb, camera centres and geometry gradients
         self.hdl.barrier(channel=0)
         capi.check(exchange(
-            p.n, p.deg, use, capi.ptr(p.p["means"]), self.world, cams,
+            p.n, p.deg, use, capi.ptr(p.p["means"]), self.num_views, cams,
             self.rgb_ptrs.data_ptr(), scale, capi.ptr(p.g["coeffs"]), self.rank, self.world, self.geom_numel,
             self.geom_ptrs.data_ptr(), self.multicast_ptr if self.multicast_ptr else None, capi.stream()))
         self.hdl.barrier(channel=2)

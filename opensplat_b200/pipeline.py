@@ -179,12 +179,14 @@ class SplatPipeline:
                                          P(self.nth), s))
         return self._bin_blend(p["opacities"], 0)
 
-    def _bin_blend(self, opacities, flags, count_visible=False):
+    def _bin_blend(self, opacities, flags, count_visible=False, rgbs=None):
         """Binning, packing and the blend kernel of one frame (after SH colour and projection), with the frame's one
         host wait.  opacities: the [n] opacities the blend uses; flags: gsb_rasterize_forward_packed's;
-        count_visible: have the binning count the Gaussians with radii > 0 into self.plan.visible."""
+        count_visible: have the binning count the Gaussians with radii > 0 into self.plan.visible; rgbs: the [n,3]
+        colours the records carry (default self.rgbs; a trainer with several views per step passes the view's)."""
         L, P, s = self.L, capi.ptr, capi.stream()
         n, W, H = self.n, self.W, self.H
+        rgbs = self.rgbs if rgbs is None else rgbs
         bin_flags = 1 | (ops.BIN_COUNT_VISIBLE if count_visible else 0)
         limit = L.gsb_bucket_max_tile_len()
         plan = self.plan
@@ -199,7 +201,7 @@ class SplatPipeline:
             wsp, wsb = self.bucket_ws.data_ptr() + boff, self.bucket_ws.numel() - boff
             self._stage("scan")
             # cull = 1: bin only (Gaussian, tile) pairs whose extent box touches the tile
-            capi.check(L.gsb_bucket_tile_ranges(n, P(self.xys), P(self.radii), P(self.conics), P(self.rgbs),
+            capi.check(L.gsb_bucket_tile_ranges(n, P(self.xys), P(self.radii), P(self.conics), P(rgbs),
                                                 P(opacities), bin_flags, self.tb[0], self.tb[1], m_cap, len_cap, wsp,
                                                 wsb,
                                                 P(self.cum), P(self.tile_bins), P(self.tile_order), P(self.stats_dev),
@@ -236,7 +238,7 @@ class SplatPipeline:
         _, _, _, gids_sorted, self.tile_bins, sorted_index = ops.binAndSortGaussians(
             n, m, self.xys, self.depths, self.radii, self.cum, self.tb, return_index=True)
         self._stage("raster_fwd")
-        capi.check(L.gsb_pack_records(m, P(gids_sorted), P(sorted_index), P(self.xys), P(self.conics), P(self.rgbs),
+        capi.check(L.gsb_pack_records(m, P(gids_sorted), P(sorted_index), P(self.xys), P(self.conics), P(rgbs),
                                       P(opacities), P(self.records), s))
         capi.check(L.gsb_rasterize_forward_packed(H, W, self.tb[0], self.tb[1], m, P(self.tile_bins), None, None,
                                                   P(self.background), P(self.records), P(self.out_img),

@@ -27,7 +27,22 @@ replicas stay bit-identical; the statistics of a refinement are reduced by Densi
 hits nothing contributes zero gradients and zero statistics but takes every collective, as model.GaussianModel does
 under a group (parallel.allreduce_tensor_grads, Densifier.after_train); with one rank such a step trains nothing, as
 without a group.  Between refinements a step still allocates nothing and waits on the host once (the barriers are
-device-side)."""
+device-side).
+
+Several views per step (`views_per_step=B`, with or without a group):
+
+    trainer = SplatTrainer(params, cfg, views_per_step=4)
+    loss = trainer.step([cam_a, cam_b, cam_c, cam_d], gts, step)   # gts: B [H,W,3] images or [B,H,W,3]; loss [B,3]
+
+All B views render at the step's one resolution.  The SH forward evaluates the coefficient block once for the B camera
+centres (gsb_sh_forward_rgb_cam_multiview); each view then runs projection, binning (its own host wait), blend, loss,
+rasterize-backward into its own colour slot and projection backward, which sums the geometry gradients over the views
+in place (gsb_project_backward_activated_acc); the B colour gradients are expanded by one multi-view SH backward
+launch, the same kernel that expands the ranks' views under a group.  Adam sees the mean over the B x G views (G
+ranks, 1 without a group); a view that hits nothing adds zero but counts in the divisor.  The schedules (SH degree,
+downscale, means learning rate, refinement, alpha reset) advance once per step, not per view, and no learning rate is
+scaled with B.  Densification statistics are accumulated per view, in view order (densify.Densifier.accumulate_view).
+Between refinements a step allocates nothing and waits on the host once per view."""
 import ctypes as C
 
 import torch
@@ -35,7 +50,8 @@ import torch
 from . import capi, ops
 from .densify import Densifier, RefineConfig
 from .export import SceneWriter
-from .model import LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, camera_setup, downscale_factor, means_learning_rate
+from .model import (LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, Camera, camera_setup, downscale_factor,
+                    means_learning_rate)
 from .parallel import flat_views
 from .pipeline import SplatPipeline
 
@@ -66,16 +82,39 @@ def _split_coeffs(views):
     return {k: out[k] for k in PARAM_NAMES}
 
 
+def view_setups(cams, gts, views, downscale):
+    """The camera blocks (model.camera_setup) of one step's `views` cameras at `downscale`, checked against the
+    ground-truth images: returns (setups, H, W).  Raises ValueError unless there are exactly `views` cameras and
+    images, all cameras render at one resolution and every image is a float32 [H,W,3] tensor of it."""
+    cams = [cams] if isinstance(cams, Camera) else list(cams)
+    if len(cams) != views or len(gts) != views:
+        raise ValueError(f"a step takes {views} cameras and {views} ground-truth images (views_per_step={views}), "
+                         f"got {len(cams)} and {len(gts)}")
+    setups = [camera_setup(c, downscale) for c in cams]
+    H, W = setups[0][0], setups[0][1]
+    if any((su[0], su[1]) != (H, W) for su in setups):
+        raise ValueError("all views of a step must render at the same resolution, got (W, H) "
+                         f"{sorted({(su[1], su[0]) for su in setups})}")
+    for gt in gts:
+        if gt.dtype != torch.float32 or tuple(gt.shape) != (H, W, 3):
+            raise ValueError(f"every gt must be a float32 [{H},{W},3] image (this step's render resolution)")
+    return setups, H, W
+
+
 class SplatTrainer:
     def __init__(self, params, cfg=None, sh_degree=None, sh_degree_interval=1000, num_downscales=0,
                  resolution_schedule=3000, background=(0.6130, 0.0101, 0.3984), device="cuda:0", generator=None,
-                 ssim_weight=0.2, m_capacity=None, group=None):
+                 ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1):
         """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
         featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
         m_capacity: initial intersection capacity of the binning buffers (grown on demand).
         group: a process group to train data-parallel over camera views (any size, 1 included); every rank
-        constructs the trainer with the same parameters and calls step() with the same step numbers."""
+        constructs the trainer with the same parameters and calls step() with the same step numbers.
+        views_per_step: B camera views per step (per rank under a group); step() then takes B cameras and B images."""
         import torch.distributed as dist
+        self.views_per_step = B = int(views_per_step)
+        if B < 1:
+            raise ValueError("views_per_step must be >= 1")
         if group is None and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
             raise RuntimeError("SplatTrainer without a group runs in one process; pass group= to train data-parallel "
                                "over camera views")
@@ -109,22 +148,42 @@ class SplatTrainer:
         self.cam_pos = self.cam_dev[32:35]
         self.projmat = torch.zeros((4, 4), dtype=torch.float32, device=self.device)
         self.loss = torch.zeros(3, dtype=torch.float32, device=self.device)
+        if B > 1:
+            # the B cameras: views [B,16] | projs [B,16] | centres [B,3], one pinned staging block, one upload per step
+            self.cams_host = torch.zeros(35 * B, dtype=torch.float32).pin_memory()
+            self.cams_dev = torch.zeros(35 * B, dtype=torch.float32, device=self.device)
+            self.viewmats = self.cams_dev[:16 * B].view(B, 4, 4)
+            self.projs = self.cams_dev[16 * B:32 * B].view(B, 4, 4)
+            self.cam_positions = self.cams_dev[32 * B:].view(B, 3)
+            self.projmats = torch.zeros((B, 4, 4), dtype=torch.float32, device=self.device)
+            self.losses = torch.zeros((B, 3), dtype=torch.float32, device=self.device)
         self.resolution = None
         self.pixel_reallocs = 0   # resolution changes after the first step (the downscale schedule)
         self.writer = None
         self.last_info = {"refined": False}
-        self._alloc_gaussian_scratch()
         self.world, self.exchange = 1, None
         if group is not None:
             from .multigpu import ViewParallelExchange
             self.world = dist.get_world_size(group)
-            # symmetric gradient buffer + trailers; SplatPipeline.resize_gaussians rebuilds them after a refinement
-            pp.exchange = self.exchange = ViewParallelExchange(pp, group=group)
+            # symmetric gradient buffer + colour slots + trailers; SplatPipeline.resize_gaussians rebuilds them after a
+            # refinement
+            pp.exchange = self.exchange = ViewParallelExchange(pp, group=group, views_per_rank=B)
+        self._alloc_gaussian_scratch()
 
     def _alloc_gaussian_scratch(self):
-        n = self.pipe.n
-        self.opac = torch.empty(n, dtype=torch.float32, device=self.device)     # sigmoid(logits) for the blend
-        self.v_opac = torch.empty(n, dtype=torch.float32, device=self.device)   # blend gradient w.r.t. it
+        """The trainer's per-Gaussian buffers, (re)built at construction and after a refinement."""
+        pp, n, B, d = self.pipe, self.pipe.n, self.views_per_step, self.device
+        self.opac = torch.empty(n, dtype=torch.float32, device=d)     # sigmoid(logits) for the blend
+        self.v_opac = torch.empty(n, dtype=torch.float32, device=d)   # blend gradient w.r.t. it
+        if B > 1:
+            self.rgbs_views = torch.empty((B, n, 3), dtype=torch.float32, device=d)   # the B views' colours
+            if self.exchange is None:
+                # The B colour gradients and the pointer tables of the one multi-view SH backward launch; under a
+                # group the colour slots live in the exchange's symmetric allocation instead.
+                self.v_rgb_views = torch.empty((B, n, 3), dtype=torch.float32, device=d)
+                self.rgb_ptrs = torch.tensor([self.v_rgb_views[b].data_ptr() for b in range(B)], dtype=torch.int64,
+                                             device=d)
+                self.geom_ptrs = torch.tensor([pp.grad_flat.data_ptr()], dtype=torch.int64, device=d)
 
     def _set_resolution(self, W, H):
         if self.resolution is not None:
@@ -139,7 +198,8 @@ class SplatTrainer:
 
     @property
     def image(self):
-        """The image of the last step ([H,W,3], clamped to 1; the background where nothing was visible)."""
+        """The image of the last step ([H,W,3], clamped to 1; the background where nothing was visible); with
+        several views per step, the last view's."""
         return self.pipe.out_img
 
     def params(self):
@@ -154,7 +214,10 @@ class SplatTrainer:
     def step(self, cam, gt, step):
         """One training step at `step` (1-based, as opensplat.cpp counts).  cam: model.Camera; gt: [H,W,3] fp32 CUDA
         image at this step's render resolution.  Returns the device tensor {total, L1, SSIM}, which the next step
-        overwrites."""
+        overwrites.  With views_per_step = B > 1: cam is a sequence of B cameras, gt B images (a sequence or a
+        [B,H,W,3] tensor), and the result is the device [B,3] tensor of the views' {total, L1, SSIM}."""
+        if self.views_per_step > 1:
+            return self._step_views(cam, gt, step)
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         H, W, (fx, fy, cx, cy), view, proj, cam_pos = camera_setup(
             cam, downscale_factor(step, self.num_downscales, self.resolution_schedule))
@@ -188,25 +251,114 @@ class SplatTrainer:
         # refinement's collectives): its backward pass writes zero gradients, no Gaussian having radii > 0
         if visible or self.world > 1:
             self._backward(use, fx, fy, H, W)
-            # ---- the six optimizers in one launch (torch.optim.Adam defaults, as GaussianModel.optimizers_step) ----
-            pp.adam_t += 1
-            t = pp.adam_t
-            segs = adam_segments(pp.offs, self.lr)
-            table = (capi.AdamSegment * len(segs))(*[capi.AdamSegment(*sg) for sg in segs])
-            capi.check(L.gsb_adam_step_segments(len(segs), C.addressof(table), P(pp.param_flat), P(pp.grad_flat),
-                                                P(pp.adam_m), P(pp.adam_v), 0.9, 0.999, 1e-8, 1.0 - 0.9 ** t,
-                                                1.0 - 0.999 ** t, s))
+            self._adam_step()
         self.lr["means"] = means_learning_rate(step, self.cfg.max_steps, MEANS_LR_INIT)
         if visible or self.world > 1:
             # ---- Model::afterTrain on views into the flat buffers (an empty view: zero statistics, see above) ----
-            new_p, new_m, new_v, info = self.densifier.after_train(
+            self._adopt(*self.densifier.after_train(
                 step, pp.p, flat_views(pp.adam_m, pp.offs), flat_views(pp.adam_v, pp.offs),
-                pp.v_xy if visible else None, pp.radii, H, W)
-            if new_p is not pp.p:   # the Gaussian set changed: the only allocations of a step
-                pp.resize_gaussians(new_p, new_m, new_v)
-                self._alloc_gaussian_scratch()
-        self.last_info = info
+                pp.v_xy if visible else None, pp.radii, H, W))
+        else:
+            self.last_info = info
         return self.loss
+
+    def _adam_step(self):
+        """The six optimizers in one launch (torch.optim.Adam defaults, as GaussianModel.optimizers_step)."""
+        pp, P = self.pipe, capi.ptr
+        pp.adam_t += 1
+        t = pp.adam_t
+        segs = adam_segments(pp.offs, self.lr)
+        table = (capi.AdamSegment * len(segs))(*[capi.AdamSegment(*sg) for sg in segs])
+        capi.check(self.L.gsb_adam_step_segments(len(segs), C.addressof(table), P(pp.param_flat), P(pp.grad_flat),
+                                                 P(pp.adam_m), P(pp.adam_v), 0.9, 0.999, 1e-8, 1.0 - 0.9 ** t,
+                                                 1.0 - 0.999 ** t, capi.stream()))
+
+    def _adopt(self, new_p, new_m, new_v, info):
+        """The densifier's result: a changed Gaussian set re-creates the flat layout (the only allocations of a
+        step)."""
+        pp = self.pipe
+        if new_p is not pp.p:
+            pp.resize_gaussians(new_p, new_m, new_v)
+            self._alloc_gaussian_scratch()
+        self.last_info = info
+
+    def _step_views(self, cams, gts, step):
+        """step() with B = views_per_step > 1 views.  A separate body from the one-view step: that one issues
+        gsb_sh_forward_rgb_cam / gsb_sh_backward_rgb_cam (or the exchange at B = 1), whose launches and bits the
+        one-view trainer keeps; this one issues the multi-view SH forward, the accumulating projection backward and
+        one multi-view SH backward launch for the B colour gradients."""
+        pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
+        B, ex = self.views_per_step, self.exchange
+        setups, H, W = view_setups(cams, gts, B, downscale_factor(step, self.num_downscales, self.resolution_schedule))
+        if (W, H) != self.resolution:
+            self._set_resolution(W, H)
+        # One upload of the B cameras; the previous step's last host wait came after the last upload of this block.
+        host = self.cams_host
+        for b, (_, _, _, view, proj, cam_pos) in enumerate(setups):
+            host[16 * b:16 * b + 16].copy_(view.reshape(16))
+            host[16 * (B + b):16 * (B + b) + 16].copy_(proj.reshape(16))
+            host[32 * B + 3 * b:32 * B + 3 * b + 3].copy_(cam_pos)
+        self.cams_dev.copy_(host, non_blocking=True)
+        torch.matmul(self.projs, self.viewmats, out=self.projmats)    # the B `proj @ view` products
+        n, p, g, tb = pp.n, pp.p, pp.g, pp.tb
+        use = min(step // self.sh_degree_interval, self.sh_degree)
+        capi.check(L.gsb_sh_forward_rgb_cam_multiview(n, pp.deg, use, P(p["means"]), B, P(self.cam_positions),
+                                                      P(p["coeffs"]), 0.5, P(self.rgbs_views), s))
+        visible = []
+        for b in range(B):
+            fx, fy, cx, cy = setups[b][2]
+            viewmat, projmat, rgbs = self.viewmats[b], self.projmats[b], self.rgbs_views[b]
+            capi.check(L.gsb_project_forward_activated(
+                n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(viewmat), P(projmat),
+                fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths), P(pp.radii),
+                P(pp.conics), P(pp.nth), P(self.opac), s))
+            pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=rgbs)
+            off = (-self.ssim_ws.data_ptr()) % 256
+            capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gts[b]), self.ssim_weight, P(pp.v_img),
+                                          P(self.losses[b]), self.ssim_ws.data_ptr() + off,
+                                          self.ssim_ws.numel() - off, s))
+            visible.append(pp.plan.visible > 0)
+            # The backward pass of every view, an empty one included: it writes zero gradients (no Gaussian with
+            # radii > 0), so the sum over the views and the divisor B stay as they are.
+            if ex is not None:
+                ex.set_camera(self.cam_positions[b], b)
+            v_rgb = ex.v_rgbs_buffer(b) if ex is not None else self.v_rgb_views[b]
+            capi.check(L.gsb_rasterize_backward(
+                H, W, tb[0], tb[1], n, pp.m_raster, P(pp.tile_bins), P(pp.tile_order) if pp._ordered else None,
+                P(pp.conics), P(self.opac), P(pp.records), P(pp.cum), P(pp.background), P(pp.final_Ts),
+                P(pp.final_idx), P(pp.v_img), None, P(pp.grad_rows), P(pp.v_xy), P(pp.v_conic), P(v_rgb),
+                P(self.v_opac), ops.CLAMP_MAX_ONE, s))
+            if ex is not None and ex.overlap and b == B - 1:
+                ex.start_colour(degrees_to_use=use, rgbs=self.rgbs_views)   # every colour slot is final
+            pj = L.gsb_project_backward_activated if b == 0 else L.gsb_project_backward_activated_acc
+            capi.check(pj(n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(self.opac), P(viewmat),
+                          P(projmat), fx, fy, H, W, P(pp.radii), P(pp.conics), P(pp.v_xy), None, P(pp.v_conic),
+                          P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]), s))
+            # this view's densification statistics (pp.v_xy / pp.radii are overwritten by the next view)
+            self.densifier.accumulate_view(step, pp.v_xy if visible[b] else None, pp.radii, H, W)
+        # A step whose views all hit nothing trains nothing, as one empty view does; under a group with more than one
+        # rank it takes part in the step (see the module docstring).
+        trains = any(visible) or self.world > 1
+        if trains:
+            if ex is None:
+                # The colour half: the clamp's gradient on the B slots and their expansion, plus the geometry prefix
+                # times 1/B (the all-reduce role at world 1), in one launch of the data-parallel exchange kernel.
+                capi.check(L.gsb_mask_rgb_grad(n * B, P(self.rgbs_views), P(self.v_rgb_views), s))
+                capi.check(L.gsb_exchange_gradients(
+                    n, pp.deg, use, P(p["means"]), B, P(self.cam_positions), self.rgb_ptrs.data_ptr(), 1.0 / B,
+                    P(g["coeffs"]), 0, 1, pp.geom_numel, self.geom_ptrs.data_ptr(), None, s))
+            elif ex.overlap:
+                ex.finish(degrees_to_use=use)
+            else:
+                ex.exchange(degrees_to_use=use, rgbs=self.rgbs_views)
+            self._adam_step()
+        self.lr["means"] = means_learning_rate(step, self.cfg.max_steps, MEANS_LR_INIT)
+        if trains:
+            self._adopt(*self.densifier.finish_step(step, pp.p, flat_views(pp.adam_m, pp.offs),
+                                                    flat_views(pp.adam_v, pp.offs), H, W))
+        else:
+            self.last_info = {"refined": False}
+        return self.losses
 
     def _backward(self, use, fx, fy, H, W):
         """Rasterize-backward, project-backward and the SH backward of the last forward pass (degrees_to_use `use`)

@@ -11,7 +11,15 @@ turned around (its view hits nothing) on a densification step.  It checks:
   * replicas bit-identical (parameters and moments) after every step;
   * the steady state: between refinements a step allocates no device memory and waits on the host once.
 GSB_EXCHANGE_MULTICAST=0 forces the peer-pointer all-reduce, GSB_EXCHANGE_OVERLAP=0 the single-launch exchange.
+
+--views-per-rank B (default 1): every rank trains B views per step (SplatTrainer(views_per_step=B); rank r's view b
+of step s is view ((s - 1) B G + r B + b) % V).  The GaussianModel reference then runs a forward, loss and backward
+per view, keeps each view's xys.grad and radii, scales the leaf gradients by 1/B before optimizers_step (which
+averages over the ranks) and accumulates the statistics view by view (Densifier.accumulate_view, finish_step).  On
+the densification step the last view of rank 1 (of rank 0 at world size 1) is turned around.  The steady state then
+expects B host waits per step.
 Rank 0 prints one line ending in `check_ok=True|False`; the exit code is 0 iff every check held on every rank."""
+import argparse
 import os
 import sys
 
@@ -22,6 +30,9 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
+ap = argparse.ArgumentParser()
+ap.add_argument("--views-per-rank", type=int, default=1)
+B = ap.parse_args().views_per_rank
 rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
 torch.cuda.set_device(local)
 DEV = torch.device("cuda", local)
@@ -57,18 +68,34 @@ def view(step):
     return cam, gts_d[downscale_factor(step, KW["num_downscales"], KW["resolution_schedule"])][v]
 
 
+def views(step):
+    """B > 1: this rank's B (camera, image) pairs of `step`."""
+    f = downscale_factor(step, KW["num_downscales"], KW["resolution_schedule"])
+    out = []
+    for b in range(B):
+        v = ((step - 1) * B * world + rank * B + b) % V
+        empty = step == EMPTY_STEP and b == B - 1 and rank == min(1, world - 1)
+        out.append((away_cam if empty else cams[v], gts_d[f][v]))
+    return out
+
+
 def params():
     return {k: torch.from_numpy(v) for k, v in p.items()}
 
 
 def run_trainer(group, check_sync):
-    tr = SplatTrainer(params(), cfg(), device=DEV, ssim_weight=SSIM_W, group=group, **KW)
+    tr = SplatTrainer(params(), cfg(), device=DEV, ssim_weight=SSIM_W, group=group, views_per_step=B, **KW)
     torch.manual_seed(SEED)
     losses, counts, in_sync, empty_visible = [], [], True, None
     for step in range(1, STEPS + 1):
-        cam, gt = view(step)
-        loss = tr.step(cam, gt, step)
-        losses.append(float(loss[0]))
+        if B == 1:
+            cam, gt = view(step)
+            loss = tr.step(cam, gt, step)
+            losses.append(float(loss[0]))
+        else:
+            vs = views(step)
+            loss = tr.step([c for c, _ in vs], [g for _, g in vs], step)
+            losses.extend(float(x) for x in loss[:, 0].tolist())
         counts.append(tr.n)
         if step == EMPTY_STEP:
             empty_visible = tr.pipe.plan.visible
@@ -79,6 +106,8 @@ def run_trainer(group, check_sync):
 
 
 def run_model():
+    if B > 1:
+        return run_model_views()
     model = GaussianModel(params(), cfg(), device=DEV, group=dist.group.WORLD, **KW)
     torch.manual_seed(SEED)
     losses, counts = [], []
@@ -92,6 +121,52 @@ def run_model():
         model.optimizers_step()
         model.schedulers_step(step)
         model.after_train(step)
+        counts.append(model.means.shape[0])
+    return model, np.array(losses), np.array(counts)
+
+
+def model_views_step(model, pairs, step):
+    """One B-view step of GaussianModel: per view a forward, loss and backward (the leaf gradients sum over the
+    views), the gradients times 1/B, optimizers_step (the mean over the ranks), then the per-view statistics and one
+    refine decision.  Returns the B losses."""
+    model.optimizers_zero_grad()
+    losses, stats = [], []
+    for cam, gt in pairs:
+        loss = model.main_loss(model.forward(cam, step), gt, SSIM_W)
+        if loss.requires_grad:
+            loss.backward()
+        losses.append(float(loss.detach()))
+        g = model.xys.grad
+        stats.append((g.detach().clone() if g is not None else None, model.radii.clone()))
+    with torch.no_grad():
+        for k in PARAM_NAMES:
+            if getattr(model, k).grad is not None:
+                getattr(model, k).grad.mul_(1.0 / len(pairs))
+    d = model.densifier
+    trains = any(v is not None for v, _ in stats) or d._world() > 1
+    if trains:   # a step whose views all hit nothing trains nothing (one process)
+        model.optimizers_step()
+    model.schedulers_step(step)
+    if trains:
+        for v_xy, radii in stats:
+            d.accumulate_view(step, v_xy, radii, model.lastHeight, model.lastWidth)
+        with torch.no_grad():
+            p = {k: getattr(model, k).detach() for k in PARAM_NAMES}
+            new_p, new_m, new_v, _ = d.finish_step(step, p, model.adam_m, model.adam_v, model.lastHeight,
+                                                   model.lastWidth)
+            if new_p is not p:
+                for k in PARAM_NAMES:
+                    setattr(model, k, new_p[k].requires_grad_())
+                model.adam_m, model.adam_v = new_m, new_v
+    return losses
+
+
+def run_model_views():
+    model = GaussianModel(params(), cfg(), device=DEV, group=dist.group.WORLD, **KW)
+    torch.manual_seed(SEED)
+    losses, counts = [], []
+    for step in range(1, STEPS + 1):
+        losses.extend(model_views_step(model, views(step), step))
         counts.append(model.means.shape[0])
     return model, np.array(losses), np.array(counts)
 
@@ -120,11 +195,16 @@ def compare(model, tr, lm, lt, cm, ct):
 
 def steady_state():
     """10 steps between refinements under set_sync_debug_mode('error'): (allocations, BinPlan.wait calls)."""
-    tr = SplatTrainer(params(), cfg(warmup_length=10 ** 6), device=DEV, group=dist.group.WORLD, **KW)
+    tr = SplatTrainer(params(), cfg(warmup_length=10 ** 6), device=DEV, group=dist.group.WORLD, views_per_step=B,
+                      **KW)
 
     def step_at(step):                               # full resolution, no turned-around camera
-        v = (step - 1 + rank) % V
-        tr.step(cams[v], gts_d[1][v], step)
+        if B == 1:
+            v = (step - 1 + rank) % V
+            tr.step(cams[v], gts_d[1][v], step)
+        else:
+            vs = [((step - 1) * B * world + rank * B + b) % V for b in range(B)]
+            tr.step([cams[v] for v in vs], [gts_d[1][v] for v in vs], step)
     for step in range(11, 16):                       # warm-up: plan, bins, statistics, cuBLAS
         step_at(step)
     torch.cuda.synchronize()
@@ -155,7 +235,8 @@ tr, lt, ct, in_sync, empty_visible = run_trainer(dist.group.WORLD, check_sync=Tr
 model, lm, cm = run_model()
 ok, dloss, exact = compare(model, tr, lm, lt, cm, ct)
 refined = bool(cm[11] != cm[10] and cm[17] != cm[16])      # both densifications changed the Gaussian set
-empty_ok = world < 2 or rank != 1 or empty_visible == 0
+empty_ok = (world < 2 or rank != 1 or empty_visible == 0) if B == 1 else (rank != min(1, world - 1) or
+                                                                        empty_visible == 0)
 mc, overlap = bool(tr.exchange.multicast_ptr), tr.exchange.overlap
 plain_exact = None
 if world == 1:                                   # the same run without the exchange (group=None)
@@ -165,7 +246,7 @@ if world == 1:                                   # the same run without the exch
     del tp
 del tr, model
 allocs, waits = steady_state()
-steady_ok = allocs == 0 and waits == 10
+steady_ok = allocs == 0 and waits == 10 * B
 flags = torch.tensor([int(ok), int(in_sync), int(refined), int(empty_ok), int(steady_ok)], device=DEV)
 dist.all_reduce(flags, op=dist.ReduceOp.MIN)
 dl = torch.tensor([dloss], dtype=torch.float64, device=DEV)
@@ -175,6 +256,7 @@ if rank == 0:
     print(f"parallel trainer check world={world} multicast={mc} overlap={overlap}: counts {ct[0]}->{ct[-1]} "
           f"max|dloss|={float(dl[0]):.3g} matches_gaussian_model={bool(flags[0])} bit_identical={exact} "
           f"plain_trainer_bit_identical={plain_exact} replicas_in_sync={bool(flags[1])} refined={bool(flags[2])} "
-          f"empty_view_ok={bool(flags[3])} steady_allocs={allocs} steady_waits={waits} check_ok={good}")
+          f"empty_view_ok={bool(flags[3])} steady_allocs={allocs} steady_waits={waits} "
+          + (f"views_per_rank={B} " if B > 1 else "") + f"check_ok={good}")
 dist.destroy_process_group()
 sys.exit(0 if good else 1)
