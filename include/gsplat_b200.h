@@ -439,6 +439,20 @@ int gsb_ssim_l1_loss(int img_h, int img_w, const float *rendered, const float *g
                      float *v_rendered, float *loss_out, void *workspace, size_t workspace_bytes,
                      gsb_stream_t stream);
 
+/* ---- Point-cloud initialisation (Model's constructor, model.hpp:23-57) ---------------------------
+ * gsb_knn_mean_dist replaces PointsTensor::scales (kdtree_tensor.cpp:4-22, a nanoflann k-d tree on the CPU):
+ *   mean_dist [n] = the mean distance from every point of xyz [n,3] to its 3 nearest neighbours, exactly.  With
+ *   d(i,j) = ((dx*dx) + (dy*dy)) + (dz*dz), dx = x_i - x_j in fp32 and every operation rounded separately, and
+ *   d0 <= d1 <= d2 <= d3 the four smallest d(i,j) over all j (i itself included):
+ *   mean_dist[i] = ((sqrtf(d1) + sqrtf(d2)) + sqrtf(d3)) / 3.0f (IEEE sqrt and division).  The result depends only on
+ *   those values: it is deterministic, and permuting the points permutes it.  n = 0 is a no-op; 1 <= n < 4 is
+ *   GSB_ERR_INVALID_ARG (the reference reads unset result slots there).  Coordinates must be finite (not checked:
+ *   non-finite input gives unspecified values).  The workspace (gsb_knn_workspace_bytes(n) bytes) must be 256-byte
+ *   aligned. */
+size_t gsb_knn_workspace_bytes(int n);
+int gsb_knn_mean_dist(int n, const float *xyz, float *mean_dist, void *workspace, size_t workspace_bytes,
+                      gsb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -27,6 +27,7 @@ SOURCES = {
     "ssim.cu": [],
     "densify.cu": [],
     "export.cu": ["--fmad=false"],
+    "knn.cu": ["--fmad=false"],
 }
 
 

@@ -84,6 +84,8 @@ _SIGS = {
     # num_segments, segments (host AdamSegment array), param, grad, exp_avg, exp_avg_sq, b1, b2, eps, bc1, bc2, stream
     "gsb_adam_step_segments": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _vp]),
     "gsb_mse_loss_grad": (_i, [C.c_longlong, _vp, _vp, _vp, _vp, _f, _vp]),
+    "gsb_knn_workspace_bytes": (_sz, [_i]),
+    "gsb_knn_mean_dist": (_i, [_i, _vp, _vp, _vp, _sz, _vp]),
 }
 
 ADAM_MAX_SEGMENTS = 8   # GSB_ADAM_MAX_SEGMENTS
