@@ -248,10 +248,23 @@ class SplatPipeline:
         self._stage("end_fwd")
         return self.out_img
 
+    def _raster_backward(self, opacities, v_opacities, v_rgbs, flags):
+        """The blend kernel's backward of the last frame (_bin_blend's), from the gradient of its image in self.v_img
+        into self.v_xy / self.v_conic, `v_rgbs` ([n,3]) and `v_opacities` ([n]).  opacities: the ones the blend used;
+        flags: the ones it was launched with.  The frame's binning state is read here, so callers need not know it:
+        which path produced the frame (only the fast path leaves a tile order), the records and the capacity they
+        were sized with, the per-pixel state of the blend."""
+        P = capi.ptr
+        capi.check(self.L.gsb_rasterize_backward(
+            self.H, self.W, self.tb[0], self.tb[1], self.n, self.m_raster, P(self.tile_bins),
+            P(self.tile_order) if self._ordered else None, P(self.conics), P(opacities), P(self.records), P(self.cum),
+            P(self.background), P(self.final_Ts), P(self.final_idx), P(self.v_img), None, P(self.grad_rows),
+            P(self.v_xy), P(self.v_conic), P(v_rgbs), P(v_opacities), flags, capi.stream()))
+
     def backward(self):
         """MSE loss against self.target + the whole backward path; grads land in self.grad_flat."""
         L, P, s = self.L, capi.ptr, capi.stream()
-        n, W, H, m = self.n, self.W, self.H, self.m_raster   # m: what the records buffer was sized with
+        n, W, H = self.n, self.W, self.H
         fx, fy, cx, cy = self.intr
         p, g = self.p, self.g
         cnt = H * W * 3
@@ -259,12 +272,7 @@ class SplatPipeline:
         capi.check(L.gsb_mse_loss_grad(cnt, P(self.out_img), P(self.target), P(self.v_img), P(self.loss), 1.0 / cnt, s))
         v_rgbs = self.exchange.v_rgbs_buffer() if self.exchange is not None else self.v_rgbs
         self._stage("raster_bwd")
-        capi.check(L.gsb_rasterize_backward(H, W, self.tb[0], self.tb[1], n, m, P(self.tile_bins),
-                                    P(self.tile_order) if self._ordered else None, P(self.conics),
-                                    P(p["opacities"]), P(self.records), P(self.cum), P(self.background),
-                                    P(self.final_Ts), P(self.final_idx),
-                                    P(self.v_img), None, P(self.grad_rows), P(self.v_xy), P(self.v_conic),
-                                    P(v_rgbs), P(g["opacities"]), 0, s))
+        self._raster_backward(p["opacities"], g["opacities"], v_rgbs, 0)
         if self.exchange is not None and self.exchange.overlap:
             self.exchange.start_colour(average=True)   # colour pulls + SH expansion start now, on a side stream
         self._stage("project_bwd")

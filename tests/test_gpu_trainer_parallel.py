@@ -105,10 +105,10 @@ def test_exchange_launch_with_per_view_camera_pointers_does_both_roles():
     assert torch.equal(geom_b, g0)
 
 
-def test_empty_view_backward_writes_exact_zeros():
-    """What a rank whose view hits nothing contributes to the data-parallel exchange: the trainer's backward pass
-    (rasterize-backward, project-backward, SH backward) on such a view writes zeros into the whole gradient buffer
-    and the colour gradient."""
+def test_empty_view_backward_helpers_write_exact_zeros():
+    """What a rank whose view hits nothing contributes to the data-parallel exchange: the trainer's per-view backward
+    pass (rasterize-backward, project-backward) and its SH backward on such a view write zeros into the whole
+    gradient buffer and the colour gradient."""
     from opensplat_b200.model import Camera
     from opensplat_b200.trainer import SplatTrainer
     from test_gpu_trainer import _cams, make_problem, refine_config
@@ -126,7 +126,8 @@ def test_empty_view_backward_writes_exact_zeros():
     assert pp.plan.visible == 0
     pp.grad_flat.fill_(float("nan"))
     pp.v_rgbs.fill_(float("nan"))
-    tr._backward(1, intr[0], intr[1], H, W)
+    tr._backward_view(0, 1, intr[0], intr[1])
+    tr._sh_backward(1)
     torch.cuda.synchronize()
     for name, (o, c, _) in pp.offs.items():
         assert bool((pp.grad_flat[o:o + c] == 0).all()), name

@@ -176,12 +176,13 @@ def main():
     for s in range(190, 200):
         tr.step(cam, gt, s)
     n0 = tr.n
-    ms_r = timed(lambda i: tr.step(cam, gt, 200), 1)
+    losses = []
+    ms_r = timed(lambda i: losses.append(tr.step(cam, gt, 200)), 1)
     info = tr.last_info
     out["splat_trainer"]["refine"] = {"step_ms": ms_r, "n_before": n0, "n_after": tr.n,
                                       "n_splits": info.get("n_splits"), "culled": info.get("culled")}
     out["speedup_iters_per_s"] = out["splat_trainer"]["iters_per_s"] / out["gaussian_model"]["iters_per_s"]
-    out["final_loss_trainer"] = float(tr.loss[0])
+    out["final_loss_trainer"] = float(losses[-1][0])
     print(json.dumps(out))
 
 
