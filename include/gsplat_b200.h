@@ -453,6 +453,30 @@ size_t gsb_knn_workspace_bytes(int n);
 int gsb_knn_mean_dist(int n, const float *xyz, float *mean_dist, void *workspace, size_t workspace_bytes,
                       gsb_stream_t stream);
 
+/* ---- Training images (Camera::loadImage / Camera::getImage, input_data.cpp:40-117) --------------------------------
+ * Images are 3-channel u8, [h,w,3] row-major and dense.
+ * gsb_resize_area_u8 is cv::resize(src, dst, ..., INTER_AREA) of OpenCV 4's CPU code, byte for byte, for dst_h <= src_h and
+ *   dst_w <= src_w.  inv_scale = 0: the call with dsize given (getImage: the scales come from the sizes);
+ *   0 < inv_scale <= 1: the call with an empty dsize and fx = fy = inv_scale (loadImage's 1/downscaleFactor), and then
+ *   dst must be cvRound(src * (double)inv_scale) on both axes.  An integer scale (within DBL_EPSILON) takes OpenCV's
+ *   fast path (at 2x2 full cells round as (s+2)>>2, other full cells as rint(float(s) * (1.f/area)), border cells as
+ *   rint(float(s)/count)); any other scale the general path (double cell edges, float weights and row sums).  Equal
+ *   sizes copy.  src and dst must not overlap.
+ * gsb_undistort_u8 is cv::undistort(src, tmp, K, {k1,k2,p1,p2,k3}, newK) followed by the crop
+ *   dst = tmp[roi_y:roi_y+roi_h, roi_x:roi_x+roi_w], writing only the ROI: dst is [roi_h,roi_w,3].  K and newK are
+ *   (fx, fy, cx, cy) with zero skew, given as the float values of the reference's CV_32F matrices; the map is
+ *   computed in fp64 stripe by stripe as cv::undistort does, quantised to 1/32 pixel, and the remap is OpenCV's
+ *   fixed-point bilinear with BORDER_CONSTANT 0.  An empty ROI is a no-op.
+ * gsb_u8_to_f32_views converts num_views images of [h,w,3] u8 (views: a DEVICE array of num_views device addresses,
+ *   int64) into out [num_views,h,w,3] float32 = float(u) / 255.0f (IEEE division, as imageToTensor), in one launch.
+ *   num_views = 0 is a no-op; at most 65535. */
+int gsb_resize_area_u8(int src_h, int src_w, const uint8_t *src, int dst_h, int dst_w, uint8_t *dst, float inv_scale,
+                       gsb_stream_t stream);
+int gsb_undistort_u8(int h, int w, const uint8_t *src, float fx, float fy, float cx, float cy, float k1, float k2,
+                     float p1, float p2, float k3, float new_fx, float new_fy, float new_cx, float new_cy, int roi_x,
+                     int roi_y, int roi_w, int roi_h, uint8_t *dst, gsb_stream_t stream);
+int gsb_u8_to_f32_views(int num_views, const int64_t *views, int h, int w, float *out, gsb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

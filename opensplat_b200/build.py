@@ -28,6 +28,7 @@ SOURCES = {
     "densify.cu": [],
     "export.cu": ["--fmad=false"],
     "knn.cu": ["--fmad=false"],
+    "image.cu": ["--fmad=false"],
 }
 
 

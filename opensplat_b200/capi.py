@@ -86,6 +86,11 @@ _SIGS = {
     "gsb_mse_loss_grad": (_i, [C.c_longlong, _vp, _vp, _vp, _vp, _f, _vp]),
     "gsb_knn_workspace_bytes": (_sz, [_i]),
     "gsb_knn_mean_dist": (_i, [_i, _vp, _vp, _vp, _sz, _vp]),
+    "gsb_resize_area_u8": (_i, [_i, _i, _vp, _i, _i, _vp, _f, _vp]),
+    # h, w, src, fx, fy, cx, cy, k1, k2, p1, p2, k3, new fx, fy, cx, cy, roi x, y, w, h, dst, stream
+    "gsb_undistort_u8": (_i, [_i, _i, _vp, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _i, _i, _i, _i, _vp,
+                              _vp]),
+    "gsb_u8_to_f32_views": (_i, [_i, _vp, _i, _i, _vp, _vp]),
 }
 
 ADAM_MAX_SEGMENTS = 8   # GSB_ADAM_MAX_SEGMENTS

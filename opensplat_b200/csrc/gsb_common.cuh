@@ -5,7 +5,7 @@
 #include <stdio.h>
 #include "../../include/gsplat_b200.h"
 
-#define GSB_VERSION 700
+#define GSB_VERSION 800
 
 // ---- error plumbing (thread-local message, C ABI returns the code) -------------------------
 void gsb_set_error(int code, const char *what, const char *file, int line);

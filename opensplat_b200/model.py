@@ -31,12 +31,14 @@ def projection_matrix(z_near, z_far, fov_x, fov_y, device):
 
 
 class Camera:
-    """The fields of the reference's Camera that Model::forward reads (input_data.hpp:12-44)."""
+    """The fields of the reference's Camera that Model::forward reads (input_data.hpp:12-44), and its distortion
+    coefficients k1, k2, k3, p1, p2, which Camera::loadImage (images.ImageSet) undistorts the image with."""
 
-    def __init__(self, width, height, fx, fy, cx, cy, cam_to_world):
+    def __init__(self, width, height, fx, fy, cx, cy, cam_to_world, k1=0.0, k2=0.0, k3=0.0, p1=0.0, p2=0.0):
         self.width, self.height = int(width), int(height)
         self.fx, self.fy, self.cx, self.cy = float(fx), float(fy), float(cx), float(cy)
         self.camToWorld = torch.as_tensor(cam_to_world, dtype=torch.float32)
+        self.k1, self.k2, self.k3, self.p1, self.p2 = float(k1), float(k2), float(k3), float(p1), float(p2)
 
 
 # learning rates of Model::setupOptimizers (model.cpp:58-70)

@@ -159,6 +159,7 @@ class SplatTrainer:
         self.cam_positions = self.cams_dev[32 * B:].view(B, 3)
         self.projmats = torch.zeros((B, 4, 4), dtype=torch.float32, device=self.device)
         self.losses = torch.zeros((B, 3), dtype=torch.float32, device=self.device)
+        self.eval_loss = torch.zeros(3, dtype=torch.float32, device=self.device)    # evaluate()'s result
         self.resolution = None
         self.pixel_reallocs = 0   # resolution changes after the first step (the downscale schedule)
         self.writer = None
@@ -286,6 +287,44 @@ class SplatTrainer:
         else:
             self.last_info = {"refined": False}
         return self.losses[0] if B == 1 else self.losses
+
+    def evaluate(self, cam, gt, step):
+        """The loss of one view without training on it (opensplat.cpp:203-207, the --val camera): Model::forward at
+        `step`'s downscale factor and SH degree, then mainLoss against gt (a float32 [H,W,3] CUDA image at that
+        resolution).  It runs the forward kernels and the loss of a one-view step() (at any views_per_step) and
+        returns the device tensor {total, L1, SSIM}, overwritten by the next evaluate().  Parameters, Adam state and
+        the densification statistics are left alone, and the next step() computes what it would have computed
+        without this call.  Other trainer state it does change: `image` becomes the evaluated view's render; a view
+        at another resolution than the last step's reallocates the pixel buffers, and the next step reallocates them
+        back, each counted in `pixel_reallocs`; and the binning buffers grow if the view needs more intersections
+        than they hold (a step grows them the same way, with no effect on its result).  Raises ValueError on a
+        wrong image."""
+        pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
+        B = self.views_per_step
+        setups, H, W = view_setups(cam, [gt], 1, downscale_factor(step, self.num_downscales, self.resolution_schedule))
+        if (W, H) != self.resolution:
+            self._set_resolution(W, H)
+        _, _, (fx, fy, cx, cy), view, proj, cam_pos = setups[0]
+        # slot 0 of the camera block; the last host wait (a binning read-back) came after the block's last upload
+        host = self.cams_host
+        host[:16].copy_(view.reshape(16))
+        host[16 * B:16 * B + 16].copy_(proj.reshape(16))
+        host[32 * B:32 * B + 3].copy_(cam_pos)
+        self.cams_dev.copy_(host, non_blocking=True)
+        n, p, tb = pp.n, pp.p, pp.tb
+        use = min(step // self.sh_degree_interval, self.sh_degree)
+        torch.matmul(self.projs[0], self.viewmats[0], out=self.projmats[0])
+        capi.check(L.gsb_sh_forward_rgb_cam(n, pp.deg, use, P(p["means"]), P(self.cam_positions[0]),
+                                            P(p["coeffs"]), 0.5, P(self.rgbs_views[0]), s))
+        capi.check(L.gsb_project_forward_activated(
+            n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmats[0]),
+            P(self.projmats[0]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
+            P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac), s))
+        pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[0])
+        off = (-self.ssim_ws.data_ptr()) % 256
+        capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(self.eval_loss),
+                                      self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off, s))
+        return self.eval_loss
 
     def _backward_view(self, b, use, fx, fy):
         """View b's backward pass after its forward pass: rasterize-backward into colour slot b, then projection
