@@ -227,50 +227,21 @@ class SplatTrainer:
         tensor {total, L1, SSIM}.  At B > 1: cam is a sequence of B cameras, gt B images (a sequence or a [B,H,W,3]
         tensor), and the result is the device [B,3] tensor of the views' {total, L1, SSIM}.  The next step overwrites
         the result.  Raises ValueError on a wrong number of views, mixed resolutions or a wrong image."""
-        pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
-        B = self.views_per_step
+        pp, B = self.pipe, self.views_per_step
         gts = [gt] if B == 1 else gt
-        setups, H, W = view_setups(cam, gts, B, downscale_factor(step, self.num_downscales, self.resolution_schedule))
-        if (W, H) != self.resolution:
-            self._set_resolution(W, H)
-        # One upload of the B cameras; the previous step's last host wait came after the last upload of this block.
-        host = self.cams_host
-        for b, (_, _, _, view, proj, cam_pos) in enumerate(setups):
-            host[16 * b:16 * b + 16].copy_(view.reshape(16))
-            host[16 * (B + b):16 * (B + b) + 16].copy_(proj.reshape(16))
-            host[32 * B + 3 * b:32 * B + 3 * b + 3].copy_(cam_pos)
-        self.cams_dev.copy_(host, non_blocking=True)
-        n, p, tb = pp.n, pp.p, pp.tb
-        use = min(step // self.sh_degree_interval, self.sh_degree)
         # ---- forward, enqueued without a host wait until each view's binning read-back ----
-        if B == 1:
-            # `proj @ view` as GaussianModel forms it, and the one-view SH forward
-            torch.matmul(self.projs[0], self.viewmats[0], out=self.projmats[0])
-            capi.check(L.gsb_sh_forward_rgb_cam(n, pp.deg, use, P(p["means"]), P(self.cam_positions[0]),
-                                                P(p["coeffs"]), 0.5, P(self.rgbs_views), s))
-        else:
-            torch.matmul(self.projs, self.viewmats, out=self.projmats)
-            capi.check(L.gsb_sh_forward_rgb_cam_multiview(n, pp.deg, use, P(p["means"]), B, P(self.cam_positions),
-                                                          P(p["coeffs"]), 0.5, P(self.rgbs_views), s))
+        setups, H, W, use = self._setup_views(cam, gts, B, step)
         visible = []
         for b in range(B):
-            fx, fy, cx, cy = setups[b][2]
-            capi.check(L.gsb_project_forward_activated(
-                n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmats[b]),
-                P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
-                P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac), s))
-            pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[b])
-            off = (-self.ssim_ws.data_ptr()) % 256
-            capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gts[b]), self.ssim_weight, P(pp.v_img),
-                                          P(self.losses[b]), self.ssim_ws.data_ptr() + off,
-                                          self.ssim_ws.numel() - off, s))
+            intr = setups[b][2]
+            self._render_view(b, intr, gts[b], self.losses[b])
             visible.append(pp.plan.visible > 0)
             # model.cpp:173-174: a lone view that hits nothing trains nothing.  Next to other views, or data-parallel
             # with more than one rank, its backward pass runs and writes zero gradients (no Gaussian has radii > 0):
             # the sum over the views and the divisor B x G stay as they are, and the rank takes the exchange's
             # barriers.
             if B > 1 or visible[b] or self.world > 1:
-                self._backward_view(b, use, fx, fy)
+                self._backward_view(b, use, intr[0], intr[1])
             # this view's densification statistics (pp.v_xy / pp.radii are overwritten by the next view)
             self.densifier.accumulate_view(step, pp.v_xy if visible[b] else None, pp.radii, H, W)
         # A step whose views all hit nothing trains nothing; with more than one rank it still takes part in the step
@@ -299,32 +270,53 @@ class SplatTrainer:
         back, each counted in `pixel_reallocs`; and the binning buffers grow if the view needs more intersections
         than they hold (a step grows them the same way, with no effect on its result).  Raises ValueError on a
         wrong image."""
-        pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
-        B = self.views_per_step
-        setups, H, W = view_setups(cam, [gt], 1, downscale_factor(step, self.num_downscales, self.resolution_schedule))
+        setups = self._setup_views(cam, [gt], 1, step)[0]
+        self._render_view(0, setups[0][2], gt, self.eval_loss)
+        return self.eval_loss
+
+    def _setup_views(self, cams, gts, views, step):
+        """What the forward passes of a step's `views` views share: view_setups at `step`'s downscale factor, the
+        render resolution, one upload of the cameras into slots 0..views-1 of the camera block (the last host wait, a
+        binning read-back, came after the block's previous upload), `proj @ view` and the SH colours.  One view takes
+        the 2-D matmul and the one-view SH forward (see the module docstring).  Returns (setups, H, W, use): use is
+        the step's SH degrees_to_use."""
+        setups, H, W = view_setups(cams, gts, views, downscale_factor(step, self.num_downscales,
+                                                                       self.resolution_schedule))
         if (W, H) != self.resolution:
             self._set_resolution(W, H)
-        _, _, (fx, fy, cx, cy), view, proj, cam_pos = setups[0]
-        # slot 0 of the camera block; the last host wait (a binning read-back) came after the block's last upload
-        host = self.cams_host
-        host[:16].copy_(view.reshape(16))
-        host[16 * B:16 * B + 16].copy_(proj.reshape(16))
-        host[32 * B:32 * B + 3].copy_(cam_pos)
+        pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
+        host, B, n, p = self.cams_host, self.views_per_step, pp.n, pp.p
+        for b, (_, _, _, view, proj, cam_pos) in enumerate(setups):
+            host[16 * b:16 * b + 16].copy_(view.reshape(16))
+            host[16 * (B + b):16 * (B + b) + 16].copy_(proj.reshape(16))
+            host[32 * B + 3 * b:32 * B + 3 * b + 3].copy_(cam_pos)
         self.cams_dev.copy_(host, non_blocking=True)
-        n, p, tb = pp.n, pp.p, pp.tb
         use = min(step // self.sh_degree_interval, self.sh_degree)
-        torch.matmul(self.projs[0], self.viewmats[0], out=self.projmats[0])
-        capi.check(L.gsb_sh_forward_rgb_cam(n, pp.deg, use, P(p["means"]), P(self.cam_positions[0]),
-                                            P(p["coeffs"]), 0.5, P(self.rgbs_views[0]), s))
+        if views == 1:
+            torch.matmul(self.projs[0], self.viewmats[0], out=self.projmats[0])
+            capi.check(L.gsb_sh_forward_rgb_cam(n, pp.deg, use, P(p["means"]), P(self.cam_positions[0]),
+                                                P(p["coeffs"]), 0.5, P(self.rgbs_views[0]), s))
+        else:
+            torch.matmul(self.projs, self.viewmats, out=self.projmats)
+            capi.check(L.gsb_sh_forward_rgb_cam_multiview(n, pp.deg, use, P(p["means"]), views, P(self.cam_positions),
+                                                          P(p["coeffs"]), 0.5, P(self.rgbs_views), s))
+        return setups, H, W, use
+
+    def _render_view(self, b, intr, gt, loss):
+        """View b's forward pass after _setup_views: projection with the activations from camera slot b (intrinsics
+        `intr`), binning and the clamped blend into the pipeline's image (the view's one host wait), then the loss
+        against gt into `loss` ({total, L1, SSIM}) and its image gradient into the pipeline's v_img."""
+        pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
+        n, p, tb, H, W = pp.n, pp.p, pp.tb, pp.H, pp.W
+        fx, fy, cx, cy = intr
         capi.check(L.gsb_project_forward_activated(
-            n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmats[0]),
-            P(self.projmats[0]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
+            n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmats[b]),
+            P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
             P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac), s))
-        pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[0])
+        pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[b])
         off = (-self.ssim_ws.data_ptr()) % 256
-        capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(self.eval_loss),
+        capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(loss),
                                       self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off, s))
-        return self.eval_loss
 
     def _backward_view(self, b, use, fx, fy):
         """View b's backward pass after its forward pass: rasterize-backward into colour slot b, then projection
