@@ -285,8 +285,12 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
         const float vttx = -fx * rz2 * vJ02, vtty = -fy * rz2 * vJ12;
         vtz += -fx * rz2 * vJ00 + 2.f * fx * ttx * rz3 * vJ02 - fy * rz2 * vJ11 +
                2.f * fy * tty * rz3 * vJ12;
-        if (clamp_x) vtz += cqx * vttx; else vtx += vttx;
-        if (clamp_y) vtz += cqy * vtty; else vty += vtty;
+        // D16: exactly on +-lim the reference's min(lim, max(-lim, q)) splits the gradient in half between the
+        // branches: half to t.x, and 0.5 cq to t.z
+        if (qx == lim_x || qx == -lim_x) { const float h = 0.5f * vttx; vtx += h; vtz += cqx * h; }
+        else if (clamp_x) vtz += cqx * vttx; else vtx += vttx;
+        if (qy == lim_y || qy == -lim_y) { const float h = 0.5f * vtty; vty += h; vtz += cqy * h; }
+        else if (clamp_y) vtz += cqy * vtty; else vty += vtty;
         vm[0] += V[0] * vtx + V[4] * vty + V[8] * vtz;
         vm[1] += V[1] * vtx + V[5] * vty + V[9] * vtz;
         vm[2] += V[2] * vtx + V[6] * vty + V[10] * vtz;

@@ -375,8 +375,11 @@ void orc_project_backward(int n, const float *means3d, const float *scales, floa
         float vttx = -fx * rz2 * vJ02, vtty = -fy * rz2 * vJ12;
         vtz += -fx * rz2 * vJ00 + 2.f * fx * ttx * rz3 * vJ02 - fy * rz2 * vJ11 +
                2.f * fy * tty * rz3 * vJ12;
-        if (clamp_x) vtz += cqx * vttx; else vtx += vttx;
-        if (clamp_y) vtz += cqy * vtty; else vty += vtty;
+        /* exactly on +-lim torch's min/max split the gradient in half between the branches (D16) */
+        if (qx == lim_x || qx == -lim_x) { float h = 0.5f * vttx; vtx += h; vtz += cqx * h; }
+        else if (clamp_x) vtz += cqx * vttx; else vtx += vttx;
+        if (qy == lim_y || qy == -lim_y) { float h = 0.5f * vtty; vty += h; vtz += cqy * h; }
+        else if (clamp_y) vtz += cqy * vtty; else vty += vtty;
         vmx += V[0] * vtx + V[4] * vty + V[8] * vtz;
         vmy += V[1] * vtx + V[5] * vty + V[9] * vtz;
         vmz += V[2] * vtx + V[6] * vty + V[10] * vtz;

@@ -57,13 +57,19 @@ def test_rasterize_forward_backward_match_reference(name, gtol):
     assert rel_l2(r["v_conic"], g["ref_v_conic"]) <= gtol
 
 
-@pytest.mark.parametrize("name,_", CASES)
+@pytest.mark.parametrize("name,_", CASES + [("projection_general", None), ("projection_ties", None)])
 def test_projection_backward_matches_reference_autograd(name, _):
+    """projection_*: general cameras (fov clamp, perspective divide, rotation in T = J V, glob_scale 1.3) and exact
+    fov-clamp ties (D16); their cotangents are zero for the Gaussians the CUDA semantics cull."""
     g = load_golden(name)
-    p, (fx, fy, cx, cy, H, W) = _project(g)
-    r = orc.project_backward(g["means"], g["scales"], 1.0, g["quats"], g["viewmat"], g["projmat"],
-                             fx, fy, cx, cy, H, W, p["radii"], p["conics"], g["ref_v_xy"], None,
-                             g["ref_v_conic"])
+    fx, fy, cx, cy = g["intrins"]
+    H, W = [int(v) for v in g["hw"]]
+    gs = float(g.get("glob_scale", 1.0))
+    p = orc.project_forward(g["means"], g["scales"], gs, g["quats"], g["viewmat"], g["projmat"], fx, fy, cx, cy, H, W,
+                            float(g.get("clip_thresh", 0.01)))
+    r = orc.project_backward(g["means"], g["scales"], gs, g["quats"], g["viewmat"], g["projmat"],
+                             fx, fy, cx, cy, H, W, p["radii"], p["conics"], g.get("v_xy", g.get("ref_v_xy")), None,
+                             g.get("v_conic", g.get("ref_v_conic")))
     assert rel_l2(r["v_mean3d"], g["ref_v_means"]) <= 1e-4
     assert rel_l2(r["v_scale"], g["ref_v_scales"]) <= 1e-4
     assert rel_l2(r["v_quat"], g["ref_v_quats"]) <= 1e-4
