@@ -215,7 +215,7 @@ class SplatPipeline(BinFrame):
             else:
                 self.exchange.exchange(average=True)
         else:
-            # SH VJP with the gradient of the clamp fused (mask = forward rgbs > 0)
+            # SH VJP with the gradient of the clamp fused (mask = forward rgbs > 0 or -0, the exact tie: D17)
             capi.check(L.gsb_sh_backward_rgb(n, self.deg, self.deg, P(self.viewdirs), P(self.rgbs), P(self.v_rgbs),
                                              P(g["coeffs"]), s))
         self._stage("end_bwd")

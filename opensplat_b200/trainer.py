@@ -354,8 +354,9 @@ class SplatTrainer:
             capi.check(L.gsb_sh_backward_rgb_cam(n, pp.deg, use, P(p["means"]), P(self.cam_positions[0]),
                                                  P(self.rgbs_views), P(self.v_rgb_views), P(g["coeffs"]), s))
         else:
-            # The clamp's gradient on the B slots and their expansion, plus the geometry prefix times 1/B (the
-            # all-reduce role at world 1), in one launch of the data-parallel exchange kernel.
+            # The clamp's gradient on the B slots (mask = rgbs > 0 or -0, the exact tie: D17) and their expansion, plus
+            # the geometry prefix times 1/B (the all-reduce role at world 1), in one launch of the data-parallel
+            # exchange kernel.
             capi.check(L.gsb_mask_rgb_grad(n * B, P(self.rgbs_views), P(self.v_rgb_views), s))
             capi.check(L.gsb_exchange_gradients(
                 n, pp.deg, use, P(p["means"]), B, P(self.cam_positions), self.rgb_ptrs.data_ptr(), 1.0 / B,
