@@ -288,7 +288,20 @@ int gsb_bucket_sort_pack(int n, int m_capacity, int len_capacity, const float *d
  *   blend epilogue: out_img is written clamped, the channels that were cut are remembered in bits 28..30 of
  *   final_idx (so m must stay below 2^28 and final_idx is private to the pair of calls), and the backward -- given
  *   the same flag and the gradient of the CLAMPED image -- passes no gradient through them (torch's clamp_max mask
- *   `x <= max`). */
+ *   `x <= max`).
+ * Depth and opacity maps (DESIGN D18): the blend's decisions are those of the colour blend; per pixel
+ *   out_depth = sum alpha T z over the blended pairs (z = the projection's view-space depth of the pair's Gaussian,
+ *   background depth 0, not normalised) and out_alpha = 1 - final_Ts.  Neither is ever clamped.
+ * gsb_gather_record_depths: record_depths [m] = depths[gaussian_ids_sorted[j]], the per-record depth stream in sorted
+ *   order.  m = the size of the id list (the m_capacity on the fast path, where gsb_bucket_sort_pack writes
+ *   gaussian_ids_sorted); given the binning stats it reads M from them on the device, writes only j < M, and writes
+ *   nothing after an overflow.  bin_stats may be NULL (generic path: all m ids are valid).
+ * gsb_rasterize_forward_packed_depth: gsb_rasterize_forward_packed plus record_depths [m] (may be NULL if m == 0),
+ *   out_depth [H,W] and out_alpha [H,W], written completely.  out_img, final_Ts and final_idx are bit-identical to
+ *   gsb_rasterize_forward_packed's.
+ * gsb_rasterize_backward_depth: gsb_rasterize_backward plus record_depths, v_output_depth [H,W] (NULL == zeros) and
+ *   v_depths [n], written completely.  v_output_alpha is the cotangent of out_alpha.  Give it the records, final_Ts
+ *   and final_idx of gsb_rasterize_forward_packed_depth (or of gsb_rasterize_forward_packed: they are the same). */
 size_t gsb_raster_records_bytes(int m);
 size_t gsb_raster_grad_rows_bytes(int m);
 int gsb_pack_records(int m, const int32_t *gaussian_ids_sorted, const int32_t *sorted_index, const float *xys,
@@ -307,6 +320,21 @@ int gsb_rasterize_backward(int img_h, int img_w, int tiles_x, int tiles_y, int n
                            const int32_t *final_idx, const float *v_output, const float *v_output_alpha,
                            void *grad_rows, float *v_xy, float *v_conic, float *v_colors, float *v_opacity,
                            unsigned flags, gsb_stream_t stream);
+int gsb_gather_record_depths(int m, const int32_t *gaussian_ids_sorted, const float *depths, const int32_t *bin_stats,
+                             float *record_depths, gsb_stream_t stream);
+int gsb_rasterize_forward_packed_depth(int img_h, int img_w, int tiles_x, int tiles_y, int m, const int32_t *tile_bins,
+                                       const int32_t *tile_order, const int32_t *bin_stats, const float *background,
+                                       void *records, float *out_img, float *final_Ts, int32_t *final_idx,
+                                       unsigned flags, const float *record_depths, float *out_depth, float *out_alpha,
+                                       gsb_stream_t stream);
+int gsb_rasterize_backward_depth(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
+                                 const int32_t *tile_bins, const int32_t *tile_order, const float *conics,
+                                 const float *opacities, void *records, const int32_t *cum_tiles_hit,
+                                 const float *background, const float *final_Ts, const int32_t *final_idx,
+                                 const float *v_output, const float *v_output_alpha, void *grad_rows, float *v_xy,
+                                 float *v_conic, float *v_colors, float *v_opacity, unsigned flags,
+                                 const float *record_depths, const float *v_output_depth, float *v_depths,
+                                 gsb_stream_t stream);
 
 /* ---- Streaming helpers around the path (SURVEY.md 8f "next" rows) ------------------------------
  * gsb_mse_loss_grad: loss = mean((img-target)^2) written to *loss_out (device float; zeroed by the

@@ -59,6 +59,11 @@ _SIGS = {
     "gsb_rasterize_forward_count": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_rasterize_backward": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                     _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint, _vp]),
+    "gsb_gather_record_depths": (_i, [_i, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_rasterize_forward_packed_depth": (_i, [_i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint,
+                                                _vp, _vp, _vp, _vp]),
+    "gsb_rasterize_backward_depth": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                          _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint, _vp, _vp, _vp, _vp]),
     "gsb_bucket_max_tile_len": (_i, []),
     "gsb_bucket_workspace_bytes": (_sz, [_i, _i, _i]),
     "gsb_bucket_tile_ranges": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),

@@ -193,6 +193,38 @@ torch::autograd::tensor_list RasterizeGaussiansClamped::backward(torch::autograd
     return rasterizeBackward(ctx, grad_outputs);
 }
 
+torch::autograd::variable_list RasterizeGaussiansDepth::forward(torch::autograd::AutogradContext *ctx,
+                                                                torch::Tensor xys, torch::Tensor depths,
+                                                                torch::Tensor radii, torch::Tensor conics,
+                                                                torch::Tensor numTilesHit, torch::Tensor colors,
+                                                                torch::Tensor opacity, int imgHeight, int imgWidth,
+                                                                torch::Tensor background) {
+    DepthMaps maps;
+    torch::Tensor rgb = rasterizeForward(ctx, 0u, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight,
+                                         imgWidth, background, &maps);
+    return {rgb, maps.depth, maps.alpha};
+}
+
+torch::autograd::tensor_list RasterizeGaussiansDepth::backward(torch::autograd::AutogradContext *ctx,
+                                                               torch::autograd::tensor_list grad_outputs) {
+    return rasterizeBackward(ctx, grad_outputs);
+}
+
+torch::autograd::variable_list RasterizeGaussiansDepthClamped::forward(
+    torch::autograd::AutogradContext *ctx, torch::Tensor xys, torch::Tensor depths, torch::Tensor radii,
+    torch::Tensor conics, torch::Tensor numTilesHit, torch::Tensor colors, torch::Tensor opacity, int imgHeight,
+    int imgWidth, torch::Tensor background) {
+    DepthMaps maps;
+    torch::Tensor rgb = rasterizeForward(ctx, GSB_RASTER_CLAMP_MAX_ONE, xys, depths, radii, conics, numTilesHit,
+                                         colors, opacity, imgHeight, imgWidth, background, &maps);
+    return {rgb, maps.depth, maps.alpha};
+}
+
+torch::autograd::tensor_list RasterizeGaussiansDepthClamped::backward(torch::autograd::AutogradContext *ctx,
+                                                                      torch::autograd::tensor_list grad_outputs) {
+    return rasterizeBackward(ctx, grad_outputs);
+}
+
 ModelForwardResult modelForward(const torch::Tensor &means, const torch::Tensor &logScales,
                                 const torch::Tensor &rawQuats, const torch::Tensor &featuresDc,
                                 const torch::Tensor &featuresRest, const torch::Tensor &opacityLogits,

@@ -78,6 +78,35 @@ public:
                                                  torch::autograd::tensor_list grad_outputs);
 };
 
+// RasterizeGaussians with the depth and opacity maps (DESIGN D18): same arguments, returns {rgb [H,W,3], depth [H,W],
+// alpha [H,W]}: depth = sum alpha T z over the pairs the colour blend blends (z = `depths`, the projection's view-space
+// depth; background 0, not normalised), alpha = 1 - T_final.  rgb is bit-identical to RasterizeGaussians'.  Gradients
+// for xys (0), depths (1), conics (3), colors (5), opacity (6): composed with ProjectGaussians[Activated], a depth loss
+// reaches the means.
+class RasterizeGaussiansDepth : public torch::autograd::Function<RasterizeGaussiansDepth> {
+public:
+    static torch::autograd::variable_list forward(torch::autograd::AutogradContext *ctx, torch::Tensor xys,
+                                                  torch::Tensor depths, torch::Tensor radii, torch::Tensor conics,
+                                                  torch::Tensor numTilesHit, torch::Tensor colors,
+                                                  torch::Tensor opacity, int imgHeight, int imgWidth,
+                                                  torch::Tensor background);
+    static torch::autograd::tensor_list backward(torch::autograd::AutogradContext *ctx,
+                                                 torch::autograd::tensor_list grad_outputs);
+};
+
+// RasterizeGaussiansDepth with rgb = clamp_max(rgb, 1) fused as in RasterizeGaussiansClamped (what Model::forward
+// renders); depth and alpha are never clamped.
+class RasterizeGaussiansDepthClamped : public torch::autograd::Function<RasterizeGaussiansDepthClamped> {
+public:
+    static torch::autograd::variable_list forward(torch::autograd::AutogradContext *ctx, torch::Tensor xys,
+                                                  torch::Tensor depths, torch::Tensor radii, torch::Tensor conics,
+                                                  torch::Tensor numTilesHit, torch::Tensor colors,
+                                                  torch::Tensor opacity, int imgHeight, int imgWidth,
+                                                  torch::Tensor background);
+    static torch::autograd::tensor_list backward(torch::autograd::AutogradContext *ctx,
+                                                 torch::autograd::tensor_list grad_outputs);
+};
+
 // Model::forward (model.cpp:82-225) with every glue op fused, on plain tensors -- what a maintainer calls from the
 // body of Model::forward to opt in (INTEGRATION.md):
 //     auto r = gsb::modelForward(means, scales, quats, featuresDc, featuresRest, opacities, backgroundColor,

@@ -31,11 +31,17 @@ inline torch::TensorOptions like(const torch::Tensor &t, torch::ScalarType dt) {
 
 
 // Bodies of RasterizeGaussians::forward / backward with the GSB_RASTER_* flags of the blend kernels
-// (rasterize_gaussians.cpp); shared with gsb::RasterizeGaussiansClamped (fused_extras.cpp).
+// (rasterize_gaussians.cpp); shared with gsb::RasterizeGaussiansClamped and gsb::RasterizeGaussiansDepth[Clamped]
+// (fused_extras.cpp).  Given depthOut, the forward also renders the depth and opacity maps into depthOut->depth /
+// depthOut->alpha (DESIGN D18) and the backward then takes grad_outputs {rgb, depth, alpha} and returns v_depths in
+// slot 1.
+struct DepthMaps {
+    torch::Tensor depth, alpha;
+};
 torch::Tensor rasterizeForward(torch::autograd::AutogradContext *ctx, unsigned flags, torch::Tensor xys,
                                torch::Tensor depths, torch::Tensor radii, torch::Tensor conics,
                                torch::Tensor numTilesHit, torch::Tensor colors, torch::Tensor opacity, int imgHeight,
-                               int imgWidth, torch::Tensor background);
+                               int imgWidth, torch::Tensor background, DepthMaps *depthOut = nullptr);
 torch::autograd::tensor_list rasterizeBackward(torch::autograd::AutogradContext *ctx,
                                                torch::autograd::tensor_list grad_outputs);
 

@@ -109,11 +109,12 @@ inline char *align256(torch::Tensor &t) {
 namespace gsb {
 
 // Body of RasterizeGaussians::forward; `flags` = GSB_RASTER_* (gsb::RasterizeGaussiansClamped passes
-// GSB_RASTER_CLAMP_MAX_ONE: clamp_max(rgb, 1) fused into the blend kernels, fused_extras.hpp).
+// GSB_RASTER_CLAMP_MAX_ONE: clamp_max(rgb, 1) fused into the blend kernels, fused_extras.hpp); depthOut: see
+// gsb_torch.hpp.
 torch::Tensor rasterizeForward(AutogradContext *ctx, unsigned flags, torch::Tensor xys, torch::Tensor depths,
                                torch::Tensor radii, torch::Tensor conics, torch::Tensor numTilesHit,
                                torch::Tensor colors, torch::Tensor opacity, int imgHeight, int imgWidth,
-                               torch::Tensor background) {
+                               torch::Tensor background, DepthMaps *depthOut) {
     const int n = (int)xys.size(0);
     TORCH_CHECK(colors.size(-1) == 3, "RasterizeGaussians: only 3 colour channels are supported");
     c10::cuda::CUDAGuard guard(xys.device());
@@ -134,6 +135,28 @@ torch::Tensor rasterizeForward(AutogradContext *ctx, unsigned flags, torch::Tens
     torch::Tensor finalTs = torch::empty({imgHeight, imgWidth}, gsb::like(x, torch::kFloat32));
     torch::Tensor finalIdx = torch::empty({imgHeight, imgWidth}, gsb::like(x, torch::kInt32));
     torch::Tensor records;
+    // depth output: the sorted Gaussian ids and the per-record depth stream gathered from them
+    const bool depth = depthOut != nullptr;
+    torch::Tensor gidsSorted, recordDepths;
+    if (depth) {
+        depthOut->depth = torch::empty({imgHeight, imgWidth}, gsb::like(x, torch::kFloat32));
+        depthOut->alpha = torch::empty({imgHeight, imgWidth}, gsb::like(x, torch::kFloat32));
+    }
+    // the blend of the frame: the plain or the DEPTH kernel on the same records
+    auto blend = [&](int m, const int32_t *bins, const int32_t *order, const int32_t *st) {
+        if (depth)
+            gsb::check(gsb_rasterize_forward_packed_depth(
+                           imgHeight, imgWidth, tilesX, tilesY, m, bins, order, st, gsb::fp(bg), records.data_ptr(),
+                           gsb::fpw(outImg), gsb::fpw(finalTs), finalIdx.data_ptr<int32_t>(), flags,
+                           gsb::fp(recordDepths), gsb::fpw(depthOut->depth), gsb::fpw(depthOut->alpha), gsb::stream()),
+                       "gsb_rasterize_forward_packed_depth");
+        else
+            gsb::check(gsb_rasterize_forward_packed(imgHeight, imgWidth, tilesX, tilesY, m, bins, order, st,
+                                                    gsb::fp(bg), records.data_ptr(), gsb::fpw(outImg),
+                                                    gsb::fpw(finalTs), finalIdx.data_ptr<int32_t>(), flags,
+                                                    gsb::stream()),
+                       "gsb_rasterize_forward_packed");
+    };
     torch::Tensor &statsHost = statsHostFor(dev);
     const int limit = gsb_bucket_max_tile_len();
     int mRaster = 0;   // what the records buffer is sized with (the blend kernels' scratch words sit behind it)
@@ -153,17 +176,22 @@ torch::Tensor rasterizeForward(AutogradContext *ctx, unsigned flags, torch::Tens
         statsHost.copy_(stats, /*non_blocking=*/true);
         at::cuda::CUDAEvent statsReady;
         statsReady.record(c10::cuda::getCurrentCUDAStream());
+        if (depth) {
+            gidsSorted = torch::empty({std::max(mCap, 1)}, gsb::like(x, torch::kInt32));
+            recordDepths = torch::empty({std::max(mCap, 1)}, gsb::like(x, torch::kFloat32));
+        }
         if (mCap > 0)
             gsb::check(gsb_bucket_sort_pack(n, mCap, lenCap, gsb::fp(d), r.data_ptr<int32_t>(),
                                             cum.data_ptr<int32_t>(), cull, tilesX, tilesY,
                                             tileBins.data_ptr<int32_t>(), stats.data_ptr<int32_t>(), wp, wsBytes,
-                                            records.data_ptr(), nullptr, nullptr, gsb::stream()),
+                                            records.data_ptr(), nullptr,
+                                            depth ? gidsSorted.data_ptr<int32_t>() : nullptr, gsb::stream()),
                        "gsb_bucket_sort_pack");
-        gsb::check(gsb_rasterize_forward_packed(imgHeight, imgWidth, tilesX, tilesY, mCap, tileBins.data_ptr<int32_t>(),
-                                                tileOrder.data_ptr<int32_t>(), stats.data_ptr<int32_t>(), gsb::fp(bg),
-                                                records.data_ptr(), gsb::fpw(outImg), gsb::fpw(finalTs),
-                                                finalIdx.data_ptr<int32_t>(), flags, gsb::stream()),
-                   "gsb_rasterize_forward_packed");
+        if (depth && n > 0)   // the ids past M hold nothing valid: the gather reads M from the stats
+            gsb::check(gsb_gather_record_depths(mCap, gidsSorted.data_ptr<int32_t>(), gsb::fp(d),
+                                                stats.data_ptr<int32_t>(), gsb::fpw(recordDepths), gsb::stream()),
+                       "gsb_gather_record_depths");
+        blend(mCap, tileBins.data_ptr<int32_t>(), tileOrder.data_ptr<int32_t>(), stats.data_ptr<int32_t>());
         // the path's single device->host read-back (rasterize_gaussians.cpp:63), waited for with the GPU busy
         statsReady.synchronize();
         const int32_t *sh = statsHost.data_ptr<int32_t>();
@@ -192,11 +220,13 @@ torch::Tensor rasterizeForward(AutogradContext *ctx, unsigned flags, torch::Tens
                                     gsb::fp(x), gsb::fp(con), gsb::fp(col), gsb::fp(op), records.data_ptr(),
                                     gsb::stream()),
                    "gsb_pack_records");
-        gsb::check(gsb_rasterize_forward_packed(imgHeight, imgWidth, tilesX, tilesY, mRef,
-                                                b.tileBins.data_ptr<int32_t>(), nullptr, nullptr, gsb::fp(bg),
-                                                records.data_ptr(), gsb::fpw(outImg), gsb::fpw(finalTs),
-                                                finalIdx.data_ptr<int32_t>(), flags, gsb::stream()),
-                   "gsb_rasterize_forward_packed");
+        if (depth) {
+            recordDepths = torch::empty({std::max(mRef, 1)}, gsb::like(x, torch::kFloat32));
+            gsb::check(gsb_gather_record_depths(mRef, b.gaussianIdsSorted.data_ptr<int32_t>(), gsb::fp(d), nullptr,
+                                                gsb::fpw(recordDepths), gsb::stream()),
+                       "gsb_gather_record_depths");
+        }
+        blend(mRef, b.tileBins.data_ptr<int32_t>(), nullptr, nullptr);
         mRaster = mRef;
         ordered = false;
         break;
@@ -207,9 +237,51 @@ torch::Tensor rasterizeForward(AutogradContext *ctx, unsigned flags, torch::Tens
     ctx->saved_data["numIntersects"] = mRaster;
     ctx->saved_data["ordered"] = ordered;
     ctx->saved_data["flags"] = (int64_t)flags;
-    ctx->save_for_backward({tileBins, con, op, records, cum, bg, finalTs, finalIdx, tileOrder});
+    ctx->saved_data["depth"] = depth;
+    if (depth)
+        ctx->save_for_backward({tileBins, con, op, records, cum, bg, finalTs, finalIdx, tileOrder, recordDepths});
+    else
+        ctx->save_for_backward({tileBins, con, op, records, cum, bg, finalTs, finalIdx, tileOrder});
     return outImg;
 }
+
+namespace {
+
+// rasterizeBackward of a frame rendered with the depth and opacity maps: grad_outputs {rgb, depth, alpha}, any of
+// them undefined (zeros); gradients for xys (0), depths (1), conics (3), colors (5), opacity (6).
+tensor_list rasterizeBackwardDepth(AutogradContext *ctx, const variable_list &saved, const tensor_list &grad_outputs) {
+    const unsigned flags = (unsigned)ctx->saved_data["flags"].toInt();
+    const int imgHeight = (int)ctx->saved_data["imgHeight"].toInt();
+    const int imgWidth = (int)ctx->saved_data["imgWidth"].toInt();
+    const int m = (int)ctx->saved_data["numIntersects"].toInt();
+    torch::Tensor tileBins = saved[0], con = saved[1], op = saved[2], records = saved[3], cum = saved[4];
+    torch::Tensor bg = saved[5], finalTs = saved[6], finalIdx = saved[7], tileOrder = saved[8], recordDepths = saved[9];
+    const bool ordered = ctx->saved_data["ordered"].toBool();
+    const int n = (int)con.size(0);
+    torch::Tensor v_out = grad_outputs[0].defined() ? gsb::f32(grad_outputs[0])
+                                                    : torch::zeros({imgHeight, imgWidth, 3}, gsb::like(con, torch::kFloat32));
+    torch::Tensor v_depth = grad_outputs[1].defined() ? gsb::f32(grad_outputs[1]) : torch::Tensor();
+    torch::Tensor v_alpha = grad_outputs[2].defined() ? gsb::f32(grad_outputs[2]) : torch::Tensor();
+    torch::Tensor rows = torch::empty({(int64_t)gsb_raster_grad_rows_bytes(m)}, gsb::like(con, torch::kUInt8));
+    torch::Tensor v_xy = torch::empty({n, 2}, gsb::like(con, torch::kFloat32));
+    torch::Tensor v_conic = torch::empty({n, 3}, gsb::like(con, torch::kFloat32));
+    torch::Tensor v_colors = torch::empty({n, 3}, gsb::like(con, torch::kFloat32));
+    torch::Tensor v_opacity = torch::empty({n, 1}, gsb::like(con, torch::kFloat32));
+    torch::Tensor v_depths = torch::empty({n}, gsb::like(con, torch::kFloat32));
+    gsb::check(gsb_rasterize_backward_depth(
+                   imgHeight, imgWidth, (imgWidth + BLOCK_X - 1) / BLOCK_X, (imgHeight + BLOCK_Y - 1) / BLOCK_Y, n, m,
+                   tileBins.data_ptr<int32_t>(), ordered ? tileOrder.data_ptr<int32_t>() : nullptr, gsb::fp(con),
+                   gsb::fp(op), records.data_ptr(), cum.data_ptr<int32_t>(), gsb::fp(bg), gsb::fp(finalTs),
+                   finalIdx.data_ptr<int32_t>(), gsb::fp(v_out), v_alpha.defined() ? gsb::fp(v_alpha) : nullptr,
+                   rows.data_ptr(), gsb::fpw(v_xy), gsb::fpw(v_conic), gsb::fpw(v_colors), gsb::fpw(v_opacity), flags,
+                   gsb::fp(recordDepths), v_depth.defined() ? gsb::fp(v_depth) : nullptr, gsb::fpw(v_depths),
+                   gsb::stream()),
+               "gsb_rasterize_backward_depth");
+    torch::Tensor none;
+    return {v_xy, v_depths, none, v_conic, none, v_colors, v_opacity, none, none, none};
+}
+
+}  // namespace
 
 tensor_list rasterizeBackward(AutogradContext *ctx, tensor_list grad_outputs) {
     const unsigned flags = (unsigned)ctx->saved_data["flags"].toInt();
@@ -222,6 +294,7 @@ tensor_list rasterizeBackward(AutogradContext *ctx, tensor_list grad_outputs) {
     const bool ordered = ctx->saved_data["ordered"].toBool();
     const int n = (int)con.size(0);
     c10::cuda::CUDAGuard guard(con.device());
+    if (ctx->saved_data["depth"].toBool()) return rasterizeBackwardDepth(ctx, saved, grad_outputs);
     torch::Tensor v_out = gsb::f32(grad_outputs[0]);  // may arrive as an expanded (stride-0) tensor
     torch::Tensor rows = torch::empty({(int64_t)gsb_raster_grad_rows_bytes(m)}, gsb::like(con, torch::kUInt8));
     torch::Tensor v_xy = torch::empty({n, 2}, gsb::like(con, torch::kFloat32));

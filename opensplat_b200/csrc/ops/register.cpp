@@ -78,9 +78,28 @@ static torch::Tensor op_rasterize_clamped(torch::Tensor xys, torch::Tensor depth
                                                  (int)imgHeight, (int)imgWidth, background);
 }
 
+static std::vector<torch::Tensor> op_rasterize_depth(torch::Tensor xys, torch::Tensor depths, torch::Tensor radii,
+                                                     torch::Tensor conics, torch::Tensor numTilesHit,
+                                                     torch::Tensor colors, torch::Tensor opacity, int64_t imgHeight,
+                                                     int64_t imgWidth, torch::Tensor background) {
+    return gsb::RasterizeGaussiansDepth::apply(xys, depths, radii, conics, numTilesHit, colors, opacity, (int)imgHeight,
+                                               (int)imgWidth, background);
+}
+
+static std::vector<torch::Tensor> op_rasterize_depth_clamped(torch::Tensor xys, torch::Tensor depths,
+                                                             torch::Tensor radii, torch::Tensor conics,
+                                                             torch::Tensor numTilesHit, torch::Tensor colors,
+                                                             torch::Tensor opacity, int64_t imgHeight,
+                                                             int64_t imgWidth, torch::Tensor background) {
+    return gsb::RasterizeGaussiansDepthClamped::apply(xys, depths, radii, conics, numTilesHit, colors, opacity,
+                                                      (int)imgHeight, (int)imgWidth, background);
+}
+
 TORCH_LIBRARY(opensplat_b200, m) {
     m.def("project_gaussians_activated", &op_project_activated);
     m.def("rasterize_gaussians_clamped", &op_rasterize_clamped);
+    m.def("rasterize_gaussians_depth", &op_rasterize_depth);
+    m.def("rasterize_gaussians_depth_clamped", &op_rasterize_depth_clamped);
     m.def("activate_gaussians", &op_activate);
     m.def("spherical_harmonics_rgb", &op_sh_rgb);
     m.def("project_gaussians", &op_project);

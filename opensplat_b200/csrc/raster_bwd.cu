@@ -43,14 +43,19 @@ __device__ __forceinline__ void zero_row(float *grad_rows, int k) {
 constexpr int BWD_MIN_BLOCKS = 6;
 // SAT: v_output is the gradient w.r.t. the CLAMPED image of the forward kernel's SAT instantiation -- channels
 // marked as cut in final_idx bits 28..30 receive no gradient (clamp_max's mask, model.cpp:222).
-template <bool SAT>
-__global__ void __launch_bounds__(RK_THREADS, BWD_MIN_BLOCKS)
+// DEPTH: the VJP of the forward's DEPTH instantiation (D18).  The depth map is one more channel with background 0:
+// per pair d += z v_depth (nothing is added to Bq's initial value) and a tenth reduced value a_z = sum alpha T v_depth
+// goes to slot 9 of the gradient row.  v_output_depth may be NULL (zeros).
+constexpr int BWD_DEPTH_MIN_BLOCKS = 5;
+template <bool SAT, bool DEPTH>
+__global__ void __launch_bounds__(RK_THREADS, DEPTH ? BWD_DEPTH_MIN_BLOCKS : BWD_MIN_BLOCKS)
 rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                           const int2 *__restrict__ tile_bins, const GsbRecord *__restrict__ records,
                           const float *__restrict__ background, const float *__restrict__ final_Ts,
                           const int *__restrict__ final_idx, const float *__restrict__ v_output,
                           const float *__restrict__ v_output_alpha, float *__restrict__ grad_rows,
-                          unsigned *__restrict__ tile_counter, const int *__restrict__ tile_order) {
+                          unsigned *__restrict__ tile_counter, const int *__restrict__ tile_order,
+                          const float *__restrict__ record_depths, const float *__restrict__ v_output_depth) {
     __shared__ WarpRing rings[RK_WARPS];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     WarpRing &ring = rings[warp];
@@ -84,6 +89,7 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
         float T[RK_PIX], Bq[RK_PIX];
         const float py0 = (float)Y0;
         float vor[RK_PIX], vog[RK_PIX], vob[RK_PIX];
+        float vD[RK_PIX];   // DEPTH only
         int binf[RK_PIX];
         int my_max = -1;
 #pragma unroll
@@ -102,11 +108,13 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                     if (f & (GSB_SAT_BIT0 << 2)) vob[j] = 0.f;
                     binf[j] = f & ~GSB_SAT_MASK;
                 }
+                if (DEPTH) vD[j] = v_output_depth ? v_output_depth[p] : 0.f;
                 const float voa = v_output_alpha ? v_output_alpha[p] : 0.f;
                 // backward.cu:313-317: T_final*ra*v_out_alpha - T_final*ra*(bg . v_out)  ==  ra * q
                 Bq[j] = -(Tf * (voa - (bg0 * vor[j] + bg1 * vog[j] + bg2 * vob[j])));
             } else {
                 T[j] = 1.f; vor[j] = vog[j] = vob[j] = 0.f; Bq[j] = 0.f;
+                if (DEPTH) vD[j] = 0.f;
                 binf[j] = -1;  // never valid
             }
             my_max = max(my_max, binf[j]);
@@ -144,6 +152,9 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
 
         for (int c = 0; c < nchunks; ++c) {
             const unsigned s = stage_of(c);
+            // DEPTH: lane l loads the depth of record l of the chunk before the wait (see the forward kernel)
+            float zl = 0.f;
+            if (DEPTH && lane < chunk_cnt(c)) zl = __ldg(record_depths + chunk_lo(c) + lane);
             mbar_wait(&ring.full[s], parity_of(c));
             const int lo = chunk_lo(c), cnt = chunk_cnt(c);
             // level-1 cull: lane l tests record l; culled records get their zero row right here
@@ -157,6 +168,8 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 const int t = 31 - __clz(live);        // back to front
                 live &= ~(1u << t);
                 const unsigned rm = __shfl_sync(0xffffffffu, my_mask, t);
+                float z = 0.f;
+                if (DEPTH) z = __shfl_sync(0xffffffffu, zl, t);
                 const int idx = lo + t;
                 const float4 q0 = ring.rec[s][t].q0;
                 const float4 q1 = ring.rec[s][t].q1;
@@ -168,6 +181,7 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 const float dy0 = q0.y - py0;
                 float s0 = 0.f, s1 = 0.f, s2 = 0.f;  // sum w, sum w dy, sum w dy^2 over this lane's pixels
                 float a_r = 0.f, a_g = 0.f, a_b = 0.f;
+                float a_z = 0.f;   // DEPTH only
                 bool any = false;
                 // slots jlo..jhi inside the y-extent (contiguous); a computed jump to jlo that leaves after jhi (an
                 // A/B measurement chose it over the forward kernel's straight line of per-slot bit tests)
@@ -187,7 +201,9 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 a_r = fmaf(fac, vor[j], a_r);                                                             \
                 a_g = fmaf(fac, vog[j], a_g);                                                             \
                 a_b = fmaf(fac, vob[j], a_b);                                                             \
-                const float d = fmaf(q2.z, vob[j], fmaf(q2.y, vog[j], q2.x * vor[j])); /* rgb . v_out */  \
+                if (DEPTH) a_z = fmaf(fac, vD[j], a_z);                                                   \
+                float d = fmaf(q2.z, vob[j], fmaf(q2.y, vog[j], q2.x * vor[j])); /* rgb . v_out */        \
+                if (DEPTH) d = fmaf(z, vD[j], d);                         /* + z v_depth */               \
                 const float v_alpha = fmaf(d, T[j], -(ra * Bq[j]));                                       \
                 Bq[j] = fmaf(d, fac, Bq[j]);                                                              \
                 /* v_sigma = -opac*vis*v_alpha = -w (backward.cu:323); v_opacity += vis*v_alpha = w/opac */ \
@@ -214,7 +230,7 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 const int k = __float_as_int(q0.w);
                 float *row = grad_rows + (size_t)k * GSB_GRAD_ROW_FLOATS;
                 if (!__any_sync(0xffffffffu, any)) {
-                    if (lane < 9) row[lane] = 0.f;
+                    if (lane < (DEPTH ? 10 : 9)) row[lane] = 0.f;
                     continue;
                 }
                 // ---- one cross-lane reduction per (tile, Gaussian): 8 values by halving, 1 by butterfly
@@ -245,11 +261,24 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 }
                 v0 += __shfl_xor_sync(0xffffffffu, v0, 2);
                 v0 += __shfl_xor_sync(0xffffffffu, v0, 1);
+                if (DEPTH) {
+                    // values 8 and 9 by one halving step, then a butterfly within each half: lanes 0..15 end with the
+                    // total of value 8 (the same sums in the same order as the butterfly below), lanes 16..31 with 9
+                    const bool up = lane & 16;
+                    const float t8 = up ? v8 : a_z, k8 = up ? a_z : v8;
+                    v8 = k8 + __shfl_xor_sync(0xffffffffu, t8, 16);
 #pragma unroll
-                for (int o = 16; o > 0; o >>= 1) v8 += __shfl_xor_sync(0xffffffffu, v8, o);
-                // lane l now holds the total of value (l >> 2); lane 1 additionally stores value 8
-                const bool w8 = (lane == 1);
-                if (((lane & 3) == 0) || w8) row[w8 ? 8 : (lane >> 2)] = w8 ? v8 : v0;
+                    for (int o = 8; o > 0; o >>= 1) v8 += __shfl_xor_sync(0xffffffffu, v8, o);
+                    // lane l holds the total of value (l >> 2); lane 1 additionally stores value 8, lane 17 value 9
+                    const bool w8 = (lane == 1), w9 = (lane == 17);
+                    if (((lane & 3) == 0) || w8 || w9) row[w8 ? 8 : w9 ? 9 : (lane >> 2)] = (w8 || w9) ? v8 : v0;
+                } else {
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) v8 += __shfl_xor_sync(0xffffffffu, v8, o);
+                    // lane l now holds the total of value (l >> 2); lane 1 additionally stores value 8
+                    const bool w8 = (lane == 1);
+                    if (((lane & 3) == 0) || w8) row[w8 ? 8 : (lane >> 2)] = w8 ? v8 : v0;
+                }
             }
             __syncwarp();
             if (issued < nchunks) { issue(issued); ++issued; }
@@ -262,15 +291,18 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
 // Sum each Gaussian's rows (contiguous in the unsorted order), apply the moment -> gradient map
 // (backward.cu:323-329 restated on sums) and write the four gradient tensors:
 //   v_sigma = -w:  v_conic = -1/2 (Sxx, Sxy, Syy),  v_xy = -(a Sx + b Sy, b Sx + c Sy),  v_opacity = S0/opac
+// DEPTH also sums slot 9 into v_depths.
+template <bool DEPTH>
 __global__ void __launch_bounds__(256)
 reduce_grad_rows_kernel(int n, const int *__restrict__ cum_tiles_hit, const float *__restrict__ grad_rows,
                         const float *__restrict__ conics, const float *__restrict__ opacities,
                         float2 *__restrict__ v_xy, float *__restrict__ v_conic,
-                        float *__restrict__ v_colors, float *__restrict__ v_opacity) {
+                        float *__restrict__ v_colors, float *__restrict__ v_opacity, float *__restrict__ v_depths) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= n) return;
     const int k0 = g ? cum_tiles_hit[g - 1] : 0, k1 = cum_tiles_hit[g];
     float a[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float az = 0.f;   // DEPTH only
     for (int k = k0; k < k1; ++k) {
         const float4 *row = reinterpret_cast<const float4 *>(grad_rows + (size_t)k * GSB_GRAD_ROW_FLOATS);
         const float4 r0 = row[0], r1 = row[1];
@@ -278,6 +310,7 @@ reduce_grad_rows_kernel(int n, const int *__restrict__ cum_tiles_hit, const floa
         a[0] += r0.x; a[1] += r0.y; a[2] += r0.z; a[3] += r0.w;
         a[4] += r1.x; a[5] += r1.y; a[6] += r1.z; a[7] += r1.w;
         a[8] += r8;
+        if (DEPTH) az += reinterpret_cast<const float *>(row)[9];
     }
     const float S0 = a[0], Sx = a[1], Sy = a[2], Sxx = a[3], Sxy = a[4], Syy = a[5];
     const float ca = conics[3 * g], cb = conics[3 * g + 1], cc = conics[3 * g + 2];
@@ -286,12 +319,59 @@ reduce_grad_rows_kernel(int n, const int *__restrict__ cum_tiles_hit, const floa
     v_conic[3 * g] = -0.5f * Sxx; v_conic[3 * g + 1] = -0.5f * Sxy; v_conic[3 * g + 2] = -0.5f * Syy;
     v_colors[3 * g] = a[6]; v_colors[3 * g + 1] = a[7]; v_colors[3 * g + 2] = a[8];
     v_opacity[g] = (op > 0.f) ? S0 / op : 0.f;
+    if (DEPTH) v_depths[g] = az;
 }
 
 }  // namespace
 
 extern "C" size_t gsb_raster_grad_rows_bytes(int m) {
     return gsb_align_up((size_t)(m > 0 ? m : 0) * GSB_GRAD_ROW_FLOATS * 4 + 256, 256);
+}
+
+// Body of gsb_rasterize_backward (depth = false) and of gsb_rasterize_backward_depth.
+static int backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m, const int32_t *tile_bins,
+                    const int32_t *tile_order, const float *conics, const float *opacities, void *records,
+                    const int32_t *cum_tiles_hit, const float *background, const float *final_Ts,
+                    const int32_t *final_idx, const float *v_output, const float *v_output_alpha, void *grad_rows,
+                    float *v_xy, float *v_conic, float *v_colors, float *v_opacity, unsigned flags, bool depth,
+                    const float *record_depths, const float *v_output_depth, float *v_depths, gsb_stream_t stream) {
+    GSB_CHECK_ARG(img_h > 0 && img_w > 0 && n >= 0 && m >= 0);
+    GSB_CHECK_ARG((flags & ~(unsigned)GSB_RASTER_CLAMP_MAX_ONE) == 0);
+    const bool sat = (flags & GSB_RASTER_CLAMP_MAX_ONE) != 0;
+    GSB_CHECK_ARG(tiles_x == gsb_div_up(img_w, GSB_TILE) && tiles_y == gsb_div_up(img_h, GSB_TILE));
+    if (n == 0) return 0;
+    GSB_CHECK_ARG(tile_bins && conics && opacities && cum_tiles_hit && background && final_Ts && final_idx &&
+                  v_output && v_xy && v_conic && v_colors && v_opacity);
+    GSB_CHECK_ARG(!depth || (v_depths && (record_depths || m == 0)));
+    GSB_CHECK_ARG(((uintptr_t)v_xy % 8) == 0);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (m > 0) {
+        GSB_CHECK_ARG(records && grad_rows && ((uintptr_t)records % 16) == 0 && ((uintptr_t)grad_rows % 16) == 0);
+        unsigned *counters = reinterpret_cast<unsigned *>(
+            reinterpret_cast<char *>(records) + gsb_raster_records_bytes(m) - 256);
+        GSB_CUDA(cudaMemsetAsync(counters, 0, 256, s));
+        const int num_tiles = tiles_x * tiles_y;
+#define GSB_BWD_LAUNCH(S, D)                                                                                    \
+    rasterize_backward_kernel<S, D><<<gsb_blend_grid((const void *)rasterize_backward_kernel<S, D>, num_tiles),  \
+                                      RK_THREADS, 0, s>>>(                                                      \
+        img_h, img_w, tiles_x, num_tiles, reinterpret_cast<const int2 *>(tile_bins),                            \
+        reinterpret_cast<const GsbRecord *>(records), background, final_Ts, final_idx, v_output, v_output_alpha, \
+        reinterpret_cast<float *>(grad_rows), counters, tile_order, record_depths, v_output_depth)
+        if (depth) {
+            if (sat) GSB_BWD_LAUNCH(true, true); else GSB_BWD_LAUNCH(false, true);
+        } else {
+            if (sat) GSB_BWD_LAUNCH(true, false); else GSB_BWD_LAUNCH(false, false);
+        }
+#undef GSB_BWD_LAUNCH
+    }
+#define GSB_REDUCE_LAUNCH(D)                                                                                    \
+    reduce_grad_rows_kernel<D><<<gsb_div_up(n, 256), 256, 0, s>>>(                                              \
+        n, cum_tiles_hit, reinterpret_cast<const float *>(grad_rows), conics, opacities,                        \
+        reinterpret_cast<float2 *>(v_xy), v_conic, v_colors, v_opacity, v_depths)
+    if (depth) GSB_REDUCE_LAUNCH(true); else GSB_REDUCE_LAUNCH(false);
+#undef GSB_REDUCE_LAUNCH
+    GSB_LAUNCH_CHECK();
+    return 0;
 }
 
 extern "C" int gsb_rasterize_backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
@@ -301,33 +381,20 @@ extern "C" int gsb_rasterize_backward(int img_h, int img_w, int tiles_x, int til
                                       const float *v_output, const float *v_output_alpha, void *grad_rows,
                                       float *v_xy, float *v_conic, float *v_colors, float *v_opacity, unsigned flags,
                                       gsb_stream_t stream) {
-    GSB_CHECK_ARG(img_h > 0 && img_w > 0 && n >= 0 && m >= 0);
-    GSB_CHECK_ARG((flags & ~(unsigned)GSB_RASTER_CLAMP_MAX_ONE) == 0);
-    const bool sat = (flags & GSB_RASTER_CLAMP_MAX_ONE) != 0;
-    GSB_CHECK_ARG(tiles_x == gsb_div_up(img_w, GSB_TILE) && tiles_y == gsb_div_up(img_h, GSB_TILE));
-    if (n == 0) return 0;
-    GSB_CHECK_ARG(tile_bins && conics && opacities && cum_tiles_hit && background && final_Ts && final_idx &&
-                  v_output && v_xy && v_conic && v_colors && v_opacity);
-    GSB_CHECK_ARG(((uintptr_t)v_xy % 8) == 0);
-    cudaStream_t s = (cudaStream_t)stream;
-    if (m > 0) {
-        GSB_CHECK_ARG(records && grad_rows && ((uintptr_t)records % 16) == 0 && ((uintptr_t)grad_rows % 16) == 0);
-        unsigned *counters = reinterpret_cast<unsigned *>(
-            reinterpret_cast<char *>(records) + gsb_raster_records_bytes(m) - 256);
-        GSB_CUDA(cudaMemsetAsync(counters, 0, 256, s));
-        const int num_tiles = tiles_x * tiles_y;
-#define GSB_BWD_LAUNCH(S)                                                                                       \
-    rasterize_backward_kernel<S><<<gsb_blend_grid((const void *)rasterize_backward_kernel<S>, num_tiles),        \
-                                   RK_THREADS, 0, s>>>(                                                         \
-        img_h, img_w, tiles_x, num_tiles, reinterpret_cast<const int2 *>(tile_bins),                            \
-        reinterpret_cast<const GsbRecord *>(records), background, final_Ts, final_idx, v_output, v_output_alpha, \
-        reinterpret_cast<float *>(grad_rows), counters, tile_order)
-        if (sat) GSB_BWD_LAUNCH(true); else GSB_BWD_LAUNCH(false);
-#undef GSB_BWD_LAUNCH
-    }
-    reduce_grad_rows_kernel<<<gsb_div_up(n, 256), 256, 0, s>>>(
-        n, cum_tiles_hit, reinterpret_cast<const float *>(grad_rows), conics, opacities,
-        reinterpret_cast<float2 *>(v_xy), v_conic, v_colors, v_opacity);
-    GSB_LAUNCH_CHECK();
-    return 0;
+    return backward(img_h, img_w, tiles_x, tiles_y, n, m, tile_bins, tile_order, conics, opacities, records,
+                    cum_tiles_hit, background, final_Ts, final_idx, v_output, v_output_alpha, grad_rows, v_xy, v_conic,
+                    v_colors, v_opacity, flags, false, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int gsb_rasterize_backward_depth(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
+                                            const int32_t *tile_bins, const int32_t *tile_order, const float *conics,
+                                            const float *opacities, void *records, const int32_t *cum_tiles_hit,
+                                            const float *background, const float *final_Ts, const int32_t *final_idx,
+                                            const float *v_output, const float *v_output_alpha, void *grad_rows,
+                                            float *v_xy, float *v_conic, float *v_colors, float *v_opacity,
+                                            unsigned flags, const float *record_depths, const float *v_output_depth,
+                                            float *v_depths, gsb_stream_t stream) {
+    return backward(img_h, img_w, tiles_x, tiles_y, n, m, tile_bins, tile_order, conics, opacities, records,
+                    cum_tiles_hit, background, final_Ts, final_idx, v_output, v_output_alpha, grad_rows, v_xy, v_conic,
+                    v_colors, v_opacity, flags, true, record_depths, v_output_depth, v_depths, stream);
 }

@@ -38,8 +38,10 @@ constexpr float GSB_SMAX_BIAS = 5.541263545158426f + 1e-3f;
 // per-intersection gradient row written by the backward blend kernel (48 B, indexed by k).  With
 // w = (unclamped alpha) * v_alpha and d = centre - pixel, summed over the tile's pixels:
 //   { S0 = sum w, Sx = sum w dx, Sy = sum w dy, Sxx = sum w dx^2, Sxy = sum w dx dy, Syy = sum w dy^2,
-//     R, G, B = sum alpha*T*v_out, 0, 0, 0 }
-// The (linear) map to v_xy / v_conic / v_opacity is applied once per Gaussian by the row-reduce kernel.
+//     R, G, B = sum alpha*T*v_out, Z, 0, 0 }
+// with Z = sum alpha*T*v_depth in the DEPTH instantiation (the depth map's gradient w.r.t. the Gaussian's depth, D18)
+// and unused otherwise.  The (linear) map to v_xy / v_conic / v_opacity is applied once per Gaussian by the row-reduce
+// kernel.
 constexpr int GSB_GRAD_ROW_FLOATS = 12;
 
 // GSB_RASTER_CLAMP_MAX_ONE (gsplat_b200.h): the forward kernel's SAT instantiation marks the colour channels of a

@@ -42,6 +42,22 @@ pack_records_kernel(int m, const int *__restrict__ gaussian_ids_sorted,
     stg_stream4(dst + 2, r.q2);
 }
 
+// record_depths[j] = depths[gaussian_ids_sorted[j]] for j < M: the per-record depth stream of the DEPTH blend
+// kernels.  On the fast path the id list is sized by the capacity, not M: entries past M hold no valid id, so M is
+// read from the binning stats on the device, and after an overflow (stats[2]) nothing is written.
+__global__ void __launch_bounds__(256)
+gather_record_depths_kernel(int m, const int *__restrict__ gaussian_ids_sorted, const float *__restrict__ depths,
+                            const int *__restrict__ bin_stats, float *__restrict__ record_depths) {
+    int mv = m;
+    if (bin_stats) {
+        if (bin_stats[2]) return;
+        mv = min(m, bin_stats[0]);
+    }
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= mv) return;
+    record_depths[i] = __ldg(depths + gaussian_ids_sorted[i]);
+}
+
 // 64 registers -> 8 CTAs (32 warps) per SM.  H100 SXM at 400 W, C2: 0.416 ms per launch against 0.445 ms with 7 CTAs
 // and 0.464 ms with 6 (which needs no spill): occupancy wins
 constexpr int FWD_MIN_BLOCKS = 8;
@@ -52,14 +68,21 @@ constexpr int FWD_MIN_BLOCKS = 8;
 // SAT = true fuses the caller's `clamp_max(rgb, 1)` (model.cpp:222) into the epilogue: the image is written clamped
 // and, per pixel, which channels were cut (!(value <= 1), torch's clamp_max mask) goes into bits 28..30 of final_idx
 // for the SAT instantiation of the backward kernel (sorted indices stay below 2^28, checked by the entry point).
-template <bool COUNT, bool SAT>
-__global__ void __launch_bounds__(RK_THREADS, FWD_MIN_BLOCKS)
+// DEPTH = true also writes out_depth = sum alpha T z over the blended pairs (z = record_depths, the per-record depth
+// stream in sorted order; background depth 0) and out_alpha = 1 - T_final (D18).  The colour arithmetic is the same
+// and in the same order, so out_img / final_Ts / final_idx are those of the DEPTH = false kernel.
+// 8 more accumulators per lane do not fit 64 registers without spilling: DEPTH takes its own minimum of CTAs per SM.
+constexpr int FWD_DEPTH_MIN_BLOCKS = 6;
+template <bool COUNT, bool SAT, bool DEPTH>
+__global__ void __launch_bounds__(RK_THREADS, DEPTH ? FWD_DEPTH_MIN_BLOCKS : FWD_MIN_BLOCKS)
 rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                          const int2 *__restrict__ tile_bins, const GsbRecord *__restrict__ records,
                          const float *__restrict__ background, float *__restrict__ out_img,
                          float *__restrict__ final_Ts, int *__restrict__ final_idx,
                          unsigned *__restrict__ tile_counter, const int *__restrict__ bin_stats,
-                         unsigned long long *__restrict__ pair_counts, const int *__restrict__ tile_order) {
+                         unsigned long long *__restrict__ pair_counts, const int *__restrict__ tile_order,
+                         const float *__restrict__ record_depths, float *__restrict__ out_depth,
+                         float *__restrict__ out_alpha) {
     // bin_stats (optional): stats of gsb_bucket_tile_ranges; [2] != 0 means the binning overflowed its
     // capacities and wrote nothing -- the host redoes the frame, this launch must not touch the records
     if (bin_stats && bin_stats[2]) return;
@@ -96,12 +119,14 @@ rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
         // NEGATED (sign bit == "done"): T*(1-alpha) <= 1e-4 then always routes it to the (rare)
         // terminate branch, which ignores pixels that are already negative.
         float T[RK_PIX], cr[RK_PIX], cg[RK_PIX], cb[RK_PIX];
+        float cd[RK_PIX];   // DEPTH only
         const float py0 = (float)Y0;
         int last[RK_PIX];
         unsigned done = 0;  // bit j: pixel j finished (or outside the image)
 #pragma unroll
         for (int j = 0; j < RK_PIX; ++j) {
             T[j] = 1.f; cr[j] = cg[j] = cb[j] = 0.f; last[j] = 0;
+            if (DEPTH) cd[j] = 0.f;
             if (X >= img_w || Y0 + 2 * j >= img_h) { done |= 1u << j; T[j] = -1.f; }
         }
 
@@ -124,6 +149,13 @@ rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
         int c = 0;
         for (; c < nchunks; ++c) {
             const unsigned s = stage_of(c);
+            // DEPTH: lane l loads the depth of record l of the chunk (one coalesced 128-B load), issued before the
+            // wait so that its latency hides behind it; the blend loop shuffles it to the record it blends
+            float zl = 0.f;
+            if (DEPTH) {
+                const int i = range.x + c * RK_CHUNK + lane;
+                if (i < range.y) zl = __ldg(record_depths + i);
+            }
             mbar_wait(&ring.full[s], parity_of(c));
             const int cnt = min(RK_CHUNK, L - c * RK_CHUNK);
             const int idx0 = range.x + c * RK_CHUNK;
@@ -136,6 +168,8 @@ rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 const int t = __ffs(live) - 1;
                 live &= live - 1;
                 const unsigned rm = __shfl_sync(0xffffffffu, my_mask, t);  // slots inside the y-extent
+                float z = 0.f;
+                if (DEPTH) z = __shfl_sync(0xffffffffu, zl, t);
                 const float4 q0 = ring.rec[s][t].q0;
                 const float4 q1 = ring.rec[s][t].q1;
                 const float4 q2 = ring.rec[s][t].q2;
@@ -168,6 +202,7 @@ rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                     cr[j] = fmaf(q2.x, vis, cr[j]);                                                       \
                     cg[j] = fmaf(q2.y, vis, cg[j]);                                                       \
                     cb[j] = fmaf(q2.z, vis, cb[j]);                                                       \
+                    if (DEPTH) cd[j] = fmaf(z, vis, cd[j]);                                               \
                     T[j] = next_T;                                                                        \
                     last[j] = idx;                                                                        \
                     if (COUNT) ++n_blend;                                                                 \
@@ -215,6 +250,10 @@ rasterize_forward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 out_img[3 * p] = o0;
                 out_img[3 * p + 1] = o1;
                 out_img[3 * p + 2] = o2;
+                if (DEPTH) {   // never clamped
+                    out_depth[p] = cd[j];
+                    out_alpha[p] = 1.f - Tf;
+                }
             }
         }
     }
@@ -271,11 +310,22 @@ static int blend_setup(int img_h, int img_w, int tiles_x, int tiles_y, int m, co
     return 0;
 }
 
-extern "C" int gsb_rasterize_forward_packed(int img_h, int img_w, int tiles_x, int tiles_y, int m,
-                                            const int32_t *tile_bins, const int32_t *tile_order,
-                                            const int32_t *bin_stats, const float *background, void *records,
-                                            float *out_img, float *final_Ts, int32_t *final_idx, unsigned flags,
-                                            gsb_stream_t stream) {
+extern "C" int gsb_gather_record_depths(int m, const int32_t *gaussian_ids_sorted, const float *depths,
+                                        const int32_t *bin_stats, float *record_depths, gsb_stream_t stream) {
+    GSB_CHECK_ARG(m >= 0);
+    if (m == 0) return 0;
+    GSB_CHECK_ARG(gaussian_ids_sorted && depths && record_depths);
+    gather_record_depths_kernel<<<gsb_div_up(m, 256), 256, 0, (cudaStream_t)stream>>>(
+        m, gaussian_ids_sorted, depths, bin_stats, record_depths);
+    GSB_LAUNCH_CHECK();
+    return 0;
+}
+
+// Body of gsb_rasterize_forward_packed (depth = false) and of gsb_rasterize_forward_packed_depth.
+static int forward_packed(int img_h, int img_w, int tiles_x, int tiles_y, int m, const int32_t *tile_bins,
+                          const int32_t *tile_order, const int32_t *bin_stats, const float *background, void *records,
+                          float *out_img, float *final_Ts, int32_t *final_idx, unsigned flags, bool depth,
+                          const float *record_depths, float *out_depth, float *out_alpha, gsb_stream_t stream) {
     GSB_CHECK_ARG((flags & ~(unsigned)GSB_RASTER_CLAMP_MAX_ONE) == 0);
     const bool sat = (flags & GSB_RASTER_CLAMP_MAX_ONE) != 0;
     GSB_CHECK_ARG(!sat || m < GSB_SAT_BIT0);
@@ -285,16 +335,40 @@ extern "C" int gsb_rasterize_forward_packed(int img_h, int img_w, int tiles_x, i
                                final_idx, s, &counters);
     if (rc) return rc;
     const int num_tiles = tiles_x * tiles_y;
-#define GSB_FWD_LAUNCH(S)                                                                                        \
-    rasterize_forward_kernel<false, S><<<gsb_blend_grid((const void *)rasterize_forward_kernel<false, S>, num_tiles), \
-                                         RK_THREADS, 0, s>>>(                                                    \
-        img_h, img_w, tiles_x, num_tiles, reinterpret_cast<const int2 *>(tile_bins),                             \
-        reinterpret_cast<const GsbRecord *>(records), background, out_img, final_Ts, final_idx, counters,        \
-        bin_stats, nullptr, tile_order)
-    if (sat) GSB_FWD_LAUNCH(true); else GSB_FWD_LAUNCH(false);
+#define GSB_FWD_LAUNCH(S, D)                                                                                     \
+    rasterize_forward_kernel<false, S, D>                                                                        \
+        <<<gsb_blend_grid((const void *)rasterize_forward_kernel<false, S, D>, num_tiles), RK_THREADS, 0, s>>>(  \
+            img_h, img_w, tiles_x, num_tiles, reinterpret_cast<const int2 *>(tile_bins),                         \
+            reinterpret_cast<const GsbRecord *>(records), background, out_img, final_Ts, final_idx, counters,    \
+            bin_stats, nullptr, tile_order, record_depths, out_depth, out_alpha)
+    if (depth) {
+        if (sat) GSB_FWD_LAUNCH(true, true); else GSB_FWD_LAUNCH(false, true);
+    } else {
+        if (sat) GSB_FWD_LAUNCH(true, false); else GSB_FWD_LAUNCH(false, false);
+    }
 #undef GSB_FWD_LAUNCH
     GSB_LAUNCH_CHECK();
     return 0;
+}
+
+extern "C" int gsb_rasterize_forward_packed(int img_h, int img_w, int tiles_x, int tiles_y, int m,
+                                            const int32_t *tile_bins, const int32_t *tile_order,
+                                            const int32_t *bin_stats, const float *background, void *records,
+                                            float *out_img, float *final_Ts, int32_t *final_idx, unsigned flags,
+                                            gsb_stream_t stream) {
+    return forward_packed(img_h, img_w, tiles_x, tiles_y, m, tile_bins, tile_order, bin_stats, background, records,
+                          out_img, final_Ts, final_idx, flags, false, nullptr, nullptr, nullptr, stream);
+}
+
+extern "C" int gsb_rasterize_forward_packed_depth(int img_h, int img_w, int tiles_x, int tiles_y, int m,
+                                                  const int32_t *tile_bins, const int32_t *tile_order,
+                                                  const int32_t *bin_stats, const float *background, void *records,
+                                                  float *out_img, float *final_Ts, int32_t *final_idx, unsigned flags,
+                                                  const float *record_depths, float *out_depth, float *out_alpha,
+                                                  gsb_stream_t stream) {
+    GSB_CHECK_ARG(out_depth && out_alpha && (record_depths || m == 0));
+    return forward_packed(img_h, img_w, tiles_x, tiles_y, m, tile_bins, tile_order, bin_stats, background, records,
+                          out_img, final_Ts, final_idx, flags, true, record_depths, out_depth, out_alpha, stream);
 }
 
 // Diagnostic twin of gsb_rasterize_forward_packed: same outputs, plus pair_counts (device uint64[4], accumulated --
@@ -312,11 +386,11 @@ extern "C" int gsb_rasterize_forward_count(int img_h, int img_w, int tiles_x, in
                                final_idx, s, &counters);
     if (rc) return rc;
     const int num_tiles = tiles_x * tiles_y;
-    const int grid = gsb_blend_grid((const void *)rasterize_forward_kernel<true, false>, num_tiles);
-    rasterize_forward_kernel<true, false><<<grid, RK_THREADS, 0, s>>>(
+    const int grid = gsb_blend_grid((const void *)rasterize_forward_kernel<true, false, false>, num_tiles);
+    rasterize_forward_kernel<true, false, false><<<grid, RK_THREADS, 0, s>>>(
         img_h, img_w, tiles_x, num_tiles, reinterpret_cast<const int2 *>(tile_bins),
         reinterpret_cast<const GsbRecord *>(records), background, out_img, final_Ts, final_idx, counters, nullptr,
-        pair_counts, nullptr);
+        pair_counts, nullptr, nullptr, nullptr, nullptr);
     GSB_LAUNCH_CHECK();
     return 0;
 }
@@ -335,10 +409,12 @@ int gsb_sm_count() {
 }
 
 // persistent grid: SMs x resident CTAs per SM (never more CTAs than there are tile groups).  The occupancy query
-// costs a few microseconds of host time per call, so its result is cached per (thread, device, kernel).
+// costs a few microseconds of host time per call, so its result is cached per (thread, device, kernel): 16 entries
+// hold the 9 blend kernels (forward x {plain, SAT} x {colour, DEPTH} + COUNT, backward x {plain, SAT} x {colour,
+// DEPTH}) on one device with room to spare.
 int gsb_blend_grid(const void *kernel, int num_tiles) {
     struct Entry { const void *kernel; int dev; int per_sm; };
-    static thread_local Entry cache[8] = {};
+    static thread_local Entry cache[16] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     int per_sm = 0;

@@ -243,7 +243,8 @@ class BinFrame:
     per-tile sort + pack, blend) with the capacities of `plan`, waits once for the stats read-back, redoes a frame that
     outgrew the plan and takes tile lists longer than gsb_bucket_max_tile_len() through the generic global sort.  Then
     the frame holds `records`, `cum`, `tile_bins`, `tile_order` (`_ordered`: only the fast path blends in that order),
-    `m_raster` (the intersection count the records are laid out for) and the frame's stats `m` / `max_len`.
+    `m_raster` (the intersection count the records are laid out for) and the frame's stats `m` / `max_len`; a frame
+    blended with a depth output also holds `record_depths`, the per-record depth stream its backward reads.
     SplatPipeline is one frame reused from frame to frame; RasterizeGaussians builds one per call on the device's
     plan."""
 
@@ -252,6 +253,7 @@ class BinFrame:
         self.stats_dev = torch.empty(4, dtype=torch.int32, device=self.dev)
         self.m = self.max_len = self.m_raster = 0
         self.m_cap = -1   # the buffers are built by the first frame
+        self.gids_sorted = self.record_depths = None   # depth output only, allocated by the first frame asking for it
         self._ordered = False
         self._ev = []     # stage events of the current step (SplatPipeline); a redone frame drops them
 
@@ -267,15 +269,27 @@ class BinFrame:
         self.records = torch.empty(self.L.gsb_raster_records_bytes(m_cap), dtype=u8, device=d)
         self.bucket_ws = torch.empty(self.L.gsb_bucket_workspace_bytes(n, m_cap, T) + 256, dtype=u8, device=d)
         self.m_cap = m_cap
+        self.gids_sorted = self.record_depths = None
+
+    def _depth_buffers(self, m):
+        """The sorted Gaussian ids and the per-record depth stream of a depth frame, for at least m records."""
+        if self.record_depths is None or self.record_depths.numel() < m:
+            self.gids_sorted = torch.empty((max(m, 1),), dtype=torch.int32, device=self.dev)
+            self.record_depths = torch.empty((max(m, 1),), dtype=torch.float32, device=self.dev)
 
     def bin_blend(self, xys, radii, conics, depths, nth, rgbs, opacities, background, out_img, final_Ts, final_idx,
-                  flags, count_visible=False):
+                  flags, count_visible=False, out_depth=None, out_alpha=None):
         """Binning, packing and the blend kernel of one frame (after SH colour and projection) into out_img [H,W,3],
         final_Ts and final_idx [H,W], with the frame's one host wait; returns out_img.  The per-Gaussian inputs are
         contiguous float32 / int32 CUDA tensors (nth: the projection's tile counts, read by the generic path only);
         flags: gsb_rasterize_forward_packed's; count_visible: have the binning count the Gaussians with radii > 0 into
-        plan.visible."""
+        plan.visible.  out_depth / out_alpha ([H,W] float32, both or neither): the frame also writes the depth and
+        opacity maps (DESIGN D18) through the DEPTH blend kernel, from the per-record depth stream it gathers from
+        `depths` (kept in `record_depths` for the backward)."""
         L, P, s, plan = self.L, capi.ptr, capi.stream(), self.plan
+        depth = out_depth is not None
+        if depth != (out_alpha is not None):
+            raise ValueError("bin_blend: out_depth and out_alpha go together")
         n, H, W = xys.shape[0], out_img.shape[0], out_img.shape[1]
         tb = tile_bounds(W, H)
         T = tb[0] * tb[1]
@@ -296,16 +310,28 @@ class BinFrame:
                                                 tb[0], tb[1], m_cap, len_cap, wsp, wsb, P(self.cum), P(self.tile_bins),
                                                 P(self.tile_order), P(self.stats_dev), s))
             plan.read_back(self.stats_dev)
+            if depth:
+                self._depth_buffers(m_cap)
             if m_cap > 0:
                 self._stage("bucket_sort_pack")
                 capi.check(L.gsb_bucket_sort_pack(n, m_cap, len_cap, P(depths), P(radii), P(self.cum), 1, tb[0],
                                                   tb[1], P(self.tile_bins), P(self.stats_dev), wsp, wsb,
-                                                  P(self.records), None, None, s))
+                                                  P(self.records), None, P(self.gids_sorted) if depth else None, s))
             self._stage("raster_fwd")
-            capi.check(L.gsb_rasterize_forward_packed(H, W, tb[0], tb[1], m_cap, P(self.tile_bins),
-                                                      P(self.tile_order), P(self.stats_dev), P(background),
-                                                      P(self.records), P(out_img), P(final_Ts), P(final_idx), flags,
-                                                      s))
+            if depth:
+                # the ids past M hold nothing valid: the gather reads M from the stats (no Gaussian: M = 0)
+                if n > 0:
+                    capi.check(L.gsb_gather_record_depths(m_cap, P(self.gids_sorted), P(depths), P(self.stats_dev),
+                                                          P(self.record_depths), s))
+                capi.check(L.gsb_rasterize_forward_packed_depth(
+                    H, W, tb[0], tb[1], m_cap, P(self.tile_bins), P(self.tile_order), P(self.stats_dev),
+                    P(background), P(self.records), P(out_img), P(final_Ts), P(final_idx), flags,
+                    P(self.record_depths), P(out_depth), P(out_alpha), s))
+            else:
+                capi.check(L.gsb_rasterize_forward_packed(H, W, tb[0], tb[1], m_cap, P(self.tile_bins),
+                                                          P(self.tile_order), P(self.stats_dev), P(background),
+                                                          P(self.records), P(out_img), P(final_Ts), P(final_idx),
+                                                          flags, s))
             self._stage("end_fwd")
             self.m, self.max_len, overflow = plan.wait()
             if not overflow:
@@ -329,8 +355,16 @@ class BinFrame:
         self._stage("raster_fwd")
         capi.check(L.gsb_pack_records(m, P(gids_sorted), P(sorted_index), P(xys), P(conics), P(rgbs), P(opacities),
                                       P(self.records), s))
-        capi.check(L.gsb_rasterize_forward_packed(H, W, tb[0], tb[1], m, P(self.tile_bins), None, None, P(background),
-                                                  P(self.records), P(out_img), P(final_Ts), P(final_idx), flags, s))
+        if depth:
+            self._depth_buffers(m)
+            capi.check(L.gsb_gather_record_depths(m, P(gids_sorted), P(depths), None, P(self.record_depths), s))
+            capi.check(L.gsb_rasterize_forward_packed_depth(
+                H, W, tb[0], tb[1], m, P(self.tile_bins), None, None, P(background), P(self.records), P(out_img),
+                P(final_Ts), P(final_idx), flags, P(self.record_depths), P(out_depth), P(out_alpha), s))
+        else:
+            capi.check(L.gsb_rasterize_forward_packed(H, W, tb[0], tb[1], m, P(self.tile_bins), None, None,
+                                                      P(background), P(self.records), P(out_img), P(final_Ts),
+                                                      P(final_idx), flags, s))
         self.m_raster, self._ordered = m, False
         self._stage("end_fwd")
         return out_img
@@ -415,7 +449,11 @@ def rasterize_forward(tile_bounds_, img_size, gaussian_ids_sorted, sorted_index,
 
 
 def rasterize_backward(img_height, img_width, n, m, tile_bins, conics, opacities, records, cum_tiles_hit,
-                       background, final_Ts, final_idx, v_output, v_output_alpha=None, tile_order=None, flags=0):
+                       background, final_Ts, final_idx, v_output, v_output_alpha=None, tile_order=None, flags=0,
+                       record_depths=None, v_output_depth=None):
+    """-> (v_xy, v_conic, v_colors, v_opacity); given the frame's record_depths (a depth frame) the backward of the
+    depth and opacity maps as well (gsb_rasterize_backward_depth, v_output_depth None == zeros), and v_depths [n]
+    follows."""
     L = capi.lib()
     tb = tile_bounds(img_width, img_height)
     rows = _ws.get(final_Ts.device, "grad_rows", L.gsb_raster_grad_rows_bytes(m) + 16)
@@ -425,6 +463,17 @@ def rasterize_backward(img_height, img_width, n, m, tile_bins, conics, opacities
     v_colors = _empty((n, 3), torch.float32, final_Ts)
     v_opacity = _empty((n, 1), torch.float32, final_Ts)
     v_output = capi.f32(v_output)
+    if record_depths is not None:
+        v_depths = _empty((n,), torch.float32, final_Ts)
+        capi.check(L.gsb_rasterize_backward_depth(
+            img_height, img_width, tb[0], tb[1], n, m, capi.ptr(tile_bins), capi.ptr(tile_order),
+            capi.ptr(capi.f32(conics)), capi.ptr(capi.f32(opacities)), capi.ptr(records), capi.ptr(cum_tiles_hit),
+            capi.ptr(capi.f32(background)), capi.ptr(final_Ts), capi.ptr(final_idx), capi.ptr(v_output),
+            capi.ptr(capi.f32(v_output_alpha)) if v_output_alpha is not None else None, rows.data_ptr() + off,
+            capi.ptr(v_xy), capi.ptr(v_conic), capi.ptr(v_colors), capi.ptr(v_opacity), int(flags),
+            capi.ptr(record_depths), capi.ptr(capi.f32(v_output_depth)) if v_output_depth is not None else None,
+            capi.ptr(v_depths), capi.stream()))
+        return v_xy, v_conic, v_colors, v_opacity, v_depths
     capi.check(L.gsb_rasterize_backward(
         img_height, img_width, tb[0], tb[1], n, m, capi.ptr(tile_bins), capi.ptr(tile_order), capi.ptr(capi.f32(conics)),
         capi.ptr(capi.f32(opacities)), capi.ptr(records), capi.ptr(cum_tiles_hit),
@@ -472,7 +521,9 @@ class RasterizeGaussians(torch.autograd.Function):
                                            imgHeight, imgWidth, background)
 
     @staticmethod
-    def _forward(ctx, flags, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background):
+    def _forward(ctx, flags, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background,
+                 depth=False):
+        """The forward of the rasterizer operators: the image, or with depth=True (image, depth map, alpha map)."""
         if colors.shape[-1] != 3:
             raise ValueError("only 3-channel colors are supported")
         xys, depths, conics, colors, opacity, background = (capi.f32(t) for t in (xys, depths, conics, colors,
@@ -481,19 +532,21 @@ class RasterizeGaussians(torch.autograd.Function):
         out = _empty((H, W, 3), torch.float32, xys)
         fT = _empty((H, W), torch.float32, xys)
         fI = _empty((H, W), torch.int32, xys)
+        od = _empty((H, W), torch.float32, xys) if depth else None
+        oa = _empty((H, W), torch.float32, xys) if depth else None
         # one frame per call on the device's plan; the backward gets its tensors through save_for_backward
         f = BinFrame(_plan_for(xys.device), xys.device)
         f.bin_blend(xys, radii.contiguous(), conics, depths, numTilesHit, colors, opacity, background, out, fT, fI,
-                    flags)
+                    flags, out_depth=od, out_alpha=oa)
         ctx.meta = (H, W, xys.shape[0], f.m_raster, flags)
         ctx.save_for_backward(f.tile_bins, conics, opacity, f.records, f.cum, background, fT, fI,
-                              f.tile_order if f._ordered else None)
-        return out
+                              f.tile_order if f._ordered else None, f.record_depths if depth else None)
+        return (out, od, oa) if depth else out
 
     @staticmethod
     def backward(ctx, v_outImg):
         H, W, n, m, flags = ctx.meta
-        bins, conics, opacity, records, cum, background, fT, fI, order = ctx.saved_tensors
+        bins, conics, opacity, records, cum, background, fT, fI, order, _ = ctx.saved_tensors
         v_xy, v_conic, v_colors, v_opacity = rasterize_backward(H, W, n, m, bins, conics, opacity, records, cum,
                                                                 background, fT, fI, v_outImg.contiguous(), None,
                                                                 tile_order=order, flags=flags)
@@ -510,6 +563,41 @@ class RasterizeGaussiansClamped(RasterizeGaussians):
     def forward(ctx, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background):
         return RasterizeGaussians._forward(ctx, CLAMP_MAX_ONE, xys, depths, radii, conics, numTilesHit, colors,
                                            opacity, imgHeight, imgWidth, background)
+
+
+class RasterizeGaussiansDepth(torch.autograd.Function):
+    """RasterizeGaussians with the depth and opacity maps (DESIGN D18): same arguments, returns (rgb [H,W,3],
+    depth [H,W], alpha [H,W]) with depth = sum alpha T z over the pairs the colour blend blends (z = `depths`, the
+    projection's view-space depth; background depth 0, not normalised) and alpha = 1 - T_final.  rgb is bit-identical
+    to RasterizeGaussians'.  Gradients go to xys (0), depths (1), conics (3), colors (5) and opacity (6), so a depth
+    loss reaches the means through ProjectGaussians' depths output.  C++ twin: gsb::RasterizeGaussiansDepth."""
+
+    @staticmethod
+    def forward(ctx, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background):
+        return RasterizeGaussians._forward(ctx, 0, xys, depths, radii, conics, numTilesHit, colors, opacity,
+                                           imgHeight, imgWidth, background, depth=True)
+
+    @staticmethod
+    def backward(ctx, v_outImg, v_depth, v_alpha):
+        H, W, n, m, flags = ctx.meta
+        bins, conics, opacity, records, cum, background, fT, fI, order, rd = ctx.saved_tensors
+        if v_outImg is None:
+            v_outImg = torch.zeros((H, W, 3), dtype=torch.float32, device=fT.device)
+        v_xy, v_conic, v_colors, v_opacity, v_depths = rasterize_backward(
+            H, W, n, m, bins, conics, opacity, records, cum, background, fT, fI, v_outImg.contiguous(),
+            v_alpha.contiguous() if v_alpha is not None else None, tile_order=order, flags=flags, record_depths=rd,
+            v_output_depth=v_depth.contiguous() if v_depth is not None else None)
+        return v_xy, v_depths, None, v_conic, None, v_colors, v_opacity, None, None, None
+
+
+class RasterizeGaussiansDepthClamped(RasterizeGaussiansDepth):
+    """RasterizeGaussiansDepth with rgb = clamp_max(rgb, 1) fused as in RasterizeGaussiansClamped; depth and alpha are
+    never clamped.  C++ twin: gsb::RasterizeGaussiansDepthClamped."""
+
+    @staticmethod
+    def forward(ctx, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background):
+        return RasterizeGaussians._forward(ctx, CLAMP_MAX_ONE, xys, depths, radii, conics, numTilesHit, colors,
+                                           opacity, imgHeight, imgWidth, background, depth=True)
 
 
 class ProjectGaussiansActivated(torch.autograd.Function):

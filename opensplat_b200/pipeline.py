@@ -167,13 +167,15 @@ class SplatPipeline(BinFrame):
                                          P(self.nth), s))
         return self._bin_blend(p["opacities"], 0)
 
-    def _bin_blend(self, opacities, flags, count_visible=False, rgbs=None):
+    def _bin_blend(self, opacities, flags, count_visible=False, rgbs=None, out_img=None, out_depth=None,
+                   out_alpha=None):
         """bin_blend on the pipeline's projection and pixel buffers.  opacities: the [n] opacities the blend uses;
         rgbs: the [n,3] colours the records carry (default self.rgbs; a trainer with several views per step passes the
-        view's)."""
+        view's); out_img: the image (default self.out_img); out_depth / out_alpha: bin_blend's depth output."""
         return self.bin_blend(self.xys, self.radii, self.conics, self.depths, self.nth,
-                              self.rgbs if rgbs is None else rgbs, opacities, self.background, self.out_img,
-                              self.final_Ts, self.final_idx, flags, count_visible)
+                              self.rgbs if rgbs is None else rgbs, opacities, self.background,
+                              self.out_img if out_img is None else out_img, self.final_Ts, self.final_idx, flags,
+                              count_visible, out_depth=out_depth, out_alpha=out_alpha)
 
     def _raster_backward(self, opacities, v_opacities, v_rgbs, flags):
         """The blend kernel's backward of the last frame (_bin_blend's), from the gradient of its image in self.v_img

@@ -98,6 +98,8 @@ def view_setups(cams, gts, views, downscale):
     ground-truth images: returns (setups, H, W).  Raises ValueError unless there are exactly `views` cameras and
     images, all cameras render at one resolution and every image is a float32 [H,W,3] tensor of it."""
     cams = [cams] if isinstance(cams, Camera) else list(cams)
+    if gts is None:      # a render without ground truth (SplatTrainer.render)
+        gts = [None] * len(cams)
     if len(cams) != views or len(gts) != views:
         raise ValueError(f"a step takes {views} cameras and {views} ground-truth images (views_per_step={views}), "
                          f"got {len(cams)} and {len(gts)}")
@@ -107,6 +109,8 @@ def view_setups(cams, gts, views, downscale):
         raise ValueError("all views of a step must render at the same resolution, got (W, H) "
                          f"{sorted({(su[1], su[0]) for su in setups})}")
     for gt in gts:
+        if gt is None:
+            continue
         if gt.dtype != torch.float32 or tuple(gt.shape) != (H, W, 3):
             raise ValueError(f"every gt must be a float32 [{H},{W},3] image (this step's render resolution)")
     return setups, H, W
@@ -161,6 +165,7 @@ class SplatTrainer:
         self.losses = torch.zeros((B, 3), dtype=torch.float32, device=self.device)
         self.eval_loss = torch.zeros(3, dtype=torch.float32, device=self.device)    # evaluate()'s result
         self.resolution = None
+        self.render_maps = None   # render()'s outputs, sized by the resolution
         self.pixel_reallocs = 0   # resolution changes after the first step (the downscale schedule)
         self.writer = None
         self.last_info = {"refined": False}
@@ -200,6 +205,7 @@ class SplatTrainer:
             self.pixel_reallocs += 1
         self.resolution = (W, H)
         self.pipe._alloc_pixels(W, H)
+        self.render_maps = None
         self.ssim_ws = torch.empty(self.L.gsb_ssim_workspace_bytes(H, W) + 256, dtype=torch.uint8, device=self.device)
 
     @property
@@ -274,6 +280,33 @@ class SplatTrainer:
         self._render_view(0, setups[0][2], gt, self.eval_loss)
         return self.eval_loss
 
+    def render(self, cam, step, normalize_depth=False):
+        """Renders one view without training on it: Model::forward at `step`'s downscale factor and SH degree (the
+        clamped colour, as evaluate() renders it) plus the depth and opacity maps (DESIGN D18).  Returns
+        {"rgb" [H,W,3], "depth" [H,W], "alpha" [H,W]}: depth = sum alpha T z over the blended pairs (z the view-space
+        depth of the Gaussian; 0 where nothing is blended), alpha = 1 - T_final; with normalize_depth, depth / alpha
+        where alpha > 0 and 0 elsewhere.  The tensors are overwritten by the next render().  Like evaluate(), it leaves
+        parameters, Adam state and the densification statistics alone, and the next step() computes what it would have
+        computed without this call; it does not change `image`.  A view at another resolution than the last step's
+        reallocates the pixel buffers, as evaluate() does."""
+        setups = self._setup_views(cam, None, 1, step)[0]
+        pp = self.pipe
+        H, W = pp.H, pp.W
+        if self.render_maps is None:
+            f32, d = torch.float32, self.device
+            self.render_maps = {"rgb": torch.empty((H, W, 3), dtype=f32, device=d),
+                                "depth": torch.empty((H, W), dtype=f32, device=d),
+                                "alpha": torch.empty((H, W), dtype=f32, device=d),
+                                "normalized": torch.empty((H, W), dtype=f32, device=d)}
+        r = self.render_maps
+        self._project_blend(0, setups[0][2], out_img=r["rgb"], out_depth=r["depth"], out_alpha=r["alpha"])
+        depth = r["depth"]
+        if normalize_depth:
+            depth = r["normalized"]
+            torch.div(r["depth"], r["alpha"], out=depth)
+            depth.masked_fill_(r["alpha"] <= 0, 0.0)
+        return {"rgb": r["rgb"], "depth": depth, "alpha": r["alpha"]}
+
     def _setup_views(self, cams, gts, views, step):
         """What the forward passes of a step's `views` views share: view_setups at `step`'s downscale factor, the
         render resolution, one upload of the cameras into slots 0..views-1 of the camera block (the last host wait, a
@@ -302,10 +335,10 @@ class SplatTrainer:
                                                           P(p["coeffs"]), 0.5, P(self.rgbs_views), s))
         return setups, H, W, use
 
-    def _render_view(self, b, intr, gt, loss):
-        """View b's forward pass after _setup_views: projection with the activations from camera slot b (intrinsics
-        `intr`), binning and the clamped blend into the pipeline's image (the view's one host wait), then the loss
-        against gt into `loss` ({total, L1, SSIM}) and its image gradient into the pipeline's v_img."""
+    def _project_blend(self, b, intr, out_img=None, out_depth=None, out_alpha=None):
+        """View b's projection with the activations from camera slot b (intrinsics `intr`), then binning and the
+        clamped blend (the view's one host wait) into the pipeline's image, or into out_img with the depth and opacity
+        maps (render())."""
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         n, p, tb, H, W = pp.n, pp.p, pp.tb, pp.H, pp.W
         fx, fy, cx, cy = intr
@@ -313,7 +346,15 @@ class SplatTrainer:
             n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmats[b]),
             P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
             P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac), s))
-        pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[b])
+        pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[b], out_img=out_img,
+                      out_depth=out_depth, out_alpha=out_alpha)
+
+    def _render_view(self, b, intr, gt, loss):
+        """View b's forward pass after _setup_views: _project_blend, then the loss against gt into `loss` ({total, L1,
+        SSIM}) and its image gradient into the pipeline's v_img."""
+        pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
+        H, W = pp.H, pp.W
+        self._project_blend(b, intr)
         off = (-self.ssim_ws.data_ptr()) % 256
         capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(loss),
                                       self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off, s))
