@@ -186,6 +186,35 @@ int gsb_project_backward_activated_acc(int n, const float *means3d, const float 
                                        const float *v_depth, const float *v_conic, const float *v_opacity,
                                        float *v_mean3d, float *v_log_scales, float *v_raw_quats,
                                        float *v_opacity_logits, gsb_stream_t stream);
+/* gsb_project_forward_activated_aa: gsb_project_forward_activated with the anti-aliased opacity (DESIGN D19, the
+ *   "antialiased" mode of gsplat / Mip-Splatting's 2-D filter): opacities [n] = sigmoid(logits) * comp, comp =
+ *   sqrt(max(0, det0 / det)) where radii > 0 and 0 elsewhere; det0 = cxx0 cyy0 - cxy^2 is the determinant of the
+ *   screen covariance before the 0.3 px^2 blur, det the one after it.  Every other output is bit-identical to
+ *   gsb_project_forward_activated's, so binning and blending are unchanged.
+ * gsb_project_backward_activated_aa / _aa_acc: its exact VJP, written / added like gsb_project_backward_activated /
+ *   _acc, with the same arguments except that they take the opacity LOGITS (opacity_logits [n]) where those take the
+ *   saved opacities.  v_opacity (NULL == zeros) reaches the logits as v_opacity * comp * o (1 - o) and, where comp > 0,
+ *   the geometry through comp. */
+int gsb_project_forward_activated_aa(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                     const float *raw_quats, const float *opacity_logits, const float *viewmat,
+                                     const float *projmat, float fx, float fy, float cx, float cy, int img_h,
+                                     int img_w, int tiles_x, int tiles_y, float clip_thresh, float *cov3d, float *xys,
+                                     float *depths, int32_t *radii, float *conics, int32_t *num_tiles_hit,
+                                     float *opacities, gsb_stream_t stream);
+int gsb_project_backward_activated_aa(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                      const float *raw_quats, const float *opacity_logits, const float *viewmat,
+                                      const float *projmat, float fx, float fy, int img_h, int img_w,
+                                      const int32_t *radii, const float *conics, const float *v_xy,
+                                      const float *v_depth, const float *v_conic, const float *v_opacity,
+                                      float *v_mean3d, float *v_log_scales, float *v_raw_quats,
+                                      float *v_opacity_logits, gsb_stream_t stream);
+int gsb_project_backward_activated_aa_acc(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                          const float *raw_quats, const float *opacity_logits, const float *viewmat,
+                                          const float *projmat, float fx, float fy, int img_h, int img_w,
+                                          const int32_t *radii, const float *conics, const float *v_xy,
+                                          const float *v_depth, const float *v_conic, const float *v_opacity,
+                                          float *v_mean3d, float *v_log_scales, float *v_raw_quats,
+                                          float *v_opacity_logits, gsb_stream_t stream);
 
 /* ---- Tile binning ----------------------------------------------------------------------------
  * gsb_cumsum_tiles_hit replaces torch::cumsum(numTilesHit, 0, kInt32) (rasterize_gaussians.cpp:62).

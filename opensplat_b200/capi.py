@@ -46,6 +46,13 @@ _SIGS = {
                                             _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_project_backward_activated_acc": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
                                                 _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    # the anti-aliased opacity (DESIGN D19): the arguments of the three above; the backward takes logits for opac
+    "gsb_project_forward_activated_aa": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i, _i, _i,
+                                              _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_project_backward_activated_aa": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
+                                               _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_project_backward_activated_aa_acc": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
+                                                   _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_cumsum_workspace_bytes": (_sz, [_i]),
     "gsb_cumsum_tiles_hit": (_i, [_i, _vp, _vp, _vp, _sz, _vp]),
     "gsb_map_gaussian_to_intersects": (_i, [_i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),

@@ -117,8 +117,10 @@ torch::autograd::tensor_list SphericalHarmonicsRgb::backward(torch::autograd::Au
     return {torch::Tensor(), torch::Tensor(), torch::Tensor(), vDc, vRest};
 }
 
-torch::autograd::variable_list ProjectGaussiansActivated::forward(
-    torch::autograd::AutogradContext *ctx, torch::Tensor means, torch::Tensor logScales, double globScale,
+// The body of ProjectGaussiansActivated[Antialiased]: `aa` picks the anti-aliased kernels (DESIGN D19), whose backward
+// takes the opacity logits where the plain one takes the saved sigmoid.
+static torch::autograd::variable_list projectActivatedForward(
+    torch::autograd::AutogradContext *ctx, bool aa, torch::Tensor means, torch::Tensor logScales, double globScale,
     torch::Tensor rawQuats, torch::Tensor opacityLogits, torch::Tensor viewMat, torch::Tensor projMat, double fx,
     double fy, double cx, double cy, int64_t imgHeight, int64_t imgWidth, std::tuple<int, int, int> tileBounds,
     double clipThresh) {
@@ -134,28 +136,30 @@ torch::autograd::variable_list ProjectGaussiansActivated::forward(
     torch::Tensor conics = torch::empty({n, 3}, like(m, torch::kFloat32));
     torch::Tensor numTilesHit = torch::empty({n}, like(m, torch::kInt32));
     torch::Tensor opac = torch::empty({n, 1}, like(m, torch::kFloat32));
-    check(gsb_project_forward_activated(n, fp(m), fp(ls), (float)globScale, fp(rq), fp(ol), fp(V), fp(P), (float)fx,
-                                        (float)fy, (float)cx, (float)cy, (int)imgHeight, (int)imgWidth,
-                                        std::get<0>(tileBounds), std::get<1>(tileBounds), (float)clipThresh,
-                                        fpw(cov3d), fpw(xys), fpw(depths), radii.data_ptr<int32_t>(), fpw(conics),
-                                        numTilesHit.data_ptr<int32_t>(), fpw(opac), stream()),
-          "gsb_project_forward_activated");
+    check((aa ? gsb_project_forward_activated_aa : gsb_project_forward_activated)(
+              n, fp(m), fp(ls), (float)globScale, fp(rq), fp(ol), fp(V), fp(P), (float)fx, (float)fy, (float)cx,
+              (float)cy, (int)imgHeight, (int)imgWidth, std::get<0>(tileBounds), std::get<1>(tileBounds),
+              (float)clipThresh, fpw(cov3d), fpw(xys), fpw(depths), radii.data_ptr<int32_t>(), fpw(conics),
+              numTilesHit.data_ptr<int32_t>(), fpw(opac), stream()),
+          aa ? "gsb_project_forward_activated_aa" : "gsb_project_forward_activated");
     ctx->saved_data["imgHeight"] = imgHeight;
     ctx->saved_data["imgWidth"] = imgWidth;
     ctx->saved_data["globScale"] = globScale;
     ctx->saved_data["fx"] = fx;
     ctx->saved_data["fy"] = fy;
     ctx->saved_data["logitSizes"] = opacityLogits.sizes().vec();
-    ctx->save_for_backward({m, ls, rq, V, P, radii, conics, opac});
+    ctx->saved_data["aa"] = aa;
+    ctx->save_for_backward({m, ls, rq, V, P, radii, conics, aa ? ol : opac});
     ctx->mark_non_differentiable({radii, numTilesHit});
     return {xys, depths, radii, conics, numTilesHit, cov3d, opac};
 }
 
-torch::autograd::tensor_list ProjectGaussiansActivated::backward(torch::autograd::AutogradContext *ctx,
-                                                                 torch::autograd::tensor_list g) {
+static torch::autograd::tensor_list projectActivatedBackward(torch::autograd::AutogradContext *ctx,
+                                                             torch::autograd::tensor_list g) {
     auto saved = ctx->get_saved_variables();
     torch::Tensor m = saved[0], ls = saved[1], rq = saved[2], V = saved[3], P = saved[4];
-    torch::Tensor radii = saved[5], conics = saved[6], opac = saved[7];
+    torch::Tensor radii = saved[5], conics = saved[6], opac = saved[7];   // opac: the logits when aa
+    const bool aa = ctx->saved_data["aa"].toBool();
     const int n = (int)m.size(0);
     c10::cuda::CUDAGuard guard(m.device());
     // cotangents of xys (0), depths (1), conics (3), opacities (6); undefined == zeros
@@ -167,16 +171,44 @@ torch::autograd::tensor_list ProjectGaussiansActivated::backward(torch::autograd
     torch::Tensor v_ls = torch::empty({n, 3}, like(m, torch::kFloat32));
     torch::Tensor v_rq = torch::empty({n, 4}, like(m, torch::kFloat32));
     torch::Tensor v_ol = torch::empty({n}, like(m, torch::kFloat32));
-    check(gsb_project_backward_activated(
+    check((aa ? gsb_project_backward_activated_aa : gsb_project_backward_activated)(
               n, fp(m), fp(ls), (float)ctx->saved_data["globScale"].toDouble(), fp(rq), fp(opac), fp(V), fp(P),
               (float)ctx->saved_data["fx"].toDouble(), (float)ctx->saved_data["fy"].toDouble(),
               (int)ctx->saved_data["imgHeight"].toInt(), (int)ctx->saved_data["imgWidth"].toInt(),
               radii.data_ptr<int32_t>(), fp(conics), fp(v_xy), v_depth.defined() ? fp(v_depth) : nullptr, fp(v_conic),
               v_opac.defined() ? fp(v_opac) : nullptr, fpw(v_mean), fpw(v_ls), fpw(v_rq), fpw(v_ol), stream()),
-          "gsb_project_backward_activated");
+          aa ? "gsb_project_backward_activated_aa" : "gsb_project_backward_activated");
     torch::Tensor none;
     return {v_mean, v_ls, none, v_rq, v_ol.reshape(ctx->saved_data["logitSizes"].toIntVector()),
             none, none, none, none, none, none, none, none, none, none};
+}
+
+torch::autograd::variable_list ProjectGaussiansActivated::forward(
+    torch::autograd::AutogradContext *ctx, torch::Tensor means, torch::Tensor logScales, double globScale,
+    torch::Tensor rawQuats, torch::Tensor opacityLogits, torch::Tensor viewMat, torch::Tensor projMat, double fx,
+    double fy, double cx, double cy, int64_t imgHeight, int64_t imgWidth, std::tuple<int, int, int> tileBounds,
+    double clipThresh) {
+    return projectActivatedForward(ctx, false, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat,
+                                   fx, fy, cx, cy, imgHeight, imgWidth, tileBounds, clipThresh);
+}
+
+torch::autograd::tensor_list ProjectGaussiansActivated::backward(torch::autograd::AutogradContext *ctx,
+                                                                 torch::autograd::tensor_list g) {
+    return projectActivatedBackward(ctx, g);
+}
+
+torch::autograd::variable_list ProjectGaussiansActivatedAntialiased::forward(
+    torch::autograd::AutogradContext *ctx, torch::Tensor means, torch::Tensor logScales, double globScale,
+    torch::Tensor rawQuats, torch::Tensor opacityLogits, torch::Tensor viewMat, torch::Tensor projMat, double fx,
+    double fy, double cx, double cy, int64_t imgHeight, int64_t imgWidth, std::tuple<int, int, int> tileBounds,
+    double clipThresh) {
+    return projectActivatedForward(ctx, true, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat,
+                                   fx, fy, cx, cy, imgHeight, imgWidth, tileBounds, clipThresh);
+}
+
+torch::autograd::tensor_list ProjectGaussiansActivatedAntialiased::backward(torch::autograd::AutogradContext *ctx,
+                                                                            torch::autograd::tensor_list g) {
+    return projectActivatedBackward(ctx, g);
 }
 
 torch::Tensor RasterizeGaussiansClamped::forward(torch::autograd::AutogradContext *ctx, torch::Tensor xys,

@@ -65,6 +65,21 @@ public:
                                                  torch::autograd::tensor_list grad_outputs);
 };
 
+// ProjectGaussiansActivated with the anti-aliased opacity (DESIGN D19, gsplat's "antialiased" mode): same arguments
+// and outputs, but p[6] = sigmoid(opacities) * sqrt(max(0, det0 / det)) with det0 / det the determinants of the
+// screen covariance before / after the 0.3 px^2 blur (0 for a culled Gaussian); p[0..5] are bit-identical.
+class ProjectGaussiansActivatedAntialiased : public torch::autograd::Function<ProjectGaussiansActivatedAntialiased> {
+public:
+    static torch::autograd::variable_list forward(torch::autograd::AutogradContext *ctx, torch::Tensor means,
+                                                  torch::Tensor logScales, double globScale, torch::Tensor rawQuats,
+                                                  torch::Tensor opacityLogits, torch::Tensor viewMat,
+                                                  torch::Tensor projMat, double fx, double fy, double cx, double cy,
+                                                  int64_t imgHeight, int64_t imgWidth,
+                                                  std::tuple<int, int, int> tileBounds, double clipThresh = 0.01);
+    static torch::autograd::tensor_list backward(torch::autograd::AutogradContext *ctx,
+                                                 torch::autograd::tensor_list grad_outputs);
+};
+
 // `rgb = RasterizeGaussians::apply(...); rgb = torch::clamp_max(rgb, 1.0f);` (model.cpp:213-222) as one operator:
 // the blend kernel writes the clamped image, the backward blend kernel applies clamp_max's gradient mask.
 // Same arguments and gradient slots as RasterizeGaussians.

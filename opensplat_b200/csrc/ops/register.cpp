@@ -70,6 +70,16 @@ static std::vector<torch::Tensor> op_project_activated(torch::Tensor means, torc
                                                  projMat, fx, fy, cx, cy, imgHeight, imgWidth, tb, clipThresh);
 }
 
+static std::vector<torch::Tensor> op_project_activated_antialiased(
+    torch::Tensor means, torch::Tensor logScales, double globScale, torch::Tensor rawQuats, torch::Tensor opacityLogits,
+    torch::Tensor viewMat, torch::Tensor projMat, double fx, double fy, double cx, double cy, int64_t imgHeight,
+    int64_t imgWidth, double clipThresh) {
+    TileBounds tb = std::make_tuple((int)(imgWidth + BLOCK_X - 1) / BLOCK_X, (int)(imgHeight + BLOCK_Y - 1) / BLOCK_Y, 1);
+    return gsb::ProjectGaussiansActivatedAntialiased::apply(means, logScales, globScale, rawQuats, opacityLogits,
+                                                            viewMat, projMat, fx, fy, cx, cy, imgHeight, imgWidth, tb,
+                                                            clipThresh);
+}
+
 static torch::Tensor op_rasterize_clamped(torch::Tensor xys, torch::Tensor depths, torch::Tensor radii,
                                           torch::Tensor conics, torch::Tensor numTilesHit, torch::Tensor colors,
                                           torch::Tensor opacity, int64_t imgHeight, int64_t imgWidth,
@@ -97,6 +107,7 @@ static std::vector<torch::Tensor> op_rasterize_depth_clamped(torch::Tensor xys, 
 
 TORCH_LIBRARY(opensplat_b200, m) {
     m.def("project_gaussians_activated", &op_project_activated);
+    m.def("project_gaussians_activated_antialiased", &op_project_activated_antialiased);
     m.def("rasterize_gaussians_clamped", &op_rasterize_clamped);
     m.def("rasterize_gaussians_depth", &op_rasterize_depth);
     m.def("rasterize_gaussians_depth_clamped", &op_rasterize_depth_clamped);

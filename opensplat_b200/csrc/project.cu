@@ -52,7 +52,10 @@ __device__ __forceinline__ void load_cam(const float *__restrict__ viewmat,
 // `scales` holds log-scales (exp here), `quats` the raw quaternions (quat_to_rotmat normalises, as the reference's
 // does, so `quats / quats.norm()` needs no pass of its own), and sigmoid(opacity_logits) is written beside the
 // projection outputs for the rasterizer.
-template <bool ACT>
+// AA (with ACT only; DESIGN D19): the anti-aliased opacity -- sigmoid(logit) * comp, comp = sqrt(max(0, det0 / det)),
+// det0 the determinant of the screen covariance before the 0.3 px^2 blur and det the one after it, so the blurred
+// Gaussian carries the light of the unblurred one; comp = 0 where radii == 0.  Every other output is the ACT one.
+template <bool ACT, bool AA = false>
 __global__ void __launch_bounds__(PJ_THREADS)
 project_forward_kernel(int n, const float *__restrict__ means3d, const float *__restrict__ scales,
                        float glob_scale, const float *__restrict__ quats,
@@ -62,9 +65,11 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
                        float2 *__restrict__ xys, float *__restrict__ depths, int *__restrict__ radii,
                        float *__restrict__ conics, int *__restrict__ num_tiles_hit,
                        const float *__restrict__ opacity_logits, float *__restrict__ opacities) {
+    static_assert(ACT || !AA, "the anti-aliased opacity needs the activated projection");
     const int i = blockIdx.x * PJ_THREADS + threadIdx.x;
     if (i >= n) return;
-    if (ACT) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i]));
+    if (ACT && !AA) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i]));
+    float comp = 0.f;
     Cam cam;
     load_cam(viewmat, projmat, cam);
     const float *V = cam.V, *P = cam.P;
@@ -121,9 +126,10 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
 #pragma unroll
             for (int c = 0; c < 3; ++c)
                 TV[r][c] = T[r][0] * Cs[0][c] + T[r][1] * Cs[1][c] + T[r][2] * Cs[2][c];
-        const float cxx = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2] + 0.3f;
+        const float cxx0 = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2];
         const float cxy = TV[0][0] * T[1][0] + TV[0][1] * T[1][1] + TV[0][2] * T[1][2];
-        const float cyy = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2] + 0.3f;
+        const float cyy0 = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2];
+        const float cxx = cxx0 + 0.3f, cyy = cyy0 + 0.3f;
 
         // compute_cov2d_bounds (helpers.cuh:51-74)
         const float det = cxx * cyy - cxy * cxy;
@@ -155,9 +161,11 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
                 radius_i = (int)radius;
                 ux = pxc;
                 uy = pyc;
+                if (AA && radius_i > 0) comp = sqrtf(fmaxf(0.f, (cxx0 * cyy0 - cxy * cxy) / det));
             }
         }
     }
+    if (AA) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i])) * comp;
     float *c3o = cov3d + 6 * (size_t)i;
 #pragma unroll
     for (int k = 0; k < 6; ++k) c3o[k] = c3[k];
@@ -175,7 +183,10 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
 // gradient is taken through the sigmoid (x o (1 - o), from the saved activated opacity).
 // ACC: add this view's VJP to the four outputs (prev + vjp, one rounding each) instead of writing it -- the sum
 // over a trainer's views of one step, in view order.
-template <bool ACT, bool ACC>
+// AA: VJP of the anti-aliased forward (D19).  `opacities` holds the opacity LOGITS (o and comp are recomputed with the
+// forward's expressions, bit for bit); v_logit = v_opacity * comp * o (1 - o), and where comp > 0 the cotangent
+// v_opacity * o of comp is taken to the blurred covariance and added to vS before the T / J / clamp chain.
+template <bool ACT, bool ACC, bool AA = false>
 __global__ void __launch_bounds__(PJ_THREADS)
 project_backward_kernel(int n, const float *__restrict__ means3d, const float *__restrict__ scales,
                         float glob_scale, const float *__restrict__ quats,
@@ -187,9 +198,11 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
                         float *__restrict__ v_scale, float4 *__restrict__ v_quat,
                         const float *__restrict__ opacities, const float *__restrict__ v_opacity,
                         float *__restrict__ v_opacity_logits) {
+    static_assert(ACT || !AA, "the anti-aliased opacity needs the activated projection");
     const int i = blockIdx.x * PJ_THREADS + threadIdx.x;
     if (i >= n) return;
-    if (ACT) {
+    float comp = 0.f;
+    if (ACT && !AA) {
         const float o = opacities[i];
         if constexpr (ACC)
             v_opacity_logits[i] = v_opacity_logits[i] + (v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f);
@@ -227,9 +240,9 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
         const float gA = v_conic[3 * i], gB = 0.5f * v_conic[3 * i + 1], gC = v_conic[3 * i + 2];
         const float xg00 = A * gA + B * gB, xg01 = A * gB + B * gC;
         const float xg10 = B * gA + Cc * gB, xg11 = B * gB + Cc * gC;
-        const float vS00 = -(xg00 * A + xg01 * B);
-        const float vS01 = -(xg00 * B + xg01 * Cc);
-        const float vS11 = -(xg10 * B + xg11 * Cc);
+        float vS00 = -(xg00 * A + xg01 * B);
+        float vS01 = -(xg00 * B + xg01 * Cc);
+        float vS11 = -(xg10 * B + xg11 * Cc);
 
         // recompute forward intermediates
         const float4 q = reinterpret_cast<const float4 *>(quats)[i];
@@ -260,6 +273,32 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
         for (int c = 0; c < 3; ++c) {
             T[0][c] = J00 * V[c] + J02 * V[8 + c];
             T[1][c] = J11 * V[4 + c] + J12 * V[8 + c];
+        }
+        if constexpr (AA) {
+            // the forward's cov2d sums and det, recomputed in its order
+            float TV[2][3];
+#pragma unroll
+            for (int r = 0; r < 2; ++r)
+#pragma unroll
+                for (int c = 0; c < 3; ++c)
+                    TV[r][c] = T[r][0] * Cs[0][c] + T[r][1] * Cs[1][c] + T[r][2] * Cs[2][c];
+            const float cxx0 = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2];
+            const float cxy = TV[0][0] * T[1][0] + TV[0][1] * T[1][1] + TV[0][2] * T[1][2];
+            const float cyy0 = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2];
+            const float det = (cxx0 + 0.3f) * (cyy0 + 0.3f) - cxy * cxy;
+            comp = sqrtf(fmaxf(0.f, (cxx0 * cyy0 - cxy * cxy) / det));
+            if (v_opacity && comp > 0.f) {
+                // d comp^2 / d Sigma = ((1 - comp^2) Sigma^-1 - 0.3 det(Sigma^-1) I), per symmetric entry, written as
+                // 0.3 / det^2 [[cyy0^2 + cxy^2 + 0.3 cyy0, -cxy (cxx0 + cyy0 + 0.3)], [.., cxx0^2 + cxy^2 + 0.3 cxx0]]:
+                // the same value without the cancellation of the first form when Sigma0 is small against 0.3 I
+                const float o = 1.f / (1.f + expf(-opacities[i]));
+                const float k = 0.5f * (v_opacity[i] * o) / comp;
+                const float id = 1.f / det;
+                const float a = cyy0 * id, b = cxy * id, c = cxx0 * id, e = 0.3f * id;
+                vS00 = vS00 + k * (0.3f * (a * a + b * b + e * a));
+                vS01 = vS01 - k * (0.3f * (b * (a + c + e)));
+                vS11 = vS11 + k * (0.3f * (c * c + b * b + e * c));
+            }
         }
         float vST[2][3];
 #pragma unroll
@@ -326,6 +365,14 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
         vq = make_float4((gw - w * dot) * inv, (gx - x * dot) * inv, (gy - y * dot) * inv,
                          (gz - z * dot) * inv);
     }
+    if constexpr (AA) {
+        float vol = 0.f;
+        if (v_opacity) {
+            const float o = 1.f / (1.f + expf(-opacities[i]));
+            vol = v_opacity[i] * comp * o * (1.f - o);
+        }
+        v_opacity_logits[i] = ACC ? v_opacity_logits[i] + vol : vol;
+    }
     if constexpr (ACC) {
         const float4 pq = v_quat[i];
         v_mean3d[3 * i] += vm[0]; v_mean3d[3 * i + 1] += vm[1]; v_mean3d[3 * i + 2] += vm[2];
@@ -340,7 +387,7 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
 
 }  // namespace
 
-static int project_forward_impl(bool act, int n, const float *means3d, const float *scales, float glob_scale,
+static int project_forward_impl(bool act, bool aa, int n, const float *means3d, const float *scales, float glob_scale,
                                 const float *quats, const float *opacity_logits, const float *viewmat,
                                 const float *projmat, float fx, float fy, float cx, float cy, int img_h, int img_w,
                                 int tiles_x, int tiles_y, float clip_thresh, float *cov3d, float *xys, float *depths,
@@ -355,11 +402,11 @@ static int project_forward_impl(bool act, int n, const float *means3d, const flo
     // forward.cu:69-70 evaluates `0.5 * img_size.x / fx` in double and narrows
     const float tan_fovx = (float)(0.5 * (double)img_w / (double)fx);
     const float tan_fovy = (float)(0.5 * (double)img_h / (double)fy);
-#define GSB_PJ_F(A) project_forward_kernel<A><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
+#define GSB_PJ_F(A, AA) project_forward_kernel<A, AA><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
         n, means3d, scales, glob_scale, quats, viewmat, projmat, fx, fy, cx, cy, tan_fovx, tan_fovy, img_h, img_w,   \
         tiles_x, tiles_y, clip_thresh, cov3d, reinterpret_cast<float2 *>(xys), depths, radii, conics, num_tiles_hit, \
         opacity_logits, opacities)
-    if (act) GSB_PJ_F(true); else GSB_PJ_F(false);
+    if (aa) GSB_PJ_F(true, true); else if (act) GSB_PJ_F(true, false); else GSB_PJ_F(false, false);
 #undef GSB_PJ_F
     GSB_LAUNCH_CHECK();
     return 0;
@@ -371,7 +418,7 @@ extern "C" int gsb_project_forward(int n, const float *means3d, const float *sca
                                    int tiles_x, int tiles_y, float clip_thresh, float *cov3d, float *xys,
                                    float *depths, int32_t *radii, float *conics, int32_t *num_tiles_hit,
                                    gsb_stream_t stream) {
-    return project_forward_impl(false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx, fy, cx,
+    return project_forward_impl(false, false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx, fy, cx,
                                 cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii, conics,
                                 num_tiles_hit, nullptr, stream);
 }
@@ -383,12 +430,12 @@ extern "C" int gsb_project_forward_activated(int n, const float *means3d, const 
                                              float clip_thresh, float *cov3d, float *xys, float *depths,
                                              int32_t *radii, float *conics, int32_t *num_tiles_hit,
                                              float *opacities, gsb_stream_t stream) {
-    return project_forward_impl(true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, viewmat, projmat,
+    return project_forward_impl(true, false, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, viewmat, projmat,
                                 fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii,
                                 conics, num_tiles_hit, opacities, stream);
 }
 
-static int project_backward_impl(bool act, bool acc, int n, const float *means3d, const float *scales, float glob_scale,
+static int project_backward_impl(bool act, bool acc, bool aa, int n, const float *means3d, const float *scales, float glob_scale,
                                  const float *quats, const float *opacities, const float *viewmat,
                                  const float *projmat, float fx, float fy, int img_h, int img_w,
                                  const int32_t *radii, const float *conics, const float *v_xy, const float *v_depth,
@@ -402,11 +449,12 @@ static int project_backward_impl(bool act, bool acc, int n, const float *means3d
     GSB_CHECK_ARG(((uintptr_t)quats % 16) == 0 && ((uintptr_t)v_quat % 16) == 0 && ((uintptr_t)v_xy % 8) == 0);
     const float tan_fovx = (float)(0.5 * (double)img_w / (double)fx);
     const float tan_fovy = (float)(0.5 * (double)img_h / (double)fy);
-#define GSB_PJ_B(A, ACC) project_backward_kernel<A, ACC><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
+#define GSB_PJ_B(A, ACC, AA) project_backward_kernel<A, ACC, AA><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
         n, means3d, scales, glob_scale, quats, viewmat, projmat, fx, fy, tan_fovx, tan_fovy, img_h, img_w, radii,     \
         conics, reinterpret_cast<const float2 *>(v_xy), v_depth, v_conic, v_mean3d, v_scale,                          \
         reinterpret_cast<float4 *>(v_quat), opacities, v_opacity, v_opacity_logits)
-    if (acc) GSB_PJ_B(true, true); else if (act) GSB_PJ_B(true, false); else GSB_PJ_B(false, false);
+    if (aa) { if (acc) GSB_PJ_B(true, true, true); else GSB_PJ_B(true, false, true); }
+    else if (acc) GSB_PJ_B(true, true, false); else if (act) GSB_PJ_B(true, false, false); else GSB_PJ_B(false, false, false);
 #undef GSB_PJ_B
     GSB_LAUNCH_CHECK();
     return 0;
@@ -419,7 +467,7 @@ extern "C" int gsb_project_backward(int n, const float *means3d, const float *sc
                                     const float *v_xy, const float *v_depth, const float *v_conic,
                                     float *v_mean3d, float *v_scale, float *v_quat, gsb_stream_t stream) {
     (void)cov3d; (void)cx; (void)cy;
-    return project_backward_impl(false, false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx,
+    return project_backward_impl(false, false, false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx,
                                  fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, nullptr, v_mean3d, v_scale,
                                  v_quat, nullptr, stream);
 }
@@ -431,7 +479,7 @@ extern "C" int gsb_project_backward_activated(int n, const float *means3d, const
                                               const float *v_depth, const float *v_conic, const float *v_opacity,
                                               float *v_mean3d, float *v_log_scales, float *v_raw_quats,
                                               float *v_opacity_logits, gsb_stream_t stream) {
-    return project_backward_impl(true, false, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
+    return project_backward_impl(true, false, false, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
                                  projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
                                  v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
 }
@@ -444,7 +492,48 @@ extern "C" int gsb_project_backward_activated_acc(int n, const float *means3d, c
                                                   const float *v_xy, const float *v_depth, const float *v_conic,
                                                   const float *v_opacity, float *v_mean3d, float *v_log_scales,
                                                   float *v_raw_quats, float *v_opacity_logits, gsb_stream_t stream) {
-    return project_backward_impl(true, true, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
+    return project_backward_impl(true, true, false, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
                                  projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
                                  v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
+}
+
+// D19: the activated projection with the anti-aliased opacity, opacities = sigmoid(logits) * comp.
+extern "C" int gsb_project_forward_activated_aa(int n, const float *means3d, const float *log_scales,
+                                                float glob_scale, const float *raw_quats, const float *opacity_logits,
+                                                const float *viewmat, const float *projmat, float fx, float fy,
+                                                float cx, float cy, int img_h, int img_w, int tiles_x, int tiles_y,
+                                                float clip_thresh, float *cov3d, float *xys, float *depths,
+                                                int32_t *radii, float *conics, int32_t *num_tiles_hit,
+                                                float *opacities, gsb_stream_t stream) {
+    return project_forward_impl(true, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, viewmat,
+                                projmat, fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys,
+                                depths, radii, conics, num_tiles_hit, opacities, stream);
+}
+
+// Its VJP, from the opacity logits (the forward's opacities hold sigmoid * comp): written, and added in place.
+extern "C" int gsb_project_backward_activated_aa(int n, const float *means3d, const float *log_scales,
+                                                 float glob_scale, const float *raw_quats,
+                                                 const float *opacity_logits, const float *viewmat,
+                                                 const float *projmat, float fx, float fy, int img_h, int img_w,
+                                                 const int32_t *radii, const float *conics, const float *v_xy,
+                                                 const float *v_depth, const float *v_conic, const float *v_opacity,
+                                                 float *v_mean3d, float *v_log_scales, float *v_raw_quats,
+                                                 float *v_opacity_logits, gsb_stream_t stream) {
+    return project_backward_impl(true, false, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
+                                 viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic,
+                                 v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
+}
+
+extern "C" int gsb_project_backward_activated_aa_acc(int n, const float *means3d, const float *log_scales,
+                                                     float glob_scale, const float *raw_quats,
+                                                     const float *opacity_logits, const float *viewmat,
+                                                     const float *projmat, float fx, float fy, int img_h, int img_w,
+                                                     const int32_t *radii, const float *conics, const float *v_xy,
+                                                     const float *v_depth, const float *v_conic,
+                                                     const float *v_opacity, float *v_mean3d, float *v_log_scales,
+                                                     float *v_raw_quats, float *v_opacity_logits,
+                                                     gsb_stream_t stream) {
+    return project_backward_impl(true, true, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
+                                 viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic,
+                                 v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
 }

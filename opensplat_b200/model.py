@@ -85,9 +85,12 @@ def camera_setup(cam, downscale):
 class GaussianModel:
     def __init__(self, params, cfg=None, sh_degree=None, sh_degree_interval=1000, num_downscales=0,
                  resolution_schedule=3000, background=(0.6130, 0.0101, 0.3984), device="cuda:0", generator=None,
-                 group=None):
+                 group=None, antialiased=False):
         """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
-        featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits)."""
+        featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits).
+        antialiased: render with the anti-aliased opacity (DESIGN D19, ops.ProjectGaussiansActivatedAntialiased):
+        each Gaussian's opacity is scaled by how much the projection's 0.3 px^2 blur spread it.  The parameters, the
+        refinement and the saved files keep the raw opacity."""
         self.device = torch.device(device)
         self.cfg = cfg or RefineConfig()
         for k in PARAM_NAMES:
@@ -99,6 +102,7 @@ class GaussianModel:
         self.numDownscales, self.resolutionSchedule = int(num_downscales), int(resolution_schedule)
         self.backgroundColor = torch.tensor(background, dtype=torch.float32, device=self.device)
         self.group = group
+        self.antialiased = bool(antialiased)
         self.densifier = Densifier(self.cfg, generator=generator, group=group)
         self.writer = None
         self.xys = self.radii = None
@@ -154,7 +158,8 @@ class GaussianModel:
         view, proj, cam_pos = view.to(dev), proj.to(dev), cam_pos.to(dev)
         tb = ops.tile_bounds(width, height)
         # model.cpp:148-150,200 inside the projection: exp(scales), quaternion normalisation, sigmoid(opacities)
-        xys, depths, radii, conics, num_tiles_hit, _, opac = ops.ProjectGaussiansActivated.apply(
+        project = ops.ProjectGaussiansActivatedAntialiased if self.antialiased else ops.ProjectGaussiansActivated
+        xys, depths, radii, conics, num_tiles_hit, _, opac = project.apply(
             self.means, self.scales, 1.0, self.quats, self.opacities, view, proj @ view, fx, fy, cx, cy, height,
             width, tb)
         self.xys, self.radii, self.numTilesHit = xys, radii, num_tiles_hit

@@ -609,6 +609,13 @@ class ProjectGaussiansActivated(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat, fx, fy, cx, cy,
                 imgHeight, imgWidth, tileBounds, clipThresh=0.01):
+        return ProjectGaussiansActivated._forward(ctx, False, means, logScales, globScale, rawQuats, opacityLogits,
+                                                  viewMat, projMat, fx, fy, cx, cy, imgHeight, imgWidth, tileBounds,
+                                                  clipThresh)
+
+    @staticmethod
+    def _forward(ctx, aa, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat, fx, fy, cx, cy,
+                 imgHeight, imgWidth, tileBounds, clipThresh):
         n = means.shape[0]
         m3, ls, rq = capi.f32(means), capi.f32(logScales), capi.f32(rawQuats)
         ol = capi.f32(opacityLogits).reshape(n)
@@ -620,20 +627,23 @@ class ProjectGaussiansActivated(torch.autograd.Function):
         conics = _empty((n, 3), torch.float32, m3)
         nth = _empty((n,), torch.int32, m3)
         opac = _empty((n, 1), torch.float32, m3)
-        capi.check(capi.lib().gsb_project_forward_activated(
+        L = capi.lib()
+        capi.check((L.gsb_project_forward_activated_aa if aa else L.gsb_project_forward_activated)(
             n, capi.ptr(m3), capi.ptr(ls), float(globScale), capi.ptr(rq), capi.ptr(ol), capi.ptr(vm), capi.ptr(pm),
             float(fx), float(fy), float(cx), float(cy), int(imgHeight), int(imgWidth), tileBounds[0], tileBounds[1],
             float(clipThresh), capi.ptr(cov3d), capi.ptr(xys), capi.ptr(depths), capi.ptr(radii), capi.ptr(conics),
             capi.ptr(nth), capi.ptr(opac), capi.stream()))
-        ctx.meta = (float(globScale), float(fx), float(fy), int(imgHeight), int(imgWidth), tuple(opacityLogits.shape))
-        ctx.save_for_backward(m3, ls, rq, vm, pm, radii, conics, opac)
+        ctx.meta = (float(globScale), float(fx), float(fy), int(imgHeight), int(imgWidth), tuple(opacityLogits.shape),
+                    aa)
+        # the plain backward takes sigmoid(logits) from the forward, the anti-aliased one the logits themselves
+        ctx.save_for_backward(m3, ls, rq, vm, pm, radii, conics, ol if aa else opac)
         ctx.mark_non_differentiable(radii, nth)
         return xys, depths, radii, conics, nth, cov3d, opac
 
     @staticmethod
     def backward(ctx, v_xys, v_depths, v_radii, v_conics, v_numTiles, v_cov3d, v_opac):
         m3, ls, rq, vm, pm, radii, conics, opac = ctx.saved_tensors
-        gs, fx, fy, H, W, ol_shape = ctx.meta
+        gs, fx, fy, H, W, ol_shape, aa = ctx.meta
         n = m3.shape[0]
         if v_xys is None:
             v_xys = torch.zeros_like(m3[:, :2])
@@ -646,12 +656,28 @@ class ProjectGaussiansActivated(torch.autograd.Function):
         vx, vc = capi.f32(v_xys), capi.f32(v_conics)
         vd = capi.f32(v_depths) if v_depths is not None else None
         vo = capi.f32(v_opac).reshape(n) if v_opac is not None else None
-        capi.check(capi.lib().gsb_project_backward_activated(
+        L = capi.lib()
+        capi.check((L.gsb_project_backward_activated_aa if aa else L.gsb_project_backward_activated)(
             n, capi.ptr(m3), capi.ptr(ls), gs, capi.ptr(rq), capi.ptr(opac), capi.ptr(vm), capi.ptr(pm), fx, fy, H, W,
             capi.ptr(radii), capi.ptr(conics), capi.ptr(vx), capi.ptr(vd), capi.ptr(vc), capi.ptr(vo),
             capi.ptr(v_mean), capi.ptr(v_ls), capi.ptr(v_rq), capi.ptr(v_ol), capi.stream()))
         # 15 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4)
         return (v_mean, v_ls, None, v_rq, v_ol.reshape(ol_shape)) + (None,) * 10
+
+
+class ProjectGaussiansActivatedAntialiased(ProjectGaussiansActivated):
+    """ProjectGaussiansActivated with the anti-aliased opacity (DESIGN D19, gsplat's "antialiased" mode): the same
+    arguments and outputs, but opacities = sigmoid(logits) * sqrt(max(0, det0 / det)), det0 / det the determinants of
+    the screen covariance before / after the 0.3 px^2 blur (0 for a culled Gaussian), so that a Gaussian smaller than a
+    pixel is not drawn brighter than it is.  The other six outputs are those of ProjectGaussiansActivated, bit for bit.
+    C++ twin: gsb::ProjectGaussiansActivatedAntialiased."""
+
+    @staticmethod
+    def forward(ctx, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat, fx, fy, cx, cy,
+                imgHeight, imgWidth, tileBounds, clipThresh=0.01):
+        return ProjectGaussiansActivated._forward(ctx, True, means, logScales, globScale, rawQuats, opacityLogits,
+                                                  viewMat, projMat, fx, fy, cx, cy, imgHeight, imgWidth, tileBounds,
+                                                  clipThresh)
 
 
 class SphericalHarmonics(torch.autograd.Function):

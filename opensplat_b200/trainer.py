@@ -119,13 +119,15 @@ def view_setups(cams, gts, views, downscale):
 class SplatTrainer:
     def __init__(self, params, cfg=None, sh_degree=None, sh_degree_interval=1000, num_downscales=0,
                  resolution_schedule=3000, background=(0.6130, 0.0101, 0.3984), device="cuda:0", generator=None,
-                 ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1):
+                 ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1, antialiased=False):
         """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
         featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
         m_capacity: initial intersection capacity of the binning buffers (grown on demand).
         group: a process group to train data-parallel over camera views (any size, 1 included); every rank
         constructs the trainer with the same parameters and calls step() with the same step numbers.
-        views_per_step: B camera views per step (per rank under a group); step() then takes B cameras and B images."""
+        views_per_step: B camera views per step (per rank under a group); step() then takes B cameras and B images.
+        antialiased: train and render with the anti-aliased opacity (DESIGN D19), as model.GaussianModel(antialiased=
+        True): the projection kernels are the _aa ones, and nothing else in the step changes."""
         import torch.distributed as dist
         self.views_per_step = B = int(views_per_step)
         if B < 1:
@@ -135,6 +137,7 @@ class SplatTrainer:
                                "over camera views")
         self.device = torch.device(device)
         self.cfg = cfg or RefineConfig()
+        self.antialiased = bool(antialiased)
         t = {k: torch.as_tensor(params[k]).to(device=self.device, dtype=torch.float32) for k in PARAM_NAMES}
         n, k_bases = t["means"].shape[0], t["featuresRest"].shape[1] + 1
         self.sh_degree = ops.deg_from_sh(k_bases) if sh_degree is None else int(sh_degree)
@@ -181,7 +184,7 @@ class SplatTrainer:
     def _alloc_gaussian_scratch(self):
         """The trainer's per-Gaussian buffers, (re)built at construction and after a refinement."""
         pp, n, B, d = self.pipe, self.pipe.n, self.views_per_step, self.device
-        self.opac = torch.empty(n, dtype=torch.float32, device=d)     # sigmoid(logits) for the blend
+        self.opac = torch.empty(n, dtype=torch.float32, device=d)     # sigmoid(logits) (x comp: D19) for the blend
         self.v_opac = torch.empty(n, dtype=torch.float32, device=d)   # blend gradient w.r.t. it
         # The B views' colours and colour gradients, [B,n,3] each.  At B = 1 they are the pipeline's own [n,3]
         # buffers; under a group the colour gradients live in the exchange's symmetric allocation.
@@ -342,7 +345,8 @@ class SplatTrainer:
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         n, p, tb, H, W = pp.n, pp.p, pp.tb, pp.H, pp.W
         fx, fy, cx, cy = intr
-        capi.check(L.gsb_project_forward_activated(
+        project = L.gsb_project_forward_activated_aa if self.antialiased else L.gsb_project_forward_activated
+        capi.check(project(
             n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmats[b]),
             P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
             P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac), s))
@@ -373,8 +377,13 @@ class SplatTrainer:
         if ex is not None and ex.overlap and b == self.views_per_step - 1:
             # every colour slot is final: colour pulls + SH expansion start now, on a side stream
             ex.start_colour(degrees_to_use=use, rgbs=self.rgbs_views)
-        pj = L.gsb_project_backward_activated if b == 0 else L.gsb_project_backward_activated_acc
-        capi.check(pj(n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(self.opac), P(self.viewmats[b]),
+        if self.antialiased:     # D19: the backward recomputes o and comp from the logits
+            pj = L.gsb_project_backward_activated_aa if b == 0 else L.gsb_project_backward_activated_aa_acc
+            opac = p["opacities"]
+        else:
+            pj = L.gsb_project_backward_activated if b == 0 else L.gsb_project_backward_activated_acc
+            opac = self.opac
+        capi.check(pj(n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(opac), P(self.viewmats[b]),
                       P(self.projmats[b]), fx, fy, pp.H, pp.W, P(pp.radii), P(pp.conics), P(pp.v_xy), None,
                       P(pp.v_conic), P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]),
                       capi.stream()))
