@@ -456,6 +456,54 @@ int gsb_densify_gather_rows(int new_n, int row_floats, const int32_t *src_map, c
 int gsb_reset_opacity(int n, float max_logit, float *opacities, float *exp_avg, float *exp_avg_sq,
                       gsb_stream_t stream);
 
+/* ---- 3DGS-MCMC refinement (Kheradmand et al. 2024, gsplat's MCMCStrategy; DESIGN.md D20) ----------------------
+ * o = 1.f / (1.f + expf(-logit)) throughout (the raw sigmoid, as the projection forms it).  Random numbers come from
+ *   Philox4x32-10 with key (key0, key1) = (seed & 0xffffffff, seed >> 32) and counter (index, step, tag, 0); tag 0 is
+ *   the position noise (index = Gaussian), 1 the relocation samples, 2 the growth samples (index = sample number).
+ *   A uniform is ((x0 >> 5) 2^26 + (x1 >> 6)) 2^-53; normals are Box-Muller on u1 = ((a >> 8) + 1) 2^-24,
+ *   u2 = (b >> 8) 2^-24: (x0, x1) give z0 (cos) and z1 (sin), (x2, x3) give z2 (cos).
+ * The flat layout is a HOST array of num_segments (<= GSB_MCMC_MAX_SEGMENTS) gsb_row_segment: slice s holds row i at
+ *   floats [offset + i * row_floats, offset + (i + 1) * row_floats) of the flat buffers.
+ * gsb_mcmc_plan: the weights w_i = o_i in fp64 (0 where o_i <= min_opacity when mask_dead), their inclusive scan into
+ *   cdf [n] (fp64, monotone: a weight-0 index is never drawn; T = cdf[n-1]), with mask_dead the dead indices in
+ *   ascending order into dead [n], and result (device int32[4]) = {n_dead, T > 0, any o > 0, 0}: the one read-back
+ *   of a refinement.  workspace: gsb_mcmc_workspace_bytes(n), 256-byte aligned.  n < 2^29.
+ * gsb_mcmc_sample: samples[j] = the smallest i with cdf[i] > u_j T (u_j the uniform of counter (j, step, tag, 0)),
+ *   j < num_samples; counts [n] = how often each index was drawn (zeroed by the call).  Needs T > 0.
+ * gsb_mcmc_relocate: every row i with counts[i] > 0, ratio r = min(counts[i] + 1, 51):
+ *   alpha = -expm1(log1p(-o) / r), D = sum_{k<r} (-1)^k C(r,k+1) alpha^(k+1) / sqrt(k+1), logit <-
+ *   logit(clamp(alpha, min_opacity, 1 - 2^-23)), log-scales <- s + log(o / D), in fp64 rounded once to fp32; with
+ *   zero_moments its Adam moments in every slice are zeroed.
+ * gsb_mcmc_copy_rows: row dst_rows[j] <- row src_rows[j] of param in every slice (the rows must not overlap).
+ * gsb_mcmc_regularize: grad_logits += opacity_coef * o(1 - o), grad_log_scales += scale_coef * exp(s) (the gradients
+ *   of opacity_reg mean|o| + scale_reg mean|exp s| with opacity_coef = opacity_reg / n, scale_coef = scale_reg / 3n).
+ * gsb_mcmc_add_noise: means += Sigma (z * (sigma_100((1 - o) - 0.995f) * noise_scale)), z the three normals of counter
+ *   (i, step, 0, 0), Sigma = R diag(exp(2 s)) R^T with R from raw_quats / |raw_quats| (16-byte aligned),
+ *   sigma_100(x) = 1 / (1 + exp(-100 x)).
+ * gsb_mcmc_draws: the raw Philox words [count,4] and normals [count,3] of counters (j, step, tag, 0), j < count
+ *   (either output may be NULL; words 16-byte aligned). */
+#define GSB_MCMC_MAX_SEGMENTS 8
+typedef struct gsb_row_segment {
+    long long offset;
+    int row_floats, reserved;
+} gsb_row_segment;
+size_t gsb_mcmc_workspace_bytes(int n);
+int gsb_mcmc_plan(int n, const float *logits, float min_opacity, int mask_dead, void *workspace,
+                  size_t workspace_bytes, double *cdf, int32_t *dead, int32_t *result, gsb_stream_t stream);
+int gsb_mcmc_sample(int num_samples, int n, const double *cdf, unsigned key0, unsigned key1, int step, int tag,
+                    int32_t *samples, int32_t *counts, gsb_stream_t stream);
+int gsb_mcmc_relocate(int n, const int32_t *counts, float min_opacity, float *logits, float *log_scales,
+                      int zero_moments, int num_segments, const gsb_row_segment *segments, float *exp_avg,
+                      float *exp_avg_sq, gsb_stream_t stream);
+int gsb_mcmc_copy_rows(int num_rows, const int32_t *dst_rows, const int32_t *src_rows, int num_segments,
+                       const gsb_row_segment *segments, float *param, gsb_stream_t stream);
+int gsb_mcmc_regularize(int n, const float *logits, const float *log_scales, float opacity_coef, float scale_coef,
+                        float *grad_logits, float *grad_log_scales, gsb_stream_t stream);
+int gsb_mcmc_add_noise(int n, const float *logits, const float *log_scales, const float *raw_quats, unsigned key0,
+                       unsigned key1, int step, float noise_scale, float *means, gsb_stream_t stream);
+int gsb_mcmc_draws(int count, unsigned key0, unsigned key1, int step, int tag, int32_t *words, float *normals,
+                   gsb_stream_t stream);
+
 /* ---- Scene export (Model::savePly model.cpp:505-558, Model::saveSplat :560-594; SURVEY.md 8f row 4) ----
  * Packs the file BODY on the device (the caller writes the text header and copies the rows D2H, typically on a
  * side stream into pinned memory).  features_dc / features_rest take a row stride in floats so both the reference's

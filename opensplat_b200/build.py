@@ -26,6 +26,7 @@ SOURCES = {
     "fused.cu": [],
     "ssim.cu": [],
     "densify.cu": [],
+    "mcmc.cu": [],
     "export.cu": ["--fmad=false"],
     "knn.cu": ["--fmad=false"],
     "image.cu": ["--fmad=false"],

@@ -85,6 +85,18 @@ _SIGS = {
     "gsb_densify_means_scales": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp]),
     "gsb_densify_gather_rows": (_i, [_i, _i, _vp, _vp, _vp, _i, _vp]),
     "gsb_reset_opacity": (_i, [_i, _f, _vp, _vp, _vp, _vp]),
+    "gsb_mcmc_workspace_bytes": (_sz, [_i]),
+    # n, logits, min_opacity, mask_dead, workspace, workspace_bytes, cdf, dead, result, stream
+    "gsb_mcmc_plan": (_i, [_i, _vp, _f, _i, _vp, _sz, _vp, _vp, _vp, _vp]),
+    # num_samples, n, cdf, key0, key1, step, tag, samples, counts, stream
+    "gsb_mcmc_sample": (_i, [_i, _i, _vp, C.c_uint, C.c_uint, _i, _i, _vp, _vp, _vp]),
+    # n, counts, min_opacity, logits, log_scales, zero_moments, num_segments, segments (host), exp_avg, exp_avg_sq, stream
+    "gsb_mcmc_relocate": (_i, [_i, _vp, _f, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "gsb_mcmc_copy_rows": (_i, [_i, _vp, _vp, _i, _vp, _vp, _vp]),
+    "gsb_mcmc_regularize": (_i, [_i, _vp, _vp, _f, _f, _vp, _vp, _vp]),
+    # n, logits, log_scales, raw_quats, key0, key1, step, noise_scale, means, stream
+    "gsb_mcmc_add_noise": (_i, [_i, _vp, _vp, _vp, C.c_uint, C.c_uint, _i, _f, _vp, _vp]),
+    "gsb_mcmc_draws": (_i, [_i, C.c_uint, C.c_uint, _i, _i, _vp, _vp, _vp]),
     "gsb_ply_row_floats": (_i, [_i]),
     "gsb_pack_ply_rows": (_i, [_i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp]),
     "gsb_unpack_ply_rows": (_i, [_i, _i, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp]),
@@ -112,6 +124,16 @@ class AdamSegment(C.Structure):
     """gsb_adam_segment (include/gsplat_b200.h)."""
     _fields_ = [("offset", C.c_longlong), ("count", C.c_longlong), ("row_floats", C.c_int),
                 ("head_floats", C.c_int), ("lr_head", C.c_float), ("lr_rest", C.c_float)]
+
+
+MCMC_MAX_SEGMENTS = 8   # GSB_MCMC_MAX_SEGMENTS
+
+
+class RowSegment(C.Structure):
+    """gsb_row_segment (include/gsplat_b200.h)."""
+    _fields_ = [("offset", C.c_longlong), ("row_floats", C.c_int), ("reserved", C.c_int)]
+
+
 # optional symbols (experimental entry points) are bound when present
 _OPT_SIGS = {}
 

@@ -91,6 +91,10 @@ class GaussianModel:
         antialiased: render with the anti-aliased opacity (DESIGN D19, ops.ProjectGaussiansActivatedAntialiased):
         each Gaussian's opacity is scaled by how much the projection's 0.3 px^2 blur spread it.  The parameters, the
         refinement and the saved files keep the raw opacity."""
+        from .mcmc import MCMCConfig
+        if isinstance(cfg, MCMCConfig):
+            raise ValueError("GaussianModel refines as the reference does (RefineConfig); the MCMC strategy "
+                             "(MCMCConfig) runs in trainer.SplatTrainer")
         self.device = torch.device(device)
         self.cfg = cfg or RefineConfig()
         for k in PARAM_NAMES:

@@ -53,7 +53,12 @@ step, so the replicas stay bit-identical; the statistics of a refinement are red
 more than one rank, a rank whose views hit nothing runs the backward pass (exact zeros), contributes zero statistics
 and takes every collective, as model.GaussianModel does under a group (parallel.allreduce_tensor_grads,
 Densifier.after_train).  Between refinements a step still allocates nothing and waits on the host once per view (the
-barriers are device-side)."""
+barriers are device-side).
+
+Under a Gaussian budget (`cfg=mcmc.MCMCConfig(...)`, DESIGN D20) the step takes no densification statistics; the
+regularisers' gradients are added after the views are averaged and exchanged, and after Adam mcmc.MCMCRefiner
+relocates and grows the set on a refinement step and adds the position noise.  Every draw is keyed by (seed, step,
+index), so replicas stay identical without a collective."""
 import ctypes as C
 
 import torch
@@ -61,6 +66,7 @@ import torch
 from . import capi, ops
 from .densify import Densifier, RefineConfig
 from .export import SceneWriter
+from .mcmc import MCMCConfig, MCMCRefiner
 from .model import (LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, Camera, camera_setup, downscale_factor,
                     means_learning_rate)
 from .parallel import flat_views
@@ -122,6 +128,8 @@ class SplatTrainer:
                  ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1, antialiased=False):
         """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
         featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
+        cfg: densify.RefineConfig (the reference's refinement, the default) or mcmc.MCMCConfig (3DGS-MCMC under a
+        Gaussian budget, DESIGN D20: no densification statistics are taken, the loss returned stays the image loss).
         m_capacity: initial intersection capacity of the binning buffers (grown on demand).
         group: a process group to train data-parallel over camera views (any size, 1 included); every rank
         constructs the trainer with the same parameters and calls step() with the same step numbers.
@@ -157,7 +165,9 @@ class SplatTrainer:
         pp.background.copy_(torch.tensor(background, dtype=torch.float32))
         self.L = capi.lib()
         self.lr = dict(LEARNING_RATES)
-        self.densifier = Densifier(self.cfg, generator=generator, group=group)
+        # the refinement strategy: the reference's Model::afterTrain (RefineConfig) or 3DGS-MCMC (MCMCConfig, D20)
+        self.refiner = MCMCRefiner(self.cfg) if isinstance(self.cfg, MCMCConfig) else None
+        self.densifier = None if self.refiner is not None else Densifier(self.cfg, generator=generator, group=group)
         # the B cameras: views [B,16] | projs [B,16] | centres [B,3], one pinned staging block, one upload per step
         self.cams_host = torch.zeros(35 * B, dtype=torch.float32).pin_memory()
         self.cams_dev = torch.zeros(35 * B, dtype=torch.float32, device=self.device)
@@ -252,15 +262,21 @@ class SplatTrainer:
             if B > 1 or visible[b] or self.world > 1:
                 self._backward_view(b, use, intr[0], intr[1])
             # this view's densification statistics (pp.v_xy / pp.radii are overwritten by the next view)
-            self.densifier.accumulate_view(step, pp.v_xy if visible[b] else None, pp.radii, H, W)
+            if self.densifier is not None:
+                self.densifier.accumulate_view(step, pp.v_xy if visible[b] else None, pp.radii, H, W)
         # A step whose views all hit nothing trains nothing; with more than one rank it still takes part in the step
         # (the Adam step every replica takes, the refinement's collectives; see the module docstring).
         trains = any(visible) or self.world > 1
         if trains:
             self._sh_backward(use)
+            if self.refiner is not None:     # D20: the regularisers, on the averaged and exchanged gradients
+                self.refiner.regularize(pp)
             self._adam_step()
         self.lr["means"] = means_learning_rate(step, self.cfg.max_steps, MEANS_LR_INIT)
-        if trains:
+        if trains and self.refiner is not None:
+            # ---- D20: relocation and growth on a refinement step, then the position noise ----
+            self._adopt(*self.refiner.finish_step(step, pp, self.lr["means"]))
+        elif trains:
             # ---- the rest of Model::afterTrain on views into the flat buffers ----
             self._adopt(*self.densifier.finish_step(step, pp.p, flat_views(pp.adam_m, pp.offs),
                                                     flat_views(pp.adam_v, pp.offs), H, W))
@@ -424,7 +440,7 @@ class SplatTrainer:
                                                  1.0 - 0.999 ** t, capi.stream()))
 
     def _adopt(self, new_p, new_m, new_v, info):
-        """The densifier's result: a changed Gaussian set re-creates the flat layout (the only allocations of a
+        """The refinement's result (densify.Densifier or mcmc.MCMCRefiner): a changed Gaussian set re-creates the flat layout (the only allocations of a
         step)."""
         pp = self.pipe
         if new_p is not pp.p:

@@ -18,6 +18,9 @@ per view, keeps each view's xys.grad and radii, scales the leaf gradients by 1/B
 averages over the ranks) and accumulates the statistics view by view (Densifier.accumulate_view, finish_step).  On
 the densification step the last view of rank 1 (of rank 0 at world size 1) is turned around.  The steady state then
 expects B host waits per step.
+--mcmc: the MCMC strategy instead (SplatTrainer(cfg=mcmc.MCMCConfig), DESIGN D20; GaussianModel has no counterpart):
+relocations and growth from a set with faint Gaussians, replicas bit-identical (parameters and moments) after every
+step, and at world size 1 the run bit-identical to the same run without a group.
 Rank 0 prints one line ending in `check_ok=True|False`; the exit code is 0 iff every check held on every rank."""
 import argparse
 import os
@@ -32,7 +35,9 @@ import torch.distributed as dist  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--views-per-rank", type=int, default=1)
-B = ap.parse_args().views_per_rank
+ap.add_argument("--mcmc", action="store_true")
+ARGS = ap.parse_args()
+B = ARGS.views_per_rank
 rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
 torch.cuda.set_device(local)
 DEV = torch.device("cuda", local)
@@ -230,7 +235,53 @@ def steady_state():
     return torch.cuda.memory_stats(DEV)["allocation.all.allocated"] - before, len(waits)
 
 
+def run_mcmc(group):
+    """The MCMC trainer on this rank's views: (trainer, counts, relocated, replicas in sync after every step)."""
+    from opensplat_b200.mcmc import MCMCConfig
+    pm = params()
+    pm["opacities"][:300] = -8.0                     # faint: relocated at the first refinement
+    n0 = pm["means"].shape[0]
+    cfg = MCMCConfig(refine_start=4, refine_every=6, cap_max=int(1.12 * n0), max_steps=200, seed=SEED)
+    tr = SplatTrainer(pm, cfg, device=DEV, ssim_weight=SSIM_W, group=group, views_per_step=B, **KW)
+    counts, relocated, in_sync = [], 0, True
+    for step in range(1, STEPS + 1):
+        if B == 1:
+            tr.step(*view(step), step)
+        else:
+            vs = views(step)
+            tr.step([c for c, _ in vs], [g for _, g in vs], step)
+        counts.append(tr.n)
+        relocated += tr.last_info.get("relocated", 0)
+        if group is not None:
+            pp = tr.pipe
+            in_sync = in_sync and all(parallel.replicas_in_sync(t, world) for t in (pp.param_flat, pp.adam_m, pp.adam_v))
+    return tr, np.array(counts), relocated, in_sync
+
+
+def check_mcmc():
+    tr, ct, relocated, in_sync = run_mcmc(dist.group.WORLD)
+    plain_exact = None
+    if world == 1:
+        tp, cp, _, _ = run_mcmc(None)
+        plain_exact = bool(np.array_equal(cp, ct) and all(torch.equal(a, b) for a, b in (
+            (tp.pipe.param_flat, tr.pipe.param_flat), (tp.pipe.adam_m, tr.pipe.adam_m),
+            (tp.pipe.adam_v, tr.pipe.adam_v))))
+    refined = bool(ct[-1] > ct[0] and relocated >= 300)
+    flags = torch.tensor([int(in_sync), int(refined), int(plain_exact is not False)], device=DEV)
+    dist.all_reduce(flags, op=dist.ReduceOp.MIN)
+    good = bool(flags.all())
+    if rank == 0:
+        print(f"parallel mcmc check world={world}: counts {ct[0]}->{ct[-1]} relocated={relocated} "
+              f"replicas_in_sync={bool(flags[0])} refined={bool(flags[1])} plain_trainer_bit_identical={plain_exact} "
+              + (f"views_per_rank={B} " if B > 1 else "") + f"check_ok={good}")
+    return good
+
+
 dist.init_process_group("nccl", device_id=DEV)
+if ARGS.mcmc:
+    ok_mcmc = check_mcmc()
+    dist.destroy_process_group()
+    sys.exit(0 if ok_mcmc else 1)
 tr, lt, ct, in_sync, empty_visible = run_trainer(dist.group.WORLD, check_sync=True)
 model, lm, cm = run_model()
 ok, dloss, exact = compare(model, tr, lm, lt, cm, ct)
