@@ -381,9 +381,9 @@ int gsb_adam_step(long long n, float *param, const float *grad, float *exp_avg, 
  *   entries; segment s covers floats [offset, offset + count) of all four buffers (offset a multiple of 4; the
  *   buffers 16-byte aligned), and its element e takes lr_head if e % row_floats < head_floats, lr_rest otherwise
  *   (a merged [n,K,3] SH block: row_floats = 3K, head_floats = 3 gives featuresDc / featuresRest their own rates).
- *   Floats outside every segment are not touched.  Same update as gsb_adam_step, with one rounding for every float:
- *   the parameter step's product is rounded before the subtraction.  gsb_adam_step's compiled kernel fuses that step
- *   into one FMA on every fourth float and on its scalar tail, so those floats can differ in the last bit. */
+ *   Floats outside every segment are not touched.  Same update as gsb_adam_step, rounded the same way for every
+ *   float of both entry points (the parameter step's product is rounded before the subtraction), so a float gets
+ *   the same bits from either call. */
 #define GSB_ADAM_MAX_SEGMENTS 8
 typedef struct gsb_adam_segment {
     long long offset, count;

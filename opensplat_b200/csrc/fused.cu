@@ -43,16 +43,25 @@ mse_loss_grad_kernel(long long n4, long long n, const float *__restrict__ img,
     }
 }
 
+// One Adam update of one element with its roundings spelled out: FFMA for m, v and the denominator, the parameter
+// step as FMUL + FSUB.  Left to the compiler, the contraction of the step depends on the surrounding code (it once
+// fused it into one FFMA on some vector lanes and not others), so every path of both Adam kernels calls this one
+// function: an element's result does not depend on the kernel, the path or the lane it falls on.
+__device__ __forceinline__ void adam_update(float &pp, float gg, float &mm, float &vv, float lr, float b1, float b2,
+                                            float eps, float inv_bc1, float inv_sqrt_bc2) {
+    mm = __fmaf_rn(1.f - b1, gg, b1 * mm);
+    vv = __fmaf_rn(gg, (1.f - b2) * gg, b2 * vv);
+    // torch.optim.Adam: p -= lr/bc1 * m / (sqrt(v)/sqrt(bc2) + eps)
+    pp = __fsub_rn(pp, __fmul_rn(lr * inv_bc1, __fdividef(mm, __fmaf_rn(sqrtf(vv), inv_sqrt_bc2, eps))));
+}
+
 __global__ void __launch_bounds__(256)
 adam_kernel(long long n4, long long n, float *__restrict__ p, const float *__restrict__ g,
             float *__restrict__ m, float *__restrict__ v, float lr, float b1, float b2, float eps,
             float inv_bc1, float inv_sqrt_bc2) {
     const long long stride = (long long)gridDim.x * blockDim.x;
     auto upd = [&](float &pp, float gg, float &mm, float &vv) {
-        mm = b1 * mm + (1.f - b1) * gg;
-        vv = b2 * vv + (1.f - b2) * gg * gg;
-        // torch.optim.Adam: p -= lr/bc1 * m / (sqrt(v)/sqrt(bc2) + eps)
-        pp -= lr * inv_bc1 * __fdividef(mm, sqrtf(vv) * inv_sqrt_bc2 + eps);
+        adam_update(pp, gg, mm, vv, lr, b1, b2, eps, inv_bc1, inv_sqrt_bc2);
     };
     // two float4 per thread per trip: 8 independent 128-bit loads in flight before the first use
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -81,19 +90,6 @@ adam_kernel(long long n4, long long n, float *__restrict__ p, const float *__res
     }
     for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
         upd(p[i], g[i], m[i], v[i]);
-}
-
-// adam_kernel's update of one element with its roundings spelled out: FFMA for m, v and the denominator, the
-// parameter step as FMUL + FADD.  Left to the compiler, the contraction depends on the surrounding code: adam_kernel's
-// SASS rounds the parameter step like this in lanes x-z of its float4 path but fuses it into one FFMA in lane w and in
-// its scalar tail, so those floats of a gsb_adam_step call can differ from this in the last bit.  Both paths of the
-// segmented kernel call this one function, so its result does not depend on where a float falls.
-__device__ __forceinline__ void adam_update(float &pp, float gg, float &mm, float &vv, float lr, float b1, float b2,
-                                            float eps, float inv_bc1, float inv_sqrt_bc2) {
-    mm = __fmaf_rn(1.f - b1, gg, b1 * mm);
-    vv = __fmaf_rn(gg, (1.f - b2) * gg, b2 * vv);
-    // torch.optim.Adam: p -= lr/bc1 * m / (sqrt(v)/sqrt(bc2) + eps)
-    pp = __fsub_rn(pp, __fmul_rn(lr * inv_bc1, __fdividef(mm, __fmaf_rn(sqrtf(vv), inv_sqrt_bc2, eps))));
 }
 
 // The segment table travels by value in the kernel's parameter space (8 x 32 B).
@@ -234,12 +230,11 @@ int sm_count() {
 // loss_out (device float) is zeroed here (stream-ordered) and then accumulated into by the kernel.
 extern "C" int gsb_mse_loss_grad(long long n, const float *img, const float *target, float *v_img,
                                  float *loss_out, float inv_count, gsb_stream_t stream) {
-    GSB_CHECK_ARG(n >= 0);
-    if (n == 0) return 0;
-    GSB_CHECK_ARG(img && target && v_img && loss_out);
+    GSB_CHECK_ARG(n >= 0 && loss_out && (n == 0 || (img && target && v_img)));
+    GSB_CUDA(cudaMemsetAsync(loss_out, 0, sizeof(float), (cudaStream_t)stream));
+    if (n == 0) return 0;     // an empty image has loss 0
     const bool vec = (((uintptr_t)img | (uintptr_t)target | (uintptr_t)v_img) % 16) == 0;
     const long long n4 = vec ? n / 4 : 0;
-    GSB_CUDA(cudaMemsetAsync(loss_out, 0, sizeof(float), (cudaStream_t)stream));
     mse_loss_grad_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n4, n, img, target, v_img, loss_out,
                                                                         inv_count);
     GSB_LAUNCH_CHECK();

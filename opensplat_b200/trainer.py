@@ -8,8 +8,9 @@ pipeline.SplatPipeline, without autograd:
 
 It runs the kernels model.GaussianModel runs, with the same camera and learning-rate code, in the same order except
 that a view's densification statistics are taken right after its backward pass (they read only the view's xys
-gradient and radii, which nothing later in the step writes), so the two follow the same trajectory (same Gaussian counts, losses to rounding; the segmented Adam rounds the parameter
-step of some floats differently from gsb_adam_step, see include/gsplat_b200.h).  What changes is the bookkeeping
+gradient and radii, which nothing later in the step writes), so the two follow the same trajectory (same Gaussian counts, and
+at one view per step without a group the same parameter and moment bits: the segmented Adam rounds every float as
+gsb_adam_step does, see include/gsplat_b200.h).  What changes is the bookkeeping
 around them: one segmented Adam launch instead of six, no autograd nodes, and one host wait per step (the binning read-back, whose stats[3] visible count replaces the
 `radii.sum() == 0` test of model.cpp:173).  Between refinements a step allocates no device memory; a refinement
 (densify.Densifier, unchanged) re-creates the flat layout through SplatPipeline.resize_gaussians.

@@ -244,8 +244,7 @@ def test_trainer_follows_gaussian_model_through_refinements():
     tr, lt, ct = tg.run_trainer(p, cams, gts_d, steps, seed, cfg=tg.refine_config(), sh_degree_interval=8,
                                 antialiased=True)
     assert cm[18] == len(p["means"]) and cm[19] != cm[18] and cm[29] != cm[28]
-    exact = tg._compare(model, tr, lm, lt, cm, ct)
-    print(f"antialiased trainer vs GaussianModel over {steps} steps: bit-identical = {exact}")
+    tg._compare(model, tr, lm, lt, cm, ct, exact=True)
     # and the mode changes the training: the plain trainer's losses differ
     _, lp, _ = tg.run_trainer(p, cams, gts_d, 4, seed, cfg=tg.refine_config(), sh_degree_interval=8)
     assert np.abs(lp - lt[:4]).max() > 1e-4
@@ -259,7 +258,7 @@ def test_trainer_follows_gaussian_model_through_the_downscale_schedule():
     model, lm, cm = tg.run_model(p, cams, gts_d, 12, 3, cfg=tg.refine_config(), **kw)
     tr, lt, ct = tg.run_trainer(p, cams, gts_d, 12, 3, cfg=tg.refine_config(), **kw)
     assert tr.resolution == (W, H) and tr.pixel_reallocs == 1
-    tg._compare(model, tr, lm, lt, cm, ct)
+    tg._compare(model, tr, lm, lt, cm, ct, exact=True)
 
 
 def test_two_view_step_is_the_mean_of_two_one_view_passes():
