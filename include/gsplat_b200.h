@@ -504,6 +504,34 @@ int gsb_mcmc_add_noise(int n, const float *logits, const float *log_scales, cons
 int gsb_mcmc_draws(int count, unsigned key0, unsigned key1, int step, int tag, int32_t *words, float *normals,
                    gsb_stream_t stream);
 
+/* ---- Per-image bilateral grids (Wang et al. 2024; gsplat's bilateral-grid module; DESIGN.md D21) --------------
+ * A grid is GSB_BILAGRID_L x _Y x _X cells of 12 floats, stored channels-last [L][Y][X][12] (GSB_BILAGRID_FLOATS
+ *   floats, 16-byte aligned); a cell's 12 floats are the row-major 3x4 affine matrix [A | b].  Every grid starts at
+ *   the identity.  rgb, out, v_out and v_rgb are [H,W,3] fp32 images, 1 <= H, W <= 32768.
+ * gsb_bilagrid_slice_forward: out = A rgb + b with the coefficients trilinearly interpolated at
+ *   gx = ((px + 0.5) / W)(X - 1), gy = ((py + 0.5) / H)(Y - 1), gz = clamp((0.299 r + 0.587 g) + 0.114 b, 0, 1)(L - 1)
+ *   (F.grid_sample with align_corners=True and border padding, then the affine map); out is not clamped.
+ * gsb_bilagrid_slice_backward: v_rgb = A^T v_out + (dout/dz . v_out)(0.299, 0.587, 0.114) (written; the luma term is
+ *   0 where z <= 0 or z >= 1, and at an interior integer gz = k the derivative is the forward difference of cells k
+ *   and k + 1), and v_grid += scale * (trilinear weights x v_out (x) (rgb, 1)), summed without atomics in a fixed
+ *   order: the same inputs give the same bits.  workspace: gsb_bilagrid_workspace_bytes(H, W), 256-byte aligned.
+ * gsb_bilagrid_tv: v_grids = weight * dTV/dG over num_grids consecutive grids (written, not added), TV(G) = the sum
+ *   over the axes x, y, l of the mean of (G[i+1] - G[i])^2 over every element of that axis's difference tensor, all
+ *   grids included; with tv_out (a device float) the value TV(G) through a deterministic fp64 reduction.
+ * None of them allocates; bad sizes, NULL pointers and a short workspace are rejected before any launch. */
+#define GSB_BILAGRID_X 16
+#define GSB_BILAGRID_Y 16
+#define GSB_BILAGRID_L 8
+#define GSB_BILAGRID_COEFFS 12
+#define GSB_BILAGRID_FLOATS (GSB_BILAGRID_L * GSB_BILAGRID_Y * GSB_BILAGRID_X * GSB_BILAGRID_COEFFS)
+int gsb_bilagrid_slice_forward(int H, int W, const float *grid, const float *rgb, float *out, gsb_stream_t stream);
+size_t gsb_bilagrid_workspace_bytes(int H, int W);
+int gsb_bilagrid_slice_backward(int H, int W, const float *grid, const float *rgb, const float *v_out, float scale,
+                                float *v_rgb, float *v_grid, void *workspace, size_t workspace_bytes,
+                                gsb_stream_t stream);
+int gsb_bilagrid_tv(int num_grids, const float *grids, float weight, float *v_grids, float *tv_out,
+                    gsb_stream_t stream);
+
 /* ---- Scene export (Model::savePly model.cpp:505-558, Model::saveSplat :560-594; SURVEY.md 8f row 4) ----
  * Packs the file BODY on the device (the caller writes the text header and copies the rows D2H, typically on a
  * side stream into pinned memory).  features_dc / features_rest take a row stride in floats so both the reference's

@@ -27,6 +27,7 @@ SOURCES = {
     "ssim.cu": [],
     "densify.cu": [],
     "mcmc.cu": [],
+    "bilagrid.cu": [],
     "export.cu": ["--fmad=false"],
     "knn.cu": ["--fmad=false"],
     "image.cu": ["--fmad=false"],

@@ -97,6 +97,11 @@ _SIGS = {
     # n, logits, log_scales, raw_quats, key0, key1, step, noise_scale, means, stream
     "gsb_mcmc_add_noise": (_i, [_i, _vp, _vp, _vp, C.c_uint, C.c_uint, _i, _f, _vp, _vp]),
     "gsb_mcmc_draws": (_i, [_i, C.c_uint, C.c_uint, _i, _i, _vp, _vp, _vp]),
+    "gsb_bilagrid_slice_forward": (_i, [_i, _i, _vp, _vp, _vp, _vp]),
+    "gsb_bilagrid_workspace_bytes": (_sz, [_i, _i]),
+    # H, W, grid, rgb, v_out, scale, v_rgb, v_grid, workspace, workspace_bytes, stream
+    "gsb_bilagrid_slice_backward": (_i, [_i, _i, _vp, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
+    "gsb_bilagrid_tv": (_i, [_i, _vp, _f, _vp, _vp, _vp]),
     "gsb_ply_row_floats": (_i, [_i]),
     "gsb_pack_ply_rows": (_i, [_i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp]),
     "gsb_unpack_ply_rows": (_i, [_i, _i, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp]),
@@ -132,6 +137,10 @@ MCMC_MAX_SEGMENTS = 8   # GSB_MCMC_MAX_SEGMENTS
 class RowSegment(C.Structure):
     """gsb_row_segment (include/gsplat_b200.h)."""
     _fields_ = [("offset", C.c_longlong), ("row_floats", C.c_int), ("reserved", C.c_int)]
+
+
+BILAGRID_X, BILAGRID_Y, BILAGRID_L, BILAGRID_COEFFS = 16, 16, 8, 12   # GSB_BILAGRID_*
+BILAGRID_FLOATS = BILAGRID_L * BILAGRID_Y * BILAGRID_X * BILAGRID_COEFFS
 
 
 # optional symbols (experimental entry points) are bound when present

@@ -788,3 +788,61 @@ class ActivateGaussians(torch.autograd.Function):
                                                     capi.ptr(v_scales), capi.ptr(v_quats), capi.ptr(v_opac),
                                                     capi.ptr(v_ls), capi.ptr(v_rq), capi.ptr(v_ol), capi.stream()))
         return None, v_ls, v_rq, v_ol, None
+
+
+class BilateralGridSlice(torch.autograd.Function):
+    """One image's bilateral grid applied to an image (DESIGN D21; gsb_bilagrid_slice_forward / _backward):
+    (grid [12,L,Y,X] in F.grid_sample's order, rgb [H,W,3]) -> out [H,W,3] = A rgb + b with the coefficients
+    trilinearly interpolated at the pixel's position and luma, not clamped.  Both inputs get gradients."""
+
+    @staticmethod
+    def forward(ctx, grid, rgb):
+        shape = (capi.BILAGRID_COEFFS, capi.BILAGRID_L, capi.BILAGRID_Y, capi.BILAGRID_X)
+        if tuple(grid.shape) != shape or rgb.dim() != 3 or rgb.shape[2] != 3:
+            raise ValueError(f"grid must be {list(shape)} and rgb [H,W,3]")
+        H, W = rgb.shape[0], rgb.shape[1]
+        g = capi.f32(grid).permute(1, 2, 3, 0).contiguous()
+        r = capi.f32(rgb)
+        out = torch.empty_like(r)
+        capi.check(capi.lib().gsb_bilagrid_slice_forward(H, W, capi.ptr(g), capi.ptr(r), capi.ptr(out),
+                                                         capi.stream()))
+        ctx.save_for_backward(g, r)
+        return out
+
+    @staticmethod
+    def backward(ctx, v_out):
+        g, r = ctx.saved_tensors
+        H, W = r.shape[0], r.shape[1]
+        L = capi.lib()
+        ws = _ws.get(r.device, "bilagrid", L.gsb_bilagrid_workspace_bytes(H, W) + 256)
+        off = (-ws.data_ptr()) % 256
+        v_rgb = torch.empty_like(r)
+        v_grid = torch.zeros_like(g)
+        capi.check(L.gsb_bilagrid_slice_backward(H, W, capi.ptr(g), capi.ptr(r), capi.ptr(capi.f32(v_out)), 1.0,
+                                                 capi.ptr(v_rgb), capi.ptr(v_grid), ws.data_ptr() + off,
+                                                 ws.numel() - off, capi.stream()))
+        return v_grid.permute(3, 0, 1, 2), v_rgb
+
+
+class BilateralGridTV(torch.autograd.Function):
+    """The total variation of bilateral grids [N,12,L,Y,X] (DESIGN D21; gsb_bilagrid_tv): the sum over the axes X, Y
+    and L of the mean squared difference of neighbours along that axis, each mean over all N grids.  Returns the
+    scalar TV."""
+
+    @staticmethod
+    def forward(ctx, grids):
+        if grids.dim() != 5 or tuple(grids.shape[1:]) != (capi.BILAGRID_COEFFS, capi.BILAGRID_L, capi.BILAGRID_Y,
+                                                          capi.BILAGRID_X):
+            raise ValueError("grids must be [N,12,L,Y,X]")
+        g = capi.f32(grids).permute(0, 2, 3, 4, 1).contiguous()
+        v = torch.empty_like(g)
+        out = torch.empty((), dtype=torch.float32, device=g.device)
+        capi.check(capi.lib().gsb_bilagrid_tv(g.shape[0], capi.ptr(g), 1.0, capi.ptr(v), capi.ptr(out),
+                                              capi.stream()))
+        ctx.save_for_backward(v)
+        return out
+
+    @staticmethod
+    def backward(ctx, v_tv):
+        (v,) = ctx.saved_tensors
+        return v.permute(0, 4, 1, 2, 3) * v_tv

@@ -59,7 +59,13 @@ barriers are device-side).
 Under a Gaussian budget (`cfg=mcmc.MCMCConfig(...)`, DESIGN D20) the step takes no densification statistics; the
 regularisers' gradients are added after the views are averaged and exchanged, and after Adam mcmc.MCMCRefiner
 relocates and grows the set on a refinement step and adds the position noise.  Every draw is keyed by (seed, step,
-index), so replicas stay identical without a collective."""
+index), so replicas stay identical without a collective.
+
+With per-image appearance grids (`appearance=appearance.AppearanceConfig(num_images=...)`, DESIGN D21) every step
+names its views' training images (`step(cam, gt, step, image=i)`).  The step first writes the grids' TV gradient;
+each view's clamped render is sliced through its image's grid before the loss, and the slice backward turns the loss
+gradient into the render's gradient and adds 1/B of the grid gradient; after the Gaussians' Adam step one Adam step
+updates every grid.  evaluate(), render() and `image` stay the raw render."""
 import ctypes as C
 
 import torch
@@ -67,6 +73,7 @@ import torch
 from . import capi, ops
 from .densify import Densifier, RefineConfig
 from .export import SceneWriter
+from .appearance import Appearance, to_gsplat_order
 from .mcmc import MCMCConfig, MCMCRefiner
 from .model import (LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, Camera, camera_setup, downscale_factor,
                     means_learning_rate)
@@ -126,7 +133,8 @@ def view_setups(cams, gts, views, downscale):
 class SplatTrainer:
     def __init__(self, params, cfg=None, sh_degree=None, sh_degree_interval=1000, num_downscales=0,
                  resolution_schedule=3000, background=(0.6130, 0.0101, 0.3984), device="cuda:0", generator=None,
-                 ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1, antialiased=False):
+                 ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1, antialiased=False,
+                 appearance=None):
         """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
         featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
         cfg: densify.RefineConfig (the reference's refinement, the default) or mcmc.MCMCConfig (3DGS-MCMC under a
@@ -136,7 +144,9 @@ class SplatTrainer:
         constructs the trainer with the same parameters and calls step() with the same step numbers.
         views_per_step: B camera views per step (per rank under a group); step() then takes B cameras and B images.
         antialiased: train and render with the anti-aliased opacity (DESIGN D19), as model.GaussianModel(antialiased=
-        True): the projection kernels are the _aa ones, and nothing else in the step changes."""
+        True): the projection kernels are the _aa ones, and nothing else in the step changes.
+        appearance: an appearance.AppearanceConfig to learn one bilateral grid per training image (DESIGN D21); step()
+        then takes image=.  Not available with group=."""
         import torch.distributed as dist
         self.views_per_step = B = int(views_per_step)
         if B < 1:
@@ -144,6 +154,8 @@ class SplatTrainer:
         if group is None and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
             raise RuntimeError("SplatTrainer without a group runs in one process; pass group= to train data-parallel "
                                "over camera views")
+        if appearance is not None and group is not None:
+            raise ValueError("appearance grids are not available with group= (data-parallel training)")
         self.device = torch.device(device)
         self.cfg = cfg or RefineConfig()
         self.antialiased = bool(antialiased)
@@ -165,6 +177,7 @@ class SplatTrainer:
         pp.adam_v = torch.zeros_like(pp.param_flat)
         pp.background.copy_(torch.tensor(background, dtype=torch.float32))
         self.L = capi.lib()
+        self.appearance = None if appearance is None else Appearance(appearance, self.device)
         self.lr = dict(LEARNING_RATES)
         # the refinement strategy: the reference's Model::afterTrain (RefineConfig) or 3DGS-MCMC (MCMCConfig, D20)
         self.refiner = MCMCRefiner(self.cfg) if isinstance(self.cfg, MCMCConfig) else None
@@ -221,6 +234,11 @@ class SplatTrainer:
         self.pipe._alloc_pixels(W, H)
         self.render_maps = None
         self.ssim_ws = torch.empty(self.L.gsb_ssim_workspace_bytes(H, W) + 256, dtype=torch.uint8, device=self.device)
+        if self.appearance is not None:     # D21: the adjusted image, its loss gradient, the slice backward's workspace
+            self.adj_img = torch.empty((H, W, 3), dtype=torch.float32, device=self.device)
+            self.v_adj = torch.empty((H, W, 3), dtype=torch.float32, device=self.device)
+            self.bilagrid_ws = torch.empty(self.L.gsb_bilagrid_workspace_bytes(H, W) + 256, dtype=torch.uint8,
+                                           device=self.device)
 
     @property
     def n(self):
@@ -241,20 +259,33 @@ class SplatTrainer:
         pp = self.pipe
         return _split_coeffs(flat_views(pp.adam_m, pp.offs)), _split_coeffs(flat_views(pp.adam_v, pp.offs))
 
-    def step(self, cam, gt, step):
+    def appearance_grids(self):
+        """A copy of the appearance grids in F.grid_sample's order, [num_images, 12, L, Y, X] (D21)."""
+        if self.appearance is None:
+            raise ValueError("this trainer has no appearance grids")
+        return to_gsplat_order(self.appearance.grids)
+
+    def step(self, cam, gt, step, image=None):
         """One training step at `step` (1-based, as opensplat.cpp counts).  At views_per_step = 1: cam is one
         model.Camera, gt one [H,W,3] fp32 CUDA image at this step's render resolution, and the result is the device
         tensor {total, L1, SSIM}.  At B > 1: cam is a sequence of B cameras, gt B images (a sequence or a [B,H,W,3]
         tensor), and the result is the device [B,3] tensor of the views' {total, L1, SSIM}.  The next step overwrites
-        the result.  Raises ValueError on a wrong number of views, mixed resolutions or a wrong image."""
-        pp, B = self.pipe, self.views_per_step
+        the result.  image: with appearance grids, the training image of the view (an int) or of each of the B views
+        (a sequence of B ints); without them it must be None.  Raises ValueError on a wrong number of views, mixed
+        resolutions, a wrong image or a wrong image=."""
+        pp, B, ap = self.pipe, self.views_per_step, self.appearance
+        if ap is None and image is not None:
+            raise ValueError("image= needs a trainer constructed with appearance=")
+        images = ap.check_images(image, B) if ap is not None else [None] * B
         gts = [gt] if B == 1 else gt
         # ---- forward, enqueued without a host wait until each view's binning read-back ----
         setups, H, W, use = self._setup_views(cam, gts, B, step)
+        if ap is not None:
+            ap.tv()                         # D21: the grids' gradient starts as tv_weight * dTV
         visible = []
         for b in range(B):
             intr = setups[b][2]
-            self._render_view(b, intr, gts[b], self.losses[b])
+            self._render_view(b, intr, gts[b], self.losses[b], image=images[b])
             visible.append(pp.plan.visible > 0)
             # model.cpp:173-174: a lone view that hits nothing trains nothing.  Next to other views, or data-parallel
             # with more than one rank, its backward pass runs and writes zero gradients (no Gaussian has radii > 0):
@@ -273,6 +304,8 @@ class SplatTrainer:
             if self.refiner is not None:     # D20: the regularisers, on the averaged and exchanged gradients
                 self.refiner.regularize(pp)
             self._adam_step()
+            if ap is not None:
+                ap.adam_step(step)
         self.lr["means"] = means_learning_rate(step, self.cfg.max_steps, MEANS_LR_INIT)
         if trains and self.refiner is not None:
             # ---- D20: relocation and growth on a refinement step, then the position noise ----
@@ -370,15 +403,28 @@ class SplatTrainer:
         pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[b], out_img=out_img,
                       out_depth=out_depth, out_alpha=out_alpha)
 
-    def _render_view(self, b, intr, gt, loss):
+    def _render_view(self, b, intr, gt, loss, image=None):
         """View b's forward pass after _setup_views: _project_blend, then the loss against gt into `loss` ({total, L1,
-        SSIM}) and its image gradient into the pipeline's v_img."""
+        SSIM}) and its image gradient into the pipeline's v_img.  With a training image (D21) the loss is taken on
+        the render sliced through that image's grid, and the slice backward writes v_img and adds 1/B of the grid
+        gradient."""
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         H, W = pp.H, pp.W
         self._project_blend(b, intr)
         off = (-self.ssim_ws.data_ptr()) % 256
-        capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(loss),
+        if image is None:
+            capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(loss),
+                                          self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off, s))
+            return
+        ap = self.appearance
+        capi.check(L.gsb_bilagrid_slice_forward(H, W, P(ap.grids[image]), P(pp.out_img), P(self.adj_img), s))
+        capi.check(L.gsb_ssim_l1_loss(H, W, P(self.adj_img), P(gt), self.ssim_weight, P(self.v_adj), P(loss),
                                       self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off, s))
+        woff = (-self.bilagrid_ws.data_ptr()) % 256
+        capi.check(L.gsb_bilagrid_slice_backward(H, W, P(ap.grids[image]), P(pp.out_img), P(self.v_adj),
+                                                 1.0 / self.views_per_step, P(pp.v_img), P(ap.grad[image]),
+                                                 self.bilagrid_ws.data_ptr() + woff, self.bilagrid_ws.numel() - woff,
+                                                 s))
 
     def _backward_view(self, b, use, fx, fy):
         """View b's backward pass after its forward pass: rasterize-backward into colour slot b, then projection
