@@ -532,6 +532,42 @@ int gsb_bilagrid_slice_backward(int H, int W, const float *grid, const float *rg
 int gsb_bilagrid_tv(int num_grids, const float *grids, float weight, float *v_grids, float *tv_out,
                     gsb_stream_t stream);
 
+/* ---- Camera pose corrections (DESIGN D22; gsplat's pose optimisation) ----
+ * gsb_project_backward_activated_camgrad: gsb_project_backward_activated (accumulate = 0, antialiased = 0), _acc (1, 0),
+ *   _aa (0, 1) or _aa_acc (1, 1), with the same arguments (opacities = the logits when antialiased) and the same
+ *   per-Gaussian outputs bit for bit, that also writes the view's camera gradient: the exact VJP w.r.t. viewmat rows
+ *   0..2 and projmat rows 0, 1, 3, summed over the Gaussians with radii > 0, as one fp32 partial row of 24 floats
+ *   per block of 256 Gaussians (warp shuffle tree, then the 8 warps in order) into cam_partials
+ *   (gsb_project_camera_partials_floats(n) floats; n == 0 writes nothing).
+ * gsb_project_camera_grad_reduce: the sum of nblocks = ceil(n / 256) partial rows, in a fixed order in fp64, rounded
+ *   once into v_viewmat [4,4] and v_projmat [4,4] (row-major; row 3 of v_viewmat and row 2 of v_projmat written 0).
+ *   The same inputs give the same bits.
+ * A pose correction is GSB_POSE_FLOATS floats e = (t [3], d [6]); Rd = rot6d(d + (1,0,0,0,1,0)) has the rows b1, b2, b3
+ *   (b1 = a1/|a1|, b2 = normalize(a2 - (b1.a2) b1), b3 = b1 x b2), and the corrected camera-to-world is [R|T] Delta,
+ *   Delta = [[Rd, t], [0, 1]] (in the camera's own frame).
+ * gsb_pose_apply: view_out = Delta^-1 view [4,4], centre_out = centre + view[0:3,0:3]^T t [3], in fp64, rounded once;
+ *   e = 0 copies view and centre bit for bit.  The outputs must not overlap the inputs.
+ * gsb_pose_backward: grad [9] += scale * d/de of the loss whose gradients w.r.t. view_out and proj @ view_out are
+ *   v_viewmat and v_projmat (from gsb_project_camera_grad_reduce): G = v_viewmat + proj^T v_projmat, d/dDelta^-1 =
+ *   G view^T, chained through Delta^-1 and rot6d in fp64; the added value is rounded once.
+ * One thread each; none of them allocates; NULL pointers are rejected before any launch. */
+#define GSB_POSE_FLOATS 9
+size_t gsb_project_camera_partials_floats(int n);
+int gsb_project_backward_activated_camgrad(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                           const float *raw_quats, const float *opacities, const float *viewmat,
+                                           const float *projmat, float fx, float fy, int img_h, int img_w,
+                                           const int32_t *radii, const float *conics, const float *v_xy,
+                                           const float *v_depth, const float *v_conic, const float *v_opacity,
+                                           float *v_mean3d, float *v_log_scales, float *v_raw_quats,
+                                           float *v_opacity_logits, int accumulate, int antialiased,
+                                           float *cam_partials, gsb_stream_t stream);
+int gsb_project_camera_grad_reduce(int nblocks, const float *partials, float *v_viewmat, float *v_projmat,
+                                   gsb_stream_t stream);
+int gsb_pose_apply(const float *pose, const float *view, const float *centre, float *view_out, float *centre_out,
+                   gsb_stream_t stream);
+int gsb_pose_backward(const float *pose, const float *view, const float *proj, const float *v_viewmat,
+                      const float *v_projmat, float scale, float *grad, gsb_stream_t stream);
+
 /* ---- Scene export (Model::savePly model.cpp:505-558, Model::saveSplat :560-594; SURVEY.md 8f row 4) ----
  * Packs the file BODY on the device (the caller writes the text header and copies the rows D2H, typically on a
  * side stream into pinned memory).  features_dc / features_rest take a row stride in floats so both the reference's

@@ -86,24 +86,6 @@ class Appearance:
         self.exp_avg_sq = torch.zeros_like(self.grids)
         self.adam_t = 0
 
-    def check_images(self, image, views):
-        """The step's image indices as a list of `views` ints; raises ValueError unless image= names `views` images
-        in range."""
-        if image is None:
-            raise ValueError("a step with appearance grids needs image= (the training image of each view)")
-        if isinstance(image, (list, tuple)):
-            idx = list(image)
-        elif views == 1:
-            idx = [image]
-        else:
-            raise ValueError(f"image= must be a sequence of {views} training images")
-        if len(idx) != views:
-            raise ValueError(f"image= must name {views} training images, got {len(idx)}")
-        for i in idx:
-            if isinstance(i, bool) or not isinstance(i, int) or not 0 <= i < self.cfg.num_images:
-                raise ValueError(f"image indices must be ints in [0, {self.cfg.num_images}), got {i!r}")
-        return idx
-
     def tv(self):
         """Writes tv_weight * dTV into the gradient buffer: the step's first write of it."""
         capi.check(capi.lib().gsb_bilagrid_tv(self.cfg.num_images, capi.ptr(self.grids), float(self.cfg.tv_weight),

@@ -28,6 +28,7 @@ SOURCES = {
     "densify.cu": [],
     "mcmc.cu": [],
     "bilagrid.cu": [],
+    "pose.cu": [],
     "export.cu": ["--fmad=false"],
     "knn.cu": ["--fmad=false"],
     "image.cu": ["--fmad=false"],

@@ -102,6 +102,17 @@ _SIGS = {
     # H, W, grid, rgb, v_out, scale, v_rgb, v_grid, workspace, workspace_bytes, stream
     "gsb_bilagrid_slice_backward": (_i, [_i, _i, _vp, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
     "gsb_bilagrid_tv": (_i, [_i, _vp, _f, _vp, _vp, _vp]),
+    "gsb_project_camera_partials_floats": (_sz, [_i]),
+    # the arguments of gsb_project_backward_activated, then accumulate, antialiased, cam_partials, stream
+    "gsb_project_backward_activated_camgrad": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
+                                                    _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp,
+                                                    _vp]),
+    # nblocks, partials, v_viewmat, v_projmat, stream
+    "gsb_project_camera_grad_reduce": (_i, [_i, _vp, _vp, _vp, _vp]),
+    # pose, view, centre, view_out, centre_out, stream
+    "gsb_pose_apply": (_i, [_vp, _vp, _vp, _vp, _vp, _vp]),
+    # pose, view, proj, v_viewmat, v_projmat, scale, grad, stream
+    "gsb_pose_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
     "gsb_ply_row_floats": (_i, [_i]),
     "gsb_pack_ply_rows": (_i, [_i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp]),
     "gsb_unpack_ply_rows": (_i, [_i, _i, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp]),
@@ -141,6 +152,8 @@ class RowSegment(C.Structure):
 
 BILAGRID_X, BILAGRID_Y, BILAGRID_L, BILAGRID_COEFFS = 16, 16, 8, 12   # GSB_BILAGRID_*
 BILAGRID_FLOATS = BILAGRID_L * BILAGRID_Y * BILAGRID_X * BILAGRID_COEFFS
+POSE_FLOATS = 9   # GSB_POSE_FLOATS
+CAMGRAD_TERMS = 24   # floats per block row of gsb_project_backward_activated_camgrad's partials
 
 
 # optional symbols (experimental entry points) are bound when present

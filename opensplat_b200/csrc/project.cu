@@ -20,6 +20,30 @@
 namespace {
 
 constexpr int PJ_THREADS = 256;
+// D22: the camera gradient of one view, per Gaussian: d/dviewmat rows 0..2 (12 floats), then d/dprojmat rows 0, 1
+// and 3 (12 floats); row 3 of the viewmat and row 2 of the projmat are not read by the projection
+constexpr int CG_TERMS = 24;
+
+// The block's sum of each of the CG_TERMS terms, in a fixed tree: a shuffle tree within each warp, then the 8 warp
+// sums added in warp order; one fp32 row per block.  Every thread of the block must call it.
+__device__ __forceinline__ void camgrad_block_sum(const float (&cg)[CG_TERMS], float *__restrict__ out) {
+    __shared__ float red[PJ_THREADS / 32][CG_TERMS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < CG_TERMS; ++k) {
+        float v = cg[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v = v + __shfl_down_sync(0xffffffffu, v, o);
+        if (lane == 0) red[warp][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < CG_TERMS) {
+        float v = red[0][threadIdx.x];
+#pragma unroll
+        for (int w = 1; w < PJ_THREADS / 32; ++w) v = v + red[w][threadIdx.x];
+        out[threadIdx.x] = v;
+    }
+}
 
 struct Cam {
     float V[12];  // viewmat rows 0..2
@@ -186,7 +210,9 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
 // AA: VJP of the anti-aliased forward (D19).  `opacities` holds the opacity LOGITS (o and comp are recomputed with the
 // forward's expressions, bit for bit); v_logit = v_opacity * comp * o (1 - o), and where comp > 0 the cotangent
 // v_opacity * o of comp is taken to the blurred covariance and added to vS before the T / J / clamp chain.
-template <bool ACT, bool ACC, bool AA = false>
+// CAMGRAD (with ACT; DESIGN D22): also the exact VJP w.r.t. viewmat and projmat, summed over the block's Gaussians
+// (camgrad_block_sum) into row blockIdx.x of cam_partials; every other output is the one without CAMGRAD, bit for bit.
+template <bool ACT, bool ACC, bool AA = false, bool CAMGRAD = false>
 __global__ void __launch_bounds__(PJ_THREADS)
 project_backward_kernel(int n, const float *__restrict__ means3d, const float *__restrict__ scales,
                         float glob_scale, const float *__restrict__ quats,
@@ -197,191 +223,242 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
                         const float *__restrict__ v_conic, float *__restrict__ v_mean3d,
                         float *__restrict__ v_scale, float4 *__restrict__ v_quat,
                         const float *__restrict__ opacities, const float *__restrict__ v_opacity,
-                        float *__restrict__ v_opacity_logits) {
+                        float *__restrict__ v_opacity_logits, float *__restrict__ cam_partials = nullptr) {
     static_assert(ACT || !AA, "the anti-aliased opacity needs the activated projection");
+    static_assert(ACT || !CAMGRAD, "the camera gradient is taken with the activated projection");
     const int i = blockIdx.x * PJ_THREADS + threadIdx.x;
-    if (i >= n) return;
-    float comp = 0.f;
-    if (ACT && !AA) {
-        const float o = opacities[i];
-        if constexpr (ACC)
-            v_opacity_logits[i] = v_opacity_logits[i] + (v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f);
-        else
-            v_opacity_logits[i] = v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f;
-    }
-    float vm[3] = {0.f, 0.f, 0.f}, vs[3] = {0.f, 0.f, 0.f};
-    float4 vq = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (radii[i] > 0) {
-        Cam cam;
-        load_cam(viewmat, projmat, cam);
-        const float *V = cam.V, *P = cam.P;
-        const float px = means3d[3 * i], py = means3d[3 * i + 1], pz = means3d[3 * i + 2];
-
-        // pixel centre: xy = 0.5*W*(h.x*rw) + cx - 0.5, rw = 1/(h.w + 1e-6)
-        const float hx = P[0] * px + P[1] * py + P[2] * pz + P[3];
-        const float hy = P[4] * px + P[5] * py + P[6] * pz + P[7];
-        const float hw = P[12] * px + P[13] * py + P[14] * pz + P[15];
-        const float rw = 1.f / (hw + 1e-6f);
-        const float2 vxy = v_xy[i];
-        const float vndcx = 0.5f * (float)img_w * vxy.x, vndcy = 0.5f * (float)img_h * vxy.y;
-        const float vhx = vndcx * rw, vhy = vndcy * rw;
-        const float vhw = -(vndcx * hx + vndcy * hy) * rw * rw;
-        vm[0] = P[0] * vhx + P[4] * vhy + P[12] * vhw;
-        vm[1] = P[1] * vhx + P[5] * vhy + P[13] * vhw;
-        vm[2] = P[2] * vhx + P[6] * vhy + P[14] * vhw;
-
-        const float tx = V[0] * px + V[1] * py + V[2] * pz + V[3];
-        const float ty = V[4] * px + V[5] * py + V[6] * pz + V[7];
-        const float tz = V[8] * px + V[9] * py + V[10] * pz + V[11];
-        float vtx = 0.f, vty = 0.f, vtz = v_depth ? v_depth[i] : 0.f;
-
-        // conic = inverse(cov2d):  v_Sigma = -X G X,  G = [[vA, vB/2],[vB/2, vC]]
-        const float A = conics[3 * i], B = conics[3 * i + 1], Cc = conics[3 * i + 2];
-        const float gA = v_conic[3 * i], gB = 0.5f * v_conic[3 * i + 1], gC = v_conic[3 * i + 2];
-        const float xg00 = A * gA + B * gB, xg01 = A * gB + B * gC;
-        const float xg10 = B * gA + Cc * gB, xg11 = B * gB + Cc * gC;
-        float vS00 = -(xg00 * A + xg01 * B);
-        float vS01 = -(xg00 * B + xg01 * Cc);
-        float vS11 = -(xg10 * B + xg11 * Cc);
-
-        // recompute forward intermediates
-        const float4 q = reinterpret_cast<const float4 *>(quats)[i];
-        float R[3][3], M[3][3];
-        quat_to_rotmat(q.x, q.y, q.z, q.w, R);
-        const float a[3] = {scales[3 * i], scales[3 * i + 1], scales[3 * i + 2]};
-        const float e[3] = {ACT ? expf(a[0]) : a[0], ACT ? expf(a[1]) : a[1], ACT ? expf(a[2]) : a[2]};
-        const float s[3] = {glob_scale * e[0], glob_scale * e[1], glob_scale * e[2]};
+    // CAMGRAD: every thread of the block takes part in the reduction, so none returns early
+    if (!CAMGRAD && i >= n) return;
+    float cg[CG_TERMS];    // CAMGRAD: this Gaussian's camera-gradient terms (0 past n and where radii == 0)
 #pragma unroll
-        for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int c = 0; c < 3; ++c) M[r][c] = R[r][c] * s[c];
-        float Cs[3][3];
-#pragma unroll
-        for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-                Cs[r][c] = M[r][0] * M[c][0] + M[r][1] * M[c][1] + M[r][2] * M[c][2];
-        const float lim_x = 1.3f * tan_fovx, lim_y = 1.3f * tan_fovy;
-        const float qx = tx / tz, qy = ty / tz;
-        const bool clamp_x = !(qx > -lim_x && qx < lim_x), clamp_y = !(qy > -lim_y && qy < lim_y);
-        const float cqx = fminf(lim_x, fmaxf(-lim_x, qx)), cqy = fminf(lim_y, fmaxf(-lim_y, qy));
-        const float ttx = tz * cqx, tty = tz * cqy;
-        const float rz = 1.f / tz, rz2 = rz * rz, rz3 = rz2 * rz;
-        const float J00 = fx * rz, J02 = -fx * ttx * rz2, J11 = fy * rz, J12 = -fy * tty * rz2;
-        float T[2][3];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            T[0][c] = J00 * V[c] + J02 * V[8 + c];
-            T[1][c] = J11 * V[4 + c] + J12 * V[8 + c];
+    for (int k = 0; k < CG_TERMS; ++k) cg[k] = 0.f;
+    if (!CAMGRAD || i < n) {
+        float comp = 0.f;
+        if (ACT && !AA) {
+            const float o = opacities[i];
+            if constexpr (ACC)
+                v_opacity_logits[i] = v_opacity_logits[i] + (v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f);
+            else
+                v_opacity_logits[i] = v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f;
         }
-        if constexpr (AA) {
-            // the forward's cov2d sums and det, recomputed in its order
-            float TV[2][3];
+        float vm[3] = {0.f, 0.f, 0.f}, vs[3] = {0.f, 0.f, 0.f};
+        float4 vq = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (radii[i] > 0) {
+            Cam cam;
+            load_cam(viewmat, projmat, cam);
+            const float *V = cam.V, *P = cam.P;
+            const float px = means3d[3 * i], py = means3d[3 * i + 1], pz = means3d[3 * i + 2];
+
+            // pixel centre: xy = 0.5*W*(h.x*rw) + cx - 0.5, rw = 1/(h.w + 1e-6)
+            const float hx = P[0] * px + P[1] * py + P[2] * pz + P[3];
+            const float hy = P[4] * px + P[5] * py + P[6] * pz + P[7];
+            const float hw = P[12] * px + P[13] * py + P[14] * pz + P[15];
+            const float rw = 1.f / (hw + 1e-6f);
+            const float2 vxy = v_xy[i];
+            const float vndcx = 0.5f * (float)img_w * vxy.x, vndcy = 0.5f * (float)img_h * vxy.y;
+            const float vhx = vndcx * rw, vhy = vndcy * rw;
+            const float vhw = -(vndcx * hx + vndcy * hy) * rw * rw;
+            vm[0] = P[0] * vhx + P[4] * vhy + P[12] * vhw;
+            vm[1] = P[1] * vhx + P[5] * vhy + P[13] * vhw;
+            vm[2] = P[2] * vhx + P[6] * vhy + P[14] * vhw;
+
+            const float tx = V[0] * px + V[1] * py + V[2] * pz + V[3];
+            const float ty = V[4] * px + V[5] * py + V[6] * pz + V[7];
+            const float tz = V[8] * px + V[9] * py + V[10] * pz + V[11];
+            float vtx = 0.f, vty = 0.f, vtz = v_depth ? v_depth[i] : 0.f;
+
+            // conic = inverse(cov2d):  v_Sigma = -X G X,  G = [[vA, vB/2],[vB/2, vC]]
+            const float A = conics[3 * i], B = conics[3 * i + 1], Cc = conics[3 * i + 2];
+            const float gA = v_conic[3 * i], gB = 0.5f * v_conic[3 * i + 1], gC = v_conic[3 * i + 2];
+            const float xg00 = A * gA + B * gB, xg01 = A * gB + B * gC;
+            const float xg10 = B * gA + Cc * gB, xg11 = B * gB + Cc * gC;
+            float vS00 = -(xg00 * A + xg01 * B);
+            float vS01 = -(xg00 * B + xg01 * Cc);
+            float vS11 = -(xg10 * B + xg11 * Cc);
+
+            // recompute forward intermediates
+            const float4 q = reinterpret_cast<const float4 *>(quats)[i];
+            float R[3][3], M[3][3];
+            quat_to_rotmat(q.x, q.y, q.z, q.w, R);
+            const float a[3] = {scales[3 * i], scales[3 * i + 1], scales[3 * i + 2]};
+            const float e[3] = {ACT ? expf(a[0]) : a[0], ACT ? expf(a[1]) : a[1], ACT ? expf(a[2]) : a[2]};
+            const float s[3] = {glob_scale * e[0], glob_scale * e[1], glob_scale * e[2]};
+#pragma unroll
+            for (int r = 0; r < 3; ++r)
+#pragma unroll
+                for (int c = 0; c < 3; ++c) M[r][c] = R[r][c] * s[c];
+            float Cs[3][3];
+#pragma unroll
+            for (int r = 0; r < 3; ++r)
+#pragma unroll
+                for (int c = 0; c < 3; ++c)
+                    Cs[r][c] = M[r][0] * M[c][0] + M[r][1] * M[c][1] + M[r][2] * M[c][2];
+            const float lim_x = 1.3f * tan_fovx, lim_y = 1.3f * tan_fovy;
+            const float qx = tx / tz, qy = ty / tz;
+            const bool clamp_x = !(qx > -lim_x && qx < lim_x), clamp_y = !(qy > -lim_y && qy < lim_y);
+            const float cqx = fminf(lim_x, fmaxf(-lim_x, qx)), cqy = fminf(lim_y, fmaxf(-lim_y, qy));
+            const float ttx = tz * cqx, tty = tz * cqy;
+            const float rz = 1.f / tz, rz2 = rz * rz, rz3 = rz2 * rz;
+            const float J00 = fx * rz, J02 = -fx * ttx * rz2, J11 = fy * rz, J12 = -fy * tty * rz2;
+            float T[2][3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                T[0][c] = J00 * V[c] + J02 * V[8 + c];
+                T[1][c] = J11 * V[4 + c] + J12 * V[8 + c];
+            }
+            if constexpr (AA) {
+                // the forward's cov2d sums and det, recomputed in its order
+                float TV[2][3];
+#pragma unroll
+                for (int r = 0; r < 2; ++r)
+#pragma unroll
+                    for (int c = 0; c < 3; ++c)
+                        TV[r][c] = T[r][0] * Cs[0][c] + T[r][1] * Cs[1][c] + T[r][2] * Cs[2][c];
+                const float cxx0 = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2];
+                const float cxy = TV[0][0] * T[1][0] + TV[0][1] * T[1][1] + TV[0][2] * T[1][2];
+                const float cyy0 = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2];
+                const float det = (cxx0 + 0.3f) * (cyy0 + 0.3f) - cxy * cxy;
+                comp = sqrtf(fmaxf(0.f, (cxx0 * cyy0 - cxy * cxy) / det));
+                if (v_opacity && comp > 0.f) {
+                    // d comp^2 / d Sigma = ((1 - comp^2) Sigma^-1 - 0.3 det(Sigma^-1) I), per symmetric entry, written as
+                    // 0.3 / det^2 [[cyy0^2 + cxy^2 + 0.3 cyy0, -cxy (cxx0 + cyy0 + 0.3)], [.., cxx0^2 + cxy^2 + 0.3 cxx0]]:
+                    // the same value without the cancellation of the first form when Sigma0 is small against 0.3 I
+                    const float o = 1.f / (1.f + expf(-opacities[i]));
+                    const float k = 0.5f * (v_opacity[i] * o) / comp;
+                    const float id = 1.f / det;
+                    const float a = cyy0 * id, b = cxy * id, c = cxx0 * id, e = 0.3f * id;
+                    vS00 = vS00 + k * (0.3f * (a * a + b * b + e * a));
+                    vS01 = vS01 - k * (0.3f * (b * (a + c + e)));
+                    vS11 = vS11 + k * (0.3f * (c * c + b * b + e * c));
+                }
+            }
+            float vST[2][3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                vST[0][c] = vS00 * T[0][c] + vS01 * T[1][c];
+                vST[1][c] = vS01 * T[0][c] + vS11 * T[1][c];
+            }
+            float vV[3][3];
+#pragma unroll
+            for (int r = 0; r < 3; ++r)
+#pragma unroll
+                for (int c = 0; c < 3; ++c) vV[r][c] = T[0][r] * vST[0][c] + T[1][r] * vST[1][c];
+            float vT[2][3];
 #pragma unroll
             for (int r = 0; r < 2; ++r)
 #pragma unroll
                 for (int c = 0; c < 3; ++c)
-                    TV[r][c] = T[r][0] * Cs[0][c] + T[r][1] * Cs[1][c] + T[r][2] * Cs[2][c];
-            const float cxx0 = TV[0][0] * T[0][0] + TV[0][1] * T[0][1] + TV[0][2] * T[0][2];
-            const float cxy = TV[0][0] * T[1][0] + TV[0][1] * T[1][1] + TV[0][2] * T[1][2];
-            const float cyy0 = TV[1][0] * T[1][0] + TV[1][1] * T[1][1] + TV[1][2] * T[1][2];
-            const float det = (cxx0 + 0.3f) * (cyy0 + 0.3f) - cxy * cxy;
-            comp = sqrtf(fmaxf(0.f, (cxx0 * cyy0 - cxy * cxy) / det));
-            if (v_opacity && comp > 0.f) {
-                // d comp^2 / d Sigma = ((1 - comp^2) Sigma^-1 - 0.3 det(Sigma^-1) I), per symmetric entry, written as
-                // 0.3 / det^2 [[cyy0^2 + cxy^2 + 0.3 cyy0, -cxy (cxx0 + cyy0 + 0.3)], [.., cxx0^2 + cxy^2 + 0.3 cxx0]]:
-                // the same value without the cancellation of the first form when Sigma0 is small against 0.3 I
-                const float o = 1.f / (1.f + expf(-opacities[i]));
-                const float k = 0.5f * (v_opacity[i] * o) / comp;
-                const float id = 1.f / det;
-                const float a = cyy0 * id, b = cxy * id, c = cxx0 * id, e = 0.3f * id;
-                vS00 = vS00 + k * (0.3f * (a * a + b * b + e * a));
-                vS01 = vS01 - k * (0.3f * (b * (a + c + e)));
-                vS11 = vS11 + k * (0.3f * (c * c + b * b + e * c));
+                    vT[r][c] = 2.f * (vST[r][0] * Cs[0][c] + vST[r][1] * Cs[1][c] + vST[r][2] * Cs[2][c]);
+            const float vJ00 = vT[0][0] * V[0] + vT[0][1] * V[1] + vT[0][2] * V[2];
+            const float vJ02 = vT[0][0] * V[8] + vT[0][1] * V[9] + vT[0][2] * V[10];
+            const float vJ11 = vT[1][0] * V[4] + vT[1][1] * V[5] + vT[1][2] * V[6];
+            const float vJ12 = vT[1][0] * V[8] + vT[1][1] * V[9] + vT[1][2] * V[10];
+            const float vttx = -fx * rz2 * vJ02, vtty = -fy * rz2 * vJ12;
+            vtz += -fx * rz2 * vJ00 + 2.f * fx * ttx * rz3 * vJ02 - fy * rz2 * vJ11 +
+                   2.f * fy * tty * rz3 * vJ12;
+            // D16: exactly on +-lim the reference's min(lim, max(-lim, q)) splits the gradient in half between the
+            // branches: half to t.x, and 0.5 cq to t.z
+            if (qx == lim_x || qx == -lim_x) { const float h = 0.5f * vttx; vtx += h; vtz += cqx * h; }
+            else if (clamp_x) vtz += cqx * vttx; else vtx += vttx;
+            if (qy == lim_y || qy == -lim_y) { const float h = 0.5f * vtty; vty += h; vtz += cqy * h; }
+            else if (clamp_y) vtz += cqy * vtty; else vty += vtty;
+            vm[0] += V[0] * vtx + V[4] * vty + V[8] * vtz;
+            vm[1] += V[1] * vtx + V[5] * vty + V[9] * vtz;
+            vm[2] += V[2] * vtx + V[6] * vty + V[10] * vtz;
+            if constexpr (CAMGRAD) {
+                // D22: t = V[0:3,:] (p, 1) gives vt_r (p, 1) to row r of V, T = J V[0:3,0:3] gives J^T vT to columns
+                // 0..2; (hx, hy, hw) = P rows 0, 1, 3 times (p, 1) give vh (p, 1)
+                const float pc[3] = {px, py, pz}, vt[3] = {vtx, vty, vtz}, vh[3] = {vhx, vhy, vhw};
+#pragma unroll
+                for (int r = 0; r < 3; ++r) {
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) {
+                        cg[4 * r + c] = vt[r] * pc[c];
+                        cg[12 + 4 * r + c] = vh[r] * pc[c];
+                    }
+                    cg[4 * r + 3] = vt[r];
+                    cg[12 + 4 * r + 3] = vh[r];
+                }
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    cg[c] = cg[c] + J00 * vT[0][c];
+                    cg[4 + c] = cg[4 + c] + J11 * vT[1][c];
+                    cg[8 + c] = cg[8 + c] + (J02 * vT[0][c] + J12 * vT[1][c]);
+                }
             }
-        }
-        float vST[2][3];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            vST[0][c] = vS00 * T[0][c] + vS01 * T[1][c];
-            vST[1][c] = vS01 * T[0][c] + vS11 * T[1][c];
-        }
-        float vV[3][3];
-#pragma unroll
-        for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int c = 0; c < 3; ++c) vV[r][c] = T[0][r] * vST[0][c] + T[1][r] * vST[1][c];
-        float vT[2][3];
-#pragma unroll
-        for (int r = 0; r < 2; ++r)
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-                vT[r][c] = 2.f * (vST[r][0] * Cs[0][c] + vST[r][1] * Cs[1][c] + vST[r][2] * Cs[2][c]);
-        const float vJ00 = vT[0][0] * V[0] + vT[0][1] * V[1] + vT[0][2] * V[2];
-        const float vJ02 = vT[0][0] * V[8] + vT[0][1] * V[9] + vT[0][2] * V[10];
-        const float vJ11 = vT[1][0] * V[4] + vT[1][1] * V[5] + vT[1][2] * V[6];
-        const float vJ12 = vT[1][0] * V[8] + vT[1][1] * V[9] + vT[1][2] * V[10];
-        const float vttx = -fx * rz2 * vJ02, vtty = -fy * rz2 * vJ12;
-        vtz += -fx * rz2 * vJ00 + 2.f * fx * ttx * rz3 * vJ02 - fy * rz2 * vJ11 +
-               2.f * fy * tty * rz3 * vJ12;
-        // D16: exactly on +-lim the reference's min(lim, max(-lim, q)) splits the gradient in half between the
-        // branches: half to t.x, and 0.5 cq to t.z
-        if (qx == lim_x || qx == -lim_x) { const float h = 0.5f * vttx; vtx += h; vtz += cqx * h; }
-        else if (clamp_x) vtz += cqx * vttx; else vtx += vttx;
-        if (qy == lim_y || qy == -lim_y) { const float h = 0.5f * vtty; vty += h; vtz += cqy * h; }
-        else if (clamp_y) vtz += cqy * vtty; else vty += vtty;
-        vm[0] += V[0] * vtx + V[4] * vty + V[8] * vtz;
-        vm[1] += V[1] * vtx + V[5] * vty + V[9] * vtz;
-        vm[2] += V[2] * vtx + V[6] * vty + V[10] * vtz;
 
-        // cov3d = M M^T, M = R S
-        float vM[3][3];
+            // cov3d = M M^T, M = R S
+            float vM[3][3];
 #pragma unroll
-        for (int r = 0; r < 3; ++r)
+            for (int r = 0; r < 3; ++r)
 #pragma unroll
-            for (int c = 0; c < 3; ++c)
-                vM[r][c] = 2.f * (vV[r][0] * M[0][c] + vV[r][1] * M[1][c] + vV[r][2] * M[2][c]);
+                for (int c = 0; c < 3; ++c)
+                    vM[r][c] = 2.f * (vV[r][0] * M[0][c] + vV[r][1] * M[1][c] + vV[r][2] * M[2][c]);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            vs[c] = glob_scale * (R[0][c] * vM[0][c] + R[1][c] * vM[1][c] + R[2][c] * vM[2][c]);
-            if (ACT) vs[c] = vs[c] * e[c];   // d exp(a) = exp(a)
+            for (int c = 0; c < 3; ++c) {
+                vs[c] = glob_scale * (R[0][c] * vM[0][c] + R[1][c] * vM[1][c] + R[2][c] * vM[2][c]);
+                if (ACT) vs[c] = vs[c] * e[c];   // d exp(a) = exp(a)
+            }
+            float vR[3][3];
+#pragma unroll
+            for (int r = 0; r < 3; ++r)
+#pragma unroll
+                for (int c = 0; c < 3; ++c) vR[r][c] = vM[r][c] * s[c];
+            const float nq = sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
+            const float inv = 1.0f / nq;
+            const float w = q.x * inv, x = q.y * inv, y = q.z * inv, z = q.w * inv;
+            const float gw = 2.f * (x * (vR[2][1] - vR[1][2]) + y * (vR[0][2] - vR[2][0]) + z * (vR[1][0] - vR[0][1]));
+            const float gx = 2.f * (-2.f * x * (vR[1][1] + vR[2][2]) + y * (vR[1][0] + vR[0][1]) +
+                                    z * (vR[2][0] + vR[0][2]) + w * (vR[2][1] - vR[1][2]));
+            const float gy = 2.f * (x * (vR[1][0] + vR[0][1]) - 2.f * y * (vR[0][0] + vR[2][2]) +
+                                    z * (vR[2][1] + vR[1][2]) + w * (vR[0][2] - vR[2][0]));
+            const float gz = 2.f * (x * (vR[2][0] + vR[0][2]) + y * (vR[2][1] + vR[1][2]) -
+                                    2.f * z * (vR[0][0] + vR[1][1]) + w * (vR[1][0] - vR[0][1]));
+            const float dot = w * gw + x * gx + y * gy + z * gz;
+            vq = make_float4((gw - w * dot) * inv, (gx - x * dot) * inv, (gy - y * dot) * inv,
+                             (gz - z * dot) * inv);
         }
-        float vR[3][3];
-#pragma unroll
-        for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int c = 0; c < 3; ++c) vR[r][c] = vM[r][c] * s[c];
-        const float nq = sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
-        const float inv = 1.0f / nq;
-        const float w = q.x * inv, x = q.y * inv, y = q.z * inv, z = q.w * inv;
-        const float gw = 2.f * (x * (vR[2][1] - vR[1][2]) + y * (vR[0][2] - vR[2][0]) + z * (vR[1][0] - vR[0][1]));
-        const float gx = 2.f * (-2.f * x * (vR[1][1] + vR[2][2]) + y * (vR[1][0] + vR[0][1]) +
-                                z * (vR[2][0] + vR[0][2]) + w * (vR[2][1] - vR[1][2]));
-        const float gy = 2.f * (x * (vR[1][0] + vR[0][1]) - 2.f * y * (vR[0][0] + vR[2][2]) +
-                                z * (vR[2][1] + vR[1][2]) + w * (vR[0][2] - vR[2][0]));
-        const float gz = 2.f * (x * (vR[2][0] + vR[0][2]) + y * (vR[2][1] + vR[1][2]) -
-                                2.f * z * (vR[0][0] + vR[1][1]) + w * (vR[1][0] - vR[0][1]));
-        const float dot = w * gw + x * gx + y * gy + z * gz;
-        vq = make_float4((gw - w * dot) * inv, (gx - x * dot) * inv, (gy - y * dot) * inv,
-                         (gz - z * dot) * inv);
-    }
-    if constexpr (AA) {
-        float vol = 0.f;
-        if (v_opacity) {
-            const float o = 1.f / (1.f + expf(-opacities[i]));
-            vol = v_opacity[i] * comp * o * (1.f - o);
+        if constexpr (AA) {
+            float vol = 0.f;
+            if (v_opacity) {
+                const float o = 1.f / (1.f + expf(-opacities[i]));
+                vol = v_opacity[i] * comp * o * (1.f - o);
+            }
+            v_opacity_logits[i] = ACC ? v_opacity_logits[i] + vol : vol;
         }
-        v_opacity_logits[i] = ACC ? v_opacity_logits[i] + vol : vol;
+        if constexpr (ACC) {
+            const float4 pq = v_quat[i];
+            v_mean3d[3 * i] += vm[0]; v_mean3d[3 * i + 1] += vm[1]; v_mean3d[3 * i + 2] += vm[2];
+            v_scale[3 * i] += vs[0]; v_scale[3 * i + 1] += vs[1]; v_scale[3 * i + 2] += vs[2];
+            v_quat[i] = make_float4(pq.x + vq.x, pq.y + vq.y, pq.z + vq.z, pq.w + vq.w);
+        } else {
+            v_mean3d[3 * i] = vm[0]; v_mean3d[3 * i + 1] = vm[1]; v_mean3d[3 * i + 2] = vm[2];
+            v_scale[3 * i] = vs[0]; v_scale[3 * i + 1] = vs[1]; v_scale[3 * i + 2] = vs[2];
+            v_quat[i] = vq;
+        }
     }
-    if constexpr (ACC) {
-        const float4 pq = v_quat[i];
-        v_mean3d[3 * i] += vm[0]; v_mean3d[3 * i + 1] += vm[1]; v_mean3d[3 * i + 2] += vm[2];
-        v_scale[3 * i] += vs[0]; v_scale[3 * i + 1] += vs[1]; v_scale[3 * i + 2] += vs[2];
-        v_quat[i] = make_float4(pq.x + vq.x, pq.y + vq.y, pq.z + vq.z, pq.w + vq.w);
-    } else {
-        v_mean3d[3 * i] = vm[0]; v_mean3d[3 * i + 1] = vm[1]; v_mean3d[3 * i + 2] = vm[2];
-        v_scale[3 * i] = vs[0]; v_scale[3 * i + 1] = vs[1]; v_scale[3 * i + 2] = vs[2];
-        v_quat[i] = vq;
+    if constexpr (CAMGRAD) camgrad_block_sum(cg, cam_partials + CG_TERMS * (size_t)blockIdx.x);
+}
+
+// D22: the sum over the blocks' partial rows, one warp per term: lane l adds blocks l, l + 32, ... in fp64 in that
+// order, then a fixed shuffle tree; rounded once into v_viewmat rows 0..2 and v_projmat rows 0, 1, 3 (the rows the
+// projection reads), the other two rows written 0.
+__global__ void __launch_bounds__(CG_TERMS * 32)
+camgrad_reduce_kernel(int nblocks, const float *__restrict__ partials, float *__restrict__ v_viewmat,
+                      float *__restrict__ v_projmat) {
+    const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double s = 0.0;
+    for (int b = lane; b < nblocks; b += 32) s += (double)partials[CG_TERMS * (size_t)b + k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+    if (lane == 0) {
+        const float r = (float)s;
+        if (k < 12) v_viewmat[k] = r;
+        else v_projmat[k < 20 ? k - 12 : k - 8] = r;       // projmat rows 0, 1, then 3
+    }
+    if (threadIdx.x < 4) {
+        v_viewmat[12 + threadIdx.x] = 0.f;
+        v_projmat[8 + threadIdx.x] = 0.f;
     }
 }
 
@@ -440,7 +517,7 @@ static int project_backward_impl(bool act, bool acc, bool aa, int n, const float
                                  const float *projmat, float fx, float fy, int img_h, int img_w,
                                  const int32_t *radii, const float *conics, const float *v_xy, const float *v_depth,
                                  const float *v_conic, const float *v_opacity, float *v_mean3d, float *v_scale,
-                                 float *v_quat, float *v_opacity_logits, gsb_stream_t stream) {
+                                 float *v_quat, float *v_opacity_logits, float *cam_partials, gsb_stream_t stream) {
     GSB_CHECK_ARG(n >= 0 && img_h > 0 && img_w > 0);
     if (n == 0) return 0;
     GSB_CHECK_ARG(means3d && scales && quats && viewmat && projmat && radii && conics && v_xy && v_conic &&
@@ -449,12 +526,16 @@ static int project_backward_impl(bool act, bool acc, bool aa, int n, const float
     GSB_CHECK_ARG(((uintptr_t)quats % 16) == 0 && ((uintptr_t)v_quat % 16) == 0 && ((uintptr_t)v_xy % 8) == 0);
     const float tan_fovx = (float)(0.5 * (double)img_w / (double)fx);
     const float tan_fovy = (float)(0.5 * (double)img_h / (double)fy);
-#define GSB_PJ_B(A, ACC, AA) project_backward_kernel<A, ACC, AA><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
+#define GSB_PJ_B(A, ACC, AA, CG) project_backward_kernel<A, ACC, AA, CG><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
         n, means3d, scales, glob_scale, quats, viewmat, projmat, fx, fy, tan_fovx, tan_fovy, img_h, img_w, radii,     \
         conics, reinterpret_cast<const float2 *>(v_xy), v_depth, v_conic, v_mean3d, v_scale,                          \
-        reinterpret_cast<float4 *>(v_quat), opacities, v_opacity, v_opacity_logits)
-    if (aa) { if (acc) GSB_PJ_B(true, true, true); else GSB_PJ_B(true, false, true); }
-    else if (acc) GSB_PJ_B(true, true, false); else if (act) GSB_PJ_B(true, false, false); else GSB_PJ_B(false, false, false);
+        reinterpret_cast<float4 *>(v_quat), opacities, v_opacity, v_opacity_logits, cam_partials)
+    if (cam_partials) {
+        if (aa) { if (acc) GSB_PJ_B(true, true, true, true); else GSB_PJ_B(true, false, true, true); }
+        else if (acc) GSB_PJ_B(true, true, false, true); else GSB_PJ_B(true, false, false, true);
+    } else if (aa) { if (acc) GSB_PJ_B(true, true, true, false); else GSB_PJ_B(true, false, true, false); }
+    else if (acc) GSB_PJ_B(true, true, false, false); else if (act) GSB_PJ_B(true, false, false, false);
+    else GSB_PJ_B(false, false, false, false);
 #undef GSB_PJ_B
     GSB_LAUNCH_CHECK();
     return 0;
@@ -469,7 +550,7 @@ extern "C" int gsb_project_backward(int n, const float *means3d, const float *sc
     (void)cov3d; (void)cx; (void)cy;
     return project_backward_impl(false, false, false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx,
                                  fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, nullptr, v_mean3d, v_scale,
-                                 v_quat, nullptr, stream);
+                                 v_quat, nullptr, nullptr, stream);
 }
 
 extern "C" int gsb_project_backward_activated(int n, const float *means3d, const float *log_scales, float glob_scale,
@@ -481,7 +562,7 @@ extern "C" int gsb_project_backward_activated(int n, const float *means3d, const
                                               float *v_opacity_logits, gsb_stream_t stream) {
     return project_backward_impl(true, false, false, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
                                  projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
-                                 v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
+                                 v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr, stream);
 }
 
 // The same VJP added into the four outputs (v += vjp): a trainer's several views of one step summed in place.
@@ -494,7 +575,7 @@ extern "C" int gsb_project_backward_activated_acc(int n, const float *means3d, c
                                                   float *v_raw_quats, float *v_opacity_logits, gsb_stream_t stream) {
     return project_backward_impl(true, true, false, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
                                  projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
-                                 v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
+                                 v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr, stream);
 }
 
 // D19: the activated projection with the anti-aliased opacity, opacities = sigmoid(logits) * comp.
@@ -521,7 +602,7 @@ extern "C" int gsb_project_backward_activated_aa(int n, const float *means3d, co
                                                  float *v_opacity_logits, gsb_stream_t stream) {
     return project_backward_impl(true, false, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
                                  viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic,
-                                 v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
+                                 v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr, stream);
 }
 
 extern "C" int gsb_project_backward_activated_aa_acc(int n, const float *means3d, const float *log_scales,
@@ -535,5 +616,36 @@ extern "C" int gsb_project_backward_activated_aa_acc(int n, const float *means3d
                                                      gsb_stream_t stream) {
     return project_backward_impl(true, true, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
                                  viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic,
-                                 v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, stream);
+                                 v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr, stream);
+}
+
+// D22: the activated projection backward (any of the four variants above: accumulate = the _acc form, antialiased =
+// the _aa form, opacities then the logits) that also writes the view's camera gradient as one partial row per block.
+extern "C" size_t gsb_project_camera_partials_floats(int n) {
+    return n > 0 ? (size_t)CG_TERMS * gsb_div_up(n, PJ_THREADS) : 0;
+}
+
+extern "C" int gsb_project_backward_activated_camgrad(int n, const float *means3d, const float *log_scales,
+                                                      float glob_scale, const float *raw_quats,
+                                                      const float *opacities, const float *viewmat,
+                                                      const float *projmat, float fx, float fy, int img_h, int img_w,
+                                                      const int32_t *radii, const float *conics, const float *v_xy,
+                                                      const float *v_depth, const float *v_conic,
+                                                      const float *v_opacity, float *v_mean3d, float *v_log_scales,
+                                                      float *v_raw_quats, float *v_opacity_logits, int accumulate,
+                                                      int antialiased, float *cam_partials, gsb_stream_t stream) {
+    GSB_CHECK_ARG((accumulate == 0 || accumulate == 1) && (antialiased == 0 || antialiased == 1));
+    GSB_CHECK_ARG(n >= 0 && (n == 0 || cam_partials));
+    return project_backward_impl(true, accumulate != 0, antialiased != 0, n, means3d, log_scales, glob_scale,
+                                 raw_quats, opacities, viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy,
+                                 v_depth, v_conic, v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits,
+                                 cam_partials, stream);
+}
+
+extern "C" int gsb_project_camera_grad_reduce(int nblocks, const float *partials, float *v_viewmat, float *v_projmat,
+                                              gsb_stream_t stream) {
+    GSB_CHECK_ARG(nblocks >= 0 && (nblocks == 0 || partials) && v_viewmat && v_projmat);
+    camgrad_reduce_kernel<<<1, CG_TERMS * 32, 0, (cudaStream_t)stream>>>(nblocks, partials, v_viewmat, v_projmat);
+    GSB_LAUNCH_CHECK();
+    return 0;
 }

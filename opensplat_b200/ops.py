@@ -604,7 +604,10 @@ class ProjectGaussiansActivated(torch.autograd.Function):
     """ProjectGaussians on the RAW parameters of the model (model.cpp:148-150,200 + 152-165 as one operator):
     `scales` are log-scales (exp fused), `quats` un-normalised (the projection normalises), and the opacity logits
     ride along: returns (xys, depths, radii, conics, numTilesHit, cov3d, opacities [N,1] = sigmoid(logits)).
-    Gradients come back w.r.t. the raw parameters.  C++ twin: gsb::ProjectGaussiansActivated."""
+    Gradients come back w.r.t. the raw parameters, and w.r.t. viewMat and projMat when those require grad (DESIGN
+    D22: the exact VJP summed over the visible Gaussians, reduced inside the projection backward; row 3 of the
+    viewMat gradient and row 2 of the projMat gradient are 0, as the projection does not read them).  C++ twin:
+    gsb::ProjectGaussiansActivated (without the camera gradient)."""
 
     @staticmethod
     def forward(ctx, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat, fx, fy, cx, cy,
@@ -634,7 +637,7 @@ class ProjectGaussiansActivated(torch.autograd.Function):
             float(clipThresh), capi.ptr(cov3d), capi.ptr(xys), capi.ptr(depths), capi.ptr(radii), capi.ptr(conics),
             capi.ptr(nth), capi.ptr(opac), capi.stream()))
         ctx.meta = (float(globScale), float(fx), float(fy), int(imgHeight), int(imgWidth), tuple(opacityLogits.shape),
-                    aa)
+                    aa, tuple(viewMat.shape), tuple(projMat.shape))
         # the plain backward takes sigmoid(logits) from the forward, the anti-aliased one the logits themselves
         ctx.save_for_backward(m3, ls, rq, vm, pm, radii, conics, ol if aa else opac)
         ctx.mark_non_differentiable(radii, nth)
@@ -643,7 +646,7 @@ class ProjectGaussiansActivated(torch.autograd.Function):
     @staticmethod
     def backward(ctx, v_xys, v_depths, v_radii, v_conics, v_numTiles, v_cov3d, v_opac):
         m3, ls, rq, vm, pm, radii, conics, opac = ctx.saved_tensors
-        gs, fx, fy, H, W, ol_shape, aa = ctx.meta
+        gs, fx, fy, H, W, ol_shape, aa, vm_shape, pm_shape = ctx.meta
         n = m3.shape[0]
         if v_xys is None:
             v_xys = torch.zeros_like(m3[:, :2])
@@ -657,12 +660,25 @@ class ProjectGaussiansActivated(torch.autograd.Function):
         vd = capi.f32(v_depths) if v_depths is not None else None
         vo = capi.f32(v_opac).reshape(n) if v_opac is not None else None
         L = capi.lib()
-        capi.check((L.gsb_project_backward_activated_aa if aa else L.gsb_project_backward_activated)(
-            n, capi.ptr(m3), capi.ptr(ls), gs, capi.ptr(rq), capi.ptr(opac), capi.ptr(vm), capi.ptr(pm), fx, fy, H, W,
-            capi.ptr(radii), capi.ptr(conics), capi.ptr(vx), capi.ptr(vd), capi.ptr(vc), capi.ptr(vo),
-            capi.ptr(v_mean), capi.ptr(v_ls), capi.ptr(v_rq), capi.ptr(v_ol), capi.stream()))
-        # 15 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4)
-        return (v_mean, v_ls, None, v_rq, v_ol.reshape(ol_shape)) + (None,) * 10
+        args = (n, capi.ptr(m3), capi.ptr(ls), gs, capi.ptr(rq), capi.ptr(opac), capi.ptr(vm), capi.ptr(pm), fx, fy, H,
+                W, capi.ptr(radii), capi.ptr(conics), capi.ptr(vx), capi.ptr(vd), capi.ptr(vc), capi.ptr(vo),
+                capi.ptr(v_mean), capi.ptr(v_ls), capi.ptr(v_rq), capi.ptr(v_ol))
+        v_view = v_proj = None
+        if ctx.needs_input_grad[5] or ctx.needs_input_grad[6]:
+            # D22: the camera gradient, reduced over the Gaussians inside the projection backward
+            part = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, m3)
+            v_view = _empty((4, 4), torch.float32, m3)
+            v_proj = _empty((4, 4), torch.float32, m3)
+            capi.check(L.gsb_project_backward_activated_camgrad(*args, 0, int(aa), capi.ptr(part), capi.stream()))
+            capi.check(L.gsb_project_camera_grad_reduce(part.numel() // capi.CAMGRAD_TERMS, capi.ptr(part),
+                                                        capi.ptr(v_view), capi.ptr(v_proj), capi.stream()))
+            v_view = v_view.reshape(vm_shape) if ctx.needs_input_grad[5] else None
+            v_proj = v_proj.reshape(pm_shape) if ctx.needs_input_grad[6] else None
+        else:
+            capi.check((L.gsb_project_backward_activated_aa if aa else L.gsb_project_backward_activated)(
+                *args, capi.stream()))
+        # 15 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4), viewMat(5), projMat(6)
+        return (v_mean, v_ls, None, v_rq, v_ol.reshape(ol_shape), v_view, v_proj) + (None,) * 8
 
 
 class ProjectGaussiansActivatedAntialiased(ProjectGaussiansActivated):

@@ -65,7 +65,14 @@ With per-image appearance grids (`appearance=appearance.AppearanceConfig(num_ima
 names its views' training images (`step(cam, gt, step, image=i)`).  The step first writes the grids' TV gradient;
 each view's clamped render is sliced through its image's grid before the loss, and the slice backward turns the loss
 gradient into the render's gradient and adds 1/B of the grid gradient; after the Gaussians' Adam step one Adam step
-updates every grid.  evaluate(), render() and `image` stay the raw render."""
+updates every grid.  evaluate(), render() and `image` stay the raw render.
+
+With per-image pose corrections (`pose=pose.PoseConfig(num_images=...)`, DESIGN D22) every step names its views'
+training images the same way.  Each view's camera is corrected on the device (gsb_pose_apply) between the upload and
+`proj @ view`; the step first writes reg * e into the corrections' gradient, each view's projection backward also
+reduces the camera gradient (gsb_project_backward_activated_camgrad, gsb_project_camera_grad_reduce), which
+gsb_pose_backward takes to 1/B of its image's correction gradient; after the Gaussians' Adam step one Adam step
+updates every correction.  evaluate() and render() take image= to render at that image's corrected pose."""
 import ctypes as C
 
 import torch
@@ -74,6 +81,7 @@ from . import capi, ops
 from .densify import Densifier, RefineConfig
 from .export import SceneWriter
 from .appearance import Appearance, to_gsplat_order
+from .pose import Poses
 from .mcmc import MCMCConfig, MCMCRefiner
 from .model import (LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, Camera, camera_setup, downscale_factor,
                     means_learning_rate)
@@ -107,6 +115,26 @@ def _split_coeffs(views):
     return {k: out[k] for k in PARAM_NAMES}
 
 
+def check_images(image, views, num_images):
+    """The step's training-image indices as a list of `views` ints; raises ValueError unless image= names `views`
+    images in [0, num_images).  Shared by the per-image features (appearance grids, pose corrections)."""
+    if image is None:
+        raise ValueError("a step with per-image appearance grids or pose corrections needs image= (the training "
+                         "image of each view)")
+    if isinstance(image, (list, tuple)):
+        idx = list(image)
+    elif views == 1:
+        idx = [image]
+    else:
+        raise ValueError(f"image= must be a sequence of {views} training images")
+    if len(idx) != views:
+        raise ValueError(f"image= must name {views} training images, got {len(idx)}")
+    for i in idx:
+        if isinstance(i, bool) or not isinstance(i, int) or not 0 <= i < num_images:
+            raise ValueError(f"image indices must be ints in [0, {num_images}), got {i!r}")
+    return idx
+
+
 def view_setups(cams, gts, views, downscale):
     """The camera blocks (model.camera_setup) of one step's `views` cameras at `downscale`, checked against the
     ground-truth images: returns (setups, H, W).  Raises ValueError unless there are exactly `views` cameras and
@@ -134,7 +162,7 @@ class SplatTrainer:
     def __init__(self, params, cfg=None, sh_degree=None, sh_degree_interval=1000, num_downscales=0,
                  resolution_schedule=3000, background=(0.6130, 0.0101, 0.3984), device="cuda:0", generator=None,
                  ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1, antialiased=False,
-                 appearance=None):
+                 appearance=None, pose=None):
         """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
         featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
         cfg: densify.RefineConfig (the reference's refinement, the default) or mcmc.MCMCConfig (3DGS-MCMC under a
@@ -146,7 +174,9 @@ class SplatTrainer:
         antialiased: train and render with the anti-aliased opacity (DESIGN D19), as model.GaussianModel(antialiased=
         True): the projection kernels are the _aa ones, and nothing else in the step changes.
         appearance: an appearance.AppearanceConfig to learn one bilateral grid per training image (DESIGN D21); step()
-        then takes image=.  Not available with group=."""
+        then takes image=.  Not available with group=.
+        pose: a pose.PoseConfig to learn one camera pose correction per training image (DESIGN D22); step() then takes
+        image=, and evaluate() / render() may.  Not available with group=; with appearance=, num_images must agree."""
         import torch.distributed as dist
         self.views_per_step = B = int(views_per_step)
         if B < 1:
@@ -156,6 +186,11 @@ class SplatTrainer:
                                "over camera views")
         if appearance is not None and group is not None:
             raise ValueError("appearance grids are not available with group= (data-parallel training)")
+        if pose is not None and group is not None:
+            raise ValueError("pose corrections are not available with group= (data-parallel training)")
+        if pose is not None and appearance is not None and pose.num_images != appearance.num_images:
+            raise ValueError(f"appearance= and pose= must name the same training images, got num_images "
+                             f"{appearance.num_images} and {pose.num_images}")
         self.device = torch.device(device)
         self.cfg = cfg or RefineConfig()
         self.antialiased = bool(antialiased)
@@ -178,16 +213,25 @@ class SplatTrainer:
         pp.background.copy_(torch.tensor(background, dtype=torch.float32))
         self.L = capi.lib()
         self.appearance = None if appearance is None else Appearance(appearance, self.device)
+        self.poses = None if pose is None else Poses(pose, self.device)
+        self.num_images = next((c.num_images for c in (appearance, pose) if c is not None), None)
         self.lr = dict(LEARNING_RATES)
         # the refinement strategy: the reference's Model::afterTrain (RefineConfig) or 3DGS-MCMC (MCMCConfig, D20)
         self.refiner = MCMCRefiner(self.cfg) if isinstance(self.cfg, MCMCConfig) else None
         self.densifier = None if self.refiner is not None else Densifier(self.cfg, generator=generator, group=group)
-        # the B cameras: views [B,16] | projs [B,16] | centres [B,3], one pinned staging block, one upload per step
-        self.cams_host = torch.zeros(35 * B, dtype=torch.float32).pin_memory()
-        self.cams_dev = torch.zeros(35 * B, dtype=torch.float32, device=self.device)
+        # the B cameras: views [B,16] | projs [B,16] | centres [B,3], one pinned staging block, one upload per step;
+        # with pose corrections (D22) the uploaded views and centres go to base views [B,16] | base centres [B,3]
+        # behind them, and the corrected ones are written into the first slots
+        floats = 35 * B + (19 * B if pose is not None else 0)
+        self.cams_host = torch.zeros(floats, dtype=torch.float32).pin_memory()
+        self.cams_dev = torch.zeros(floats, dtype=torch.float32, device=self.device)
         self.viewmats = self.cams_dev[:16 * B].view(B, 4, 4)
         self.projs = self.cams_dev[16 * B:32 * B].view(B, 4, 4)
-        self.cam_positions = self.cams_dev[32 * B:].view(B, 3)
+        self.cam_positions = self.cams_dev[32 * B:35 * B].view(B, 3)
+        if pose is not None:
+            self.base_viewmats = self.cams_dev[35 * B:51 * B].view(B, 4, 4)
+            self.base_positions = self.cams_dev[51 * B:].view(B, 3)
+            self.cam_grads = torch.zeros((2, 4, 4), dtype=torch.float32, device=self.device)  # d/dview, d/dprojmat
         self.projmats = torch.zeros((B, 4, 4), dtype=torch.float32, device=self.device)
         self.losses = torch.zeros((B, 3), dtype=torch.float32, device=self.device)
         self.eval_loss = torch.zeros(3, dtype=torch.float32, device=self.device)    # evaluate()'s result
@@ -226,6 +270,10 @@ class SplatTrainer:
             self.rgb_ptrs = torch.tensor([self.v_rgb_views[b].data_ptr() for b in range(B)], dtype=torch.int64,
                                          device=d)
             self.geom_ptrs = torch.tensor([pp.grad_flat.data_ptr()], dtype=torch.int64, device=d)
+        if self.poses is not None:   # D22: the projection backward's per-block camera-gradient rows
+            floats = self.L.gsb_project_camera_partials_floats(n)
+            self.cam_blocks = floats // capi.CAMGRAD_TERMS
+            self.cam_partials = torch.empty(max(floats, 1), dtype=torch.float32, device=d)
 
     def _set_resolution(self, W, H):
         if self.resolution is not None:
@@ -265,34 +313,50 @@ class SplatTrainer:
             raise ValueError("this trainer has no appearance grids")
         return to_gsplat_order(self.appearance.grids)
 
+    def pose_deltas(self):
+        """A copy of the pose corrections, [num_images, 9]: translation e[0:3] and 6-D rotation offset e[3:9] per
+        training image (D22; pose.adjusted_camera applies one to a model.Camera)."""
+        if self.poses is None:
+            raise ValueError("this trainer has no pose corrections")
+        return self.poses.deltas.clone()
+
+    def _images(self, image, views):
+        """The training images of `views` views (check_images), or None for each view when image is None and
+        nothing requires it."""
+        if self.num_images is None:
+            if image is not None:
+                raise ValueError("image= needs a trainer constructed with appearance= or pose=")
+            return [None] * views
+        return check_images(image, views, self.num_images)
+
     def step(self, cam, gt, step, image=None):
         """One training step at `step` (1-based, as opensplat.cpp counts).  At views_per_step = 1: cam is one
         model.Camera, gt one [H,W,3] fp32 CUDA image at this step's render resolution, and the result is the device
         tensor {total, L1, SSIM}.  At B > 1: cam is a sequence of B cameras, gt B images (a sequence or a [B,H,W,3]
         tensor), and the result is the device [B,3] tensor of the views' {total, L1, SSIM}.  The next step overwrites
-        the result.  image: with appearance grids, the training image of the view (an int) or of each of the B views
-        (a sequence of B ints); without them it must be None.  Raises ValueError on a wrong number of views, mixed
-        resolutions, a wrong image or a wrong image=."""
-        pp, B, ap = self.pipe, self.views_per_step, self.appearance
-        if ap is None and image is not None:
-            raise ValueError("image= needs a trainer constructed with appearance=")
-        images = ap.check_images(image, B) if ap is not None else [None] * B
+        the result.  image: with appearance grids or pose corrections, the training image of the view (an int) or of
+        each of the B views (a sequence of B ints); without them it must be None.  Raises ValueError on a wrong number
+        of views, mixed resolutions, a wrong image or a wrong image=."""
+        pp, B, ap, po = self.pipe, self.views_per_step, self.appearance, self.poses
+        images = self._images(image, B)
         gts = [gt] if B == 1 else gt
         # ---- forward, enqueued without a host wait until each view's binning read-back ----
-        setups, H, W, use = self._setup_views(cam, gts, B, step)
+        setups, H, W, use = self._setup_views(cam, gts, B, step, images if po is not None else None)
         if ap is not None:
             ap.tv()                         # D21: the grids' gradient starts as tv_weight * dTV
+        if po is not None:
+            po.start_step()                 # D22: the corrections' gradient starts as reg * e
         visible = []
         for b in range(B):
             intr = setups[b][2]
-            self._render_view(b, intr, gts[b], self.losses[b], image=images[b])
+            self._render_view(b, intr, gts[b], self.losses[b], image=images[b] if ap is not None else None)
             visible.append(pp.plan.visible > 0)
             # model.cpp:173-174: a lone view that hits nothing trains nothing.  Next to other views, or data-parallel
             # with more than one rank, its backward pass runs and writes zero gradients (no Gaussian has radii > 0):
             # the sum over the views and the divisor B x G stay as they are, and the rank takes the exchange's
             # barriers.
             if B > 1 or visible[b] or self.world > 1:
-                self._backward_view(b, use, intr[0], intr[1])
+                self._backward_view(b, use, intr[0], intr[1], image=images[b])
             # this view's densification statistics (pp.v_xy / pp.radii are overwritten by the next view)
             if self.densifier is not None:
                 self.densifier.accumulate_view(step, pp.v_xy if visible[b] else None, pp.radii, H, W)
@@ -306,6 +370,8 @@ class SplatTrainer:
             self._adam_step()
             if ap is not None:
                 ap.adam_step(step)
+            if po is not None:
+                po.adam_step(step)
         self.lr["means"] = means_learning_rate(step, self.cfg.max_steps, MEANS_LR_INIT)
         if trains and self.refiner is not None:
             # ---- D20: relocation and growth on a refinement step, then the position noise ----
@@ -318,7 +384,7 @@ class SplatTrainer:
             self.last_info = {"refined": False}
         return self.losses[0] if B == 1 else self.losses
 
-    def evaluate(self, cam, gt, step):
+    def evaluate(self, cam, gt, step, image=None):
         """The loss of one view without training on it (opensplat.cpp:203-207, the --val camera): Model::forward at
         `step`'s downscale factor and SH degree, then mainLoss against gt (a float32 [H,W,3] CUDA image at that
         resolution).  It runs the forward kernels and the loss of a one-view step() (at any views_per_step) and
@@ -327,13 +393,13 @@ class SplatTrainer:
         without this call.  Other trainer state it does change: `image` becomes the evaluated view's render; a view
         at another resolution than the last step's reallocates the pixel buffers, and the next step reallocates them
         back, each counted in `pixel_reallocs`; and the binning buffers grow if the view needs more intersections
-        than they hold (a step grows them the same way, with no effect on its result).  Raises ValueError on a
-        wrong image."""
-        setups = self._setup_views(cam, [gt], 1, step)[0]
+        than they hold (a step grows them the same way, with no effect on its result).  image: with pose corrections,
+        render at training image `image`'s corrected pose (D22).  Raises ValueError on a wrong image or image=."""
+        setups = self._setup_views(cam, [gt], 1, step, self._view_pose(image))[0]
         self._render_view(0, setups[0][2], gt, self.eval_loss)
         return self.eval_loss
 
-    def render(self, cam, step, normalize_depth=False):
+    def render(self, cam, step, normalize_depth=False, image=None):
         """Renders one view without training on it: Model::forward at `step`'s downscale factor and SH degree (the
         clamped colour, as evaluate() renders it) plus the depth and opacity maps (DESIGN D18).  Returns
         {"rgb" [H,W,3], "depth" [H,W], "alpha" [H,W]}: depth = sum alpha T z over the blended pairs (z the view-space
@@ -341,8 +407,8 @@ class SplatTrainer:
         where alpha > 0 and 0 elsewhere.  The tensors are overwritten by the next render().  Like evaluate(), it leaves
         parameters, Adam state and the densification statistics alone, and the next step() computes what it would have
         computed without this call; it does not change `image`.  A view at another resolution than the last step's
-        reallocates the pixel buffers, as evaluate() does."""
-        setups = self._setup_views(cam, None, 1, step)[0]
+        reallocates the pixel buffers, as evaluate() does.  image: as evaluate()'s."""
+        setups = self._setup_views(cam, None, 1, step, self._view_pose(image))[0]
         pp = self.pipe
         H, W = pp.H, pp.W
         if self.render_maps is None:
@@ -360,12 +426,21 @@ class SplatTrainer:
             depth.masked_fill_(r["alpha"] <= 0, 0.0)
         return {"rgb": r["rgb"], "depth": depth, "alpha": r["alpha"]}
 
-    def _setup_views(self, cams, gts, views, step):
+    def _view_pose(self, image):
+        """evaluate() / render()'s image= as _setup_views' `images`: None without it."""
+        if image is None:
+            return None
+        if self.poses is None:
+            raise ValueError("image= in evaluate() and render() needs a trainer constructed with pose=")
+        return check_images(image, 1, self.num_images)
+
+    def _setup_views(self, cams, gts, views, step, images=None):
         """What the forward passes of a step's `views` views share: view_setups at `step`'s downscale factor, the
         render resolution, one upload of the cameras into slots 0..views-1 of the camera block (the last host wait, a
         binning read-back, came after the block's previous upload), `proj @ view` and the SH colours.  One view takes
-        the 2-D matmul and the one-view SH forward (see the module docstring).  Returns (setups, H, W, use): use is
-        the step's SH degrees_to_use."""
+        the 2-D matmul and the one-view SH forward (see the module docstring).  With `images` (D22: one training image
+        per view) each view's camera is uploaded into the base slots and corrected by its image's pose into the
+        working slots before the matmul.  Returns (setups, H, W, use): use is the step's SH degrees_to_use."""
         setups, H, W = view_setups(cams, gts, views, downscale_factor(step, self.num_downscales,
                                                                        self.resolution_schedule))
         if (W, H) != self.resolution:
@@ -373,10 +448,16 @@ class SplatTrainer:
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         host, B, n, p = self.cams_host, self.views_per_step, pp.n, pp.p
         for b, (_, _, _, view, proj, cam_pos) in enumerate(setups):
-            host[16 * b:16 * b + 16].copy_(view.reshape(16))
+            vo, co = (35 * B + 16 * b, 51 * B + 3 * b) if images is not None else (16 * b, 32 * B + 3 * b)
+            host[vo:vo + 16].copy_(view.reshape(16))
             host[16 * (B + b):16 * (B + b) + 16].copy_(proj.reshape(16))
-            host[32 * B + 3 * b:32 * B + 3 * b + 3].copy_(cam_pos)
+            host[co:co + 3].copy_(cam_pos)
         self.cams_dev.copy_(host, non_blocking=True)
+        if images is not None:
+            for b in range(views):
+                capi.check(L.gsb_pose_apply(P(self.poses.deltas[images[b]]), P(self.base_viewmats[b]),
+                                            P(self.base_positions[b]), P(self.viewmats[b]), P(self.cam_positions[b]),
+                                            s))
         use = min(step // self.sh_degree_interval, self.sh_degree)
         if views == 1:
             torch.matmul(self.projs[0], self.viewmats[0], out=self.projmats[0])
@@ -426,9 +507,11 @@ class SplatTrainer:
                                                  self.bilagrid_ws.data_ptr() + woff, self.bilagrid_ws.numel() - woff,
                                                  s))
 
-    def _backward_view(self, b, use, fx, fy):
+    def _backward_view(self, b, use, fx, fy, image=None):
         """View b's backward pass after its forward pass: rasterize-backward into colour slot b, then projection
-        backward into the geometry gradients (view 0 writes them, later views add to them).  Under a group it first
+        backward into the geometry gradients (view 0 writes them, later views add to them).  With pose corrections
+        (D22) the projection backward also reduces the view's camera gradient, which gsb_pose_backward adds, times
+        1/B, to training image `image`'s correction gradient.  Under a group it first
         publishes the view's camera centre, read by the peers' multi-view SH backward, and after the last view's
         rasterize-backward starts the exchange's colour half (degrees_to_use `use`).  On a view that hit nothing
         every gradient it writes is zero."""
@@ -446,10 +529,18 @@ class SplatTrainer:
         else:
             pj = L.gsb_project_backward_activated if b == 0 else L.gsb_project_backward_activated_acc
             opac = self.opac
-        capi.check(pj(n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(opac), P(self.viewmats[b]),
-                      P(self.projmats[b]), fx, fy, pp.H, pp.W, P(pp.radii), P(pp.conics), P(pp.v_xy), None,
-                      P(pp.v_conic), P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]),
-                      capi.stream()))
+        args = (n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(opac), P(self.viewmats[b]),
+                P(self.projmats[b]), fx, fy, pp.H, pp.W, P(pp.radii), P(pp.conics), P(pp.v_xy), None, P(pp.v_conic),
+                P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]))
+        if self.poses is None:
+            capi.check(pj(*args, capi.stream()))
+            return
+        s, po, cg = capi.stream(), self.poses, self.cam_grads
+        capi.check(L.gsb_project_backward_activated_camgrad(*args, int(b > 0), int(self.antialiased),
+                                                            P(self.cam_partials), s))
+        capi.check(L.gsb_project_camera_grad_reduce(self.cam_blocks, P(self.cam_partials), P(cg[0]), P(cg[1]), s))
+        capi.check(L.gsb_pose_backward(P(po.deltas[image]), P(self.base_viewmats[b]), P(self.projs[b]), P(cg[0]),
+                                       P(cg[1]), 1.0 / self.views_per_step, P(po.grad[image]), s))
 
     def _sh_backward(self, use):
         """The SH backward of the step's B colour gradients (degrees_to_use `use`, the clamp's gradient included) into
