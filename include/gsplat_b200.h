@@ -568,6 +568,31 @@ int gsb_pose_apply(const float *pose, const float *view, const float *centre, fl
 int gsb_pose_backward(const float *pose, const float *view, const float *proj, const float *v_viewmat,
                       const float *v_projmat, float scale, float *grad, gsb_stream_t stream);
 
+/* ---- Inverse-depth priors (DESIGN D23; graphdeco 3DGS's depth regularisation, gsplat's depth_loss) ----
+ * A prior sample p is valid iff it is finite and > 0 (0, negative, NaN and inf mean "no data").  Every result below
+ *   but the loss value is its fp32 restatement bit for bit (IEEE division, no fused multiply-add).
+ * gsb_inverse_depths: inv [n] = 1.f / depths[i] where radii[i] > 0, 0 elsewhere: the value stream the depth blend
+ *   renders (gathered in place of the sort key, so the blend still sorts by depths).
+ * gsb_inverse_depths_backward: v_z [n] = -((v_inv[i] * inv) * inv) where radii[i] > 0 (inv recomputed as above), 0
+ *   elsewhere; v_z is the projection backward's v_depth.
+ * gsb_inverse_depth_l1: over the [H,W] maps rendered R and prior P, v_rendered = scale_g * sgn(R - P) on valid pixels
+ *   (sgn(0) = 0) and 0 elsewhere, written completely; *loss_out (a device float) = sum over the valid pixels of
+ *   |R - P| / (H W), unweighted: each |R - P| rounded to fp32, summed in fp64 in a fixed order, divided and rounded
+ *   once (the same inputs give the same bits).  workspace: gsb_inverse_depth_l1_workspace_bytes(H, W), 8-byte
+ *   aligned.  1 <= H W < 2^31.
+ * gsb_depth_downscale_mean: dst [h/factor, w/factor] (integer division) = the mean of the valid samples of each
+ *   factor x factor block of src [h,w]: summed in fp32 in row-major order, then divided by their count, or 0 when the
+ *   block has none.  factor >= 1, h, w >= factor.
+ * None of them allocates; bad sizes and NULL pointers are rejected before any launch; n = 0 is a no-op. */
+int gsb_inverse_depths(int n, const float *depths, const int32_t *radii, float *inv, gsb_stream_t stream);
+int gsb_inverse_depths_backward(int n, const float *depths, const int32_t *radii, const float *v_inv, float *v_z,
+                                gsb_stream_t stream);
+size_t gsb_inverse_depth_l1_workspace_bytes(int img_h, int img_w);
+int gsb_inverse_depth_l1(int img_h, int img_w, const float *rendered, const float *prior, float scale_g,
+                         float *v_rendered, float *loss_out, void *workspace, size_t workspace_bytes,
+                         gsb_stream_t stream);
+int gsb_depth_downscale_mean(int h, int w, int factor, const float *src, float *dst, gsb_stream_t stream);
+
 /* ---- Scene export (Model::savePly model.cpp:505-558, Model::saveSplat :560-594; SURVEY.md 8f row 4) ----
  * Packs the file BODY on the device (the caller writes the text header and copies the rows D2H, typically on a
  * side stream into pinned memory).  features_dc / features_rest take a row stride in floats so both the reference's

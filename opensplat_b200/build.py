@@ -29,6 +29,7 @@ SOURCES = {
     "mcmc.cu": [],
     "bilagrid.cu": [],
     "pose.cu": [],
+    "depth.cu": ["--fmad=false"],
     "export.cu": ["--fmad=false"],
     "knn.cu": ["--fmad=false"],
     "image.cu": ["--fmad=false"],

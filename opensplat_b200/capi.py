@@ -113,6 +113,14 @@ _SIGS = {
     "gsb_pose_apply": (_i, [_vp, _vp, _vp, _vp, _vp, _vp]),
     # pose, view, proj, v_viewmat, v_projmat, scale, grad, stream
     "gsb_pose_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp]),
+    # n, depths, radii, inv, stream / n, depths, radii, v_inv, v_z, stream
+    "gsb_inverse_depths": (_i, [_i, _vp, _vp, _vp, _vp]),
+    "gsb_inverse_depths_backward": (_i, [_i, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_inverse_depth_l1_workspace_bytes": (_sz, [_i, _i]),
+    # H, W, rendered, prior, scale_g, v_rendered, loss_out, workspace, workspace_bytes, stream
+    "gsb_inverse_depth_l1": (_i, [_i, _i, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
+    # h, w, factor, src, dst, stream
+    "gsb_depth_downscale_mean": (_i, [_i, _i, _i, _vp, _vp, _vp]),
     "gsb_ply_row_floats": (_i, [_i]),
     "gsb_pack_ply_rows": (_i, [_i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp]),
     "gsb_unpack_ply_rows": (_i, [_i, _i, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp]),

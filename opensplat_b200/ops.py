@@ -278,18 +278,20 @@ class BinFrame:
             self.record_depths = torch.empty((max(m, 1),), dtype=torch.float32, device=self.dev)
 
     def bin_blend(self, xys, radii, conics, depths, nth, rgbs, opacities, background, out_img, final_Ts, final_idx,
-                  flags, count_visible=False, out_depth=None, out_alpha=None):
+                  flags, count_visible=False, out_depth=None, out_alpha=None, depth_values=None):
         """Binning, packing and the blend kernel of one frame (after SH colour and projection) into out_img [H,W,3],
         final_Ts and final_idx [H,W], with the frame's one host wait; returns out_img.  The per-Gaussian inputs are
         contiguous float32 / int32 CUDA tensors (nth: the projection's tile counts, read by the generic path only);
         flags: gsb_rasterize_forward_packed's; count_visible: have the binning count the Gaussians with radii > 0 into
         plan.visible.  out_depth / out_alpha ([H,W] float32, both or neither): the frame also writes the depth and
         opacity maps (DESIGN D18) through the DEPTH blend kernel, from the per-record depth stream it gathers from
-        `depths` (kept in `record_depths` for the backward)."""
+        `depths` (kept in `record_depths` for the backward).  depth_values ([n] float32, default `depths`): the
+        per-Gaussian value the depth map blends instead (DESIGN D23: 1/z); sorting and packing still read `depths`."""
         L, P, s, plan = self.L, capi.ptr, capi.stream(), self.plan
         depth = out_depth is not None
         if depth != (out_alpha is not None):
             raise ValueError("bin_blend: out_depth and out_alpha go together")
+        values = depths if depth_values is None else depth_values
         n, H, W = xys.shape[0], out_img.shape[0], out_img.shape[1]
         tb = tile_bounds(W, H)
         T = tb[0] * tb[1]
@@ -321,7 +323,7 @@ class BinFrame:
             if depth:
                 # the ids past M hold nothing valid: the gather reads M from the stats (no Gaussian: M = 0)
                 if n > 0:
-                    capi.check(L.gsb_gather_record_depths(m_cap, P(self.gids_sorted), P(depths), P(self.stats_dev),
+                    capi.check(L.gsb_gather_record_depths(m_cap, P(self.gids_sorted), P(values), P(self.stats_dev),
                                                           P(self.record_depths), s))
                 capi.check(L.gsb_rasterize_forward_packed_depth(
                     H, W, tb[0], tb[1], m_cap, P(self.tile_bins), P(self.tile_order), P(self.stats_dev),
@@ -357,7 +359,7 @@ class BinFrame:
                                       P(self.records), s))
         if depth:
             self._depth_buffers(m)
-            capi.check(L.gsb_gather_record_depths(m, P(gids_sorted), P(depths), None, P(self.record_depths), s))
+            capi.check(L.gsb_gather_record_depths(m, P(gids_sorted), P(values), None, P(self.record_depths), s))
             capi.check(L.gsb_rasterize_forward_packed_depth(
                 H, W, tb[0], tb[1], m, P(self.tile_bins), None, None, P(background), P(self.records), P(out_img),
                 P(final_Ts), P(final_idx), flags, P(self.record_depths), P(out_depth), P(out_alpha), s))
@@ -522,12 +524,17 @@ class RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def _forward(ctx, flags, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background,
-                 depth=False):
-        """The forward of the rasterizer operators: the image, or with depth=True (image, depth map, alpha map)."""
+                 depth=False, depth_values=None):
+        """The forward of the rasterizer operators: the image, or with depth=True (image, depth map, alpha map); the
+        depth map blends depth_values ([n], default depths) when given."""
         if colors.shape[-1] != 3:
             raise ValueError("only 3-channel colors are supported")
         xys, depths, conics, colors, opacity, background = (capi.f32(t) for t in (xys, depths, conics, colors,
                                                                                    opacity, background))
+        if depth_values is not None:
+            depth_values = capi.f32(depth_values).reshape(-1)
+            if depth_values.shape[0] != xys.shape[0]:
+                raise ValueError("depthValues must hold one value per Gaussian")
         H, W = int(imgHeight), int(imgWidth)
         out = _empty((H, W, 3), torch.float32, xys)
         fT = _empty((H, W), torch.float32, xys)
@@ -537,8 +544,9 @@ class RasterizeGaussians(torch.autograd.Function):
         # one frame per call on the device's plan; the backward gets its tensors through save_for_backward
         f = BinFrame(_plan_for(xys.device), xys.device)
         f.bin_blend(xys, radii.contiguous(), conics, depths, numTilesHit, colors, opacity, background, out, fT, fI,
-                    flags, out_depth=od, out_alpha=oa)
+                    flags, out_depth=od, out_alpha=oa, depth_values=depth_values)
         ctx.meta = (H, W, xys.shape[0], f.m_raster, flags)
+        ctx.depth_values = depth_values is not None
         ctx.save_for_backward(f.tile_bins, conics, opacity, f.records, f.cum, background, fT, fI,
                               f.tile_order if f._ordered else None, f.record_depths if depth else None)
         return (out, od, oa) if depth else out
@@ -570,12 +578,17 @@ class RasterizeGaussiansDepth(torch.autograd.Function):
     depth [H,W], alpha [H,W]) with depth = sum alpha T z over the pairs the colour blend blends (z = `depths`, the
     projection's view-space depth; background depth 0, not normalised) and alpha = 1 - T_final.  rgb is bit-identical
     to RasterizeGaussians'.  Gradients go to xys (0), depths (1), conics (3), colors (5) and opacity (6), so a depth
-    loss reaches the means through ProjectGaussians' depths output.  C++ twin: gsb::RasterizeGaussiansDepth."""
+    loss reaches the means through ProjectGaussians' depths output.
+    With the optional trailing depthValues ([n], DESIGN D23: e.g. where(radii > 0, 1 / depths, 0)) the depth map
+    blends v = depthValues in place of z: depth = sum alpha T v, with the tiles still sorted by `depths`.  Its gradient
+    then goes to depthValues (slot 10) and none to depths; rgb, alpha and the other gradients are unchanged.  C++
+    twin (without depthValues): gsb::RasterizeGaussiansDepth."""
 
     @staticmethod
-    def forward(ctx, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background):
+    def forward(ctx, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background,
+                depthValues=None):
         return RasterizeGaussians._forward(ctx, 0, xys, depths, radii, conics, numTilesHit, colors, opacity,
-                                           imgHeight, imgWidth, background, depth=True)
+                                           imgHeight, imgWidth, background, depth=True, depth_values=depthValues)
 
     @staticmethod
     def backward(ctx, v_outImg, v_depth, v_alpha):
@@ -587,17 +600,21 @@ class RasterizeGaussiansDepth(torch.autograd.Function):
             H, W, n, m, bins, conics, opacity, records, cum, background, fT, fI, v_outImg.contiguous(),
             v_alpha.contiguous() if v_alpha is not None else None, tile_order=order, flags=flags, record_depths=rd,
             v_output_depth=v_depth.contiguous() if v_depth is not None else None)
-        return v_xy, v_depths, None, v_conic, None, v_colors, v_opacity, None, None, None
+        if ctx.depth_values:    # 11 slots: the depth gradient belongs to depthValues (10), not to depths (1)
+            return v_xy, None, None, v_conic, None, v_colors, v_opacity, None, None, None, v_depths.reshape(n)
+        return v_xy, v_depths, None, v_conic, None, v_colors, v_opacity, None, None, None, None
 
 
 class RasterizeGaussiansDepthClamped(RasterizeGaussiansDepth):
     """RasterizeGaussiansDepth with rgb = clamp_max(rgb, 1) fused as in RasterizeGaussiansClamped; depth and alpha are
-    never clamped.  C++ twin: gsb::RasterizeGaussiansDepthClamped."""
+    never clamped.  The same optional depthValues.  C++ twin (without depthValues): gsb::RasterizeGaussiansDepthClamped."""
 
     @staticmethod
-    def forward(ctx, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background):
+    def forward(ctx, xys, depths, radii, conics, numTilesHit, colors, opacity, imgHeight, imgWidth, background,
+                depthValues=None):
         return RasterizeGaussians._forward(ctx, CLAMP_MAX_ONE, xys, depths, radii, conics, numTilesHit, colors,
-                                           opacity, imgHeight, imgWidth, background, depth=True)
+                                           opacity, imgHeight, imgWidth, background, depth=True,
+                                           depth_values=depthValues)
 
 
 class ProjectGaussiansActivated(torch.autograd.Function):

@@ -168,14 +168,15 @@ class SplatPipeline(BinFrame):
         return self._bin_blend(p["opacities"], 0)
 
     def _bin_blend(self, opacities, flags, count_visible=False, rgbs=None, out_img=None, out_depth=None,
-                   out_alpha=None):
+                   out_alpha=None, depth_values=None):
         """bin_blend on the pipeline's projection and pixel buffers.  opacities: the [n] opacities the blend uses;
         rgbs: the [n,3] colours the records carry (default self.rgbs; a trainer with several views per step passes the
-        view's); out_img: the image (default self.out_img); out_depth / out_alpha: bin_blend's depth output."""
+        view's); out_img: the image (default self.out_img); out_depth / out_alpha / depth_values: bin_blend's depth
+        output and the per-Gaussian value it blends (default self.depths)."""
         return self.bin_blend(self.xys, self.radii, self.conics, self.depths, self.nth,
                               self.rgbs if rgbs is None else rgbs, opacities, self.background,
                               self.out_img if out_img is None else out_img, self.final_Ts, self.final_idx, flags,
-                              count_visible, out_depth=out_depth, out_alpha=out_alpha)
+                              count_visible, out_depth=out_depth, out_alpha=out_alpha, depth_values=depth_values)
 
     def _raster_backward(self, opacities, v_opacities, v_rgbs, flags):
         """The blend kernel's backward of the last frame (_bin_blend's), from the gradient of its image in self.v_img
@@ -189,6 +190,18 @@ class SplatPipeline(BinFrame):
             P(self.tile_order) if self._ordered else None, P(self.conics), P(opacities), P(self.records), P(self.cum),
             P(self.background), P(self.final_Ts), P(self.final_idx), P(self.v_img), None, P(self.grad_rows),
             P(self.v_xy), P(self.v_conic), P(v_rgbs), P(v_opacities), flags, capi.stream()))
+
+    def _raster_backward_depth(self, opacities, v_opacities, v_rgbs, flags, v_output_depth, v_depths):
+        """_raster_backward of a depth frame (_bin_blend with out_depth): the same outputs plus, from the gradient of
+        its depth map in `v_output_depth` ([H,W]), the gradient of the per-Gaussian value it blended into `v_depths`
+        ([n]), through the frame's record_depths.  The opacity map gets no cotangent."""
+        P = capi.ptr
+        capi.check(self.L.gsb_rasterize_backward_depth(
+            self.H, self.W, self.tb[0], self.tb[1], self.n, self.m_raster, P(self.tile_bins),
+            P(self.tile_order) if self._ordered else None, P(self.conics), P(opacities), P(self.records), P(self.cum),
+            P(self.background), P(self.final_Ts), P(self.final_idx), P(self.v_img), None, P(self.grad_rows),
+            P(self.v_xy), P(self.v_conic), P(v_rgbs), P(v_opacities), flags, P(self.record_depths),
+            P(v_output_depth), P(v_depths), capi.stream()))
 
     def backward(self):
         """MSE loss against self.target + the whole backward path; grads land in self.grad_flat."""

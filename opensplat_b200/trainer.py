@@ -72,7 +72,15 @@ training images the same way.  Each view's camera is corrected on the device (gs
 `proj @ view`; the step first writes reg * e into the corrections' gradient, each view's projection backward also
 reduces the camera gradient (gsb_project_backward_activated_camgrad, gsb_project_camera_grad_reduce), which
 gsb_pose_backward takes to 1/B of its image's correction gradient; after the Gaussians' Adam step one Adam step
-updates every correction.  evaluate() and render() take image= to render at that image's corrected pose."""
+updates every correction.  evaluate() and render() take image= to render at that image's corrected pose.
+
+With per-image inverse-depth priors (`depth=depth.DepthConfig()`, DESIGN D23) a step may give each view a prior
+(`step(cam, gt, step, depth=P)`).  A view with one also renders R = sum alpha T (1/z) through the depth blend (the
+tiles still sorted by z; the colour is the same bits), takes the masked L1 against P after the colour loss
+(gsb_inverse_depth_l1, weighted by depth.depth_weight), and its backward adds the depth term to the blend's geometry
+gradients and, through gsb_inverse_depths_backward, to the projection's depth; densification statistics and a pose
+correction's gradient see it too.  A view without one issues exactly the launches of a plain trainer.  The loss
+returned stays the image loss; `depth_losses` holds the unweighted depth loss of each view."""
 import ctypes as C
 
 import torch
@@ -82,6 +90,7 @@ from .densify import Densifier, RefineConfig
 from .export import SceneWriter
 from .appearance import Appearance, to_gsplat_order
 from .pose import Poses
+from .depth import DepthConfig, depth_weight
 from .mcmc import MCMCConfig, MCMCRefiner
 from .model import (LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, Camera, camera_setup, downscale_factor,
                     means_learning_rate)
@@ -162,7 +171,7 @@ class SplatTrainer:
     def __init__(self, params, cfg=None, sh_degree=None, sh_degree_interval=1000, num_downscales=0,
                  resolution_schedule=3000, background=(0.6130, 0.0101, 0.3984), device="cuda:0", generator=None,
                  ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1, antialiased=False,
-                 appearance=None, pose=None):
+                 appearance=None, pose=None, depth=None):
         """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
         featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
         cfg: densify.RefineConfig (the reference's refinement, the default) or mcmc.MCMCConfig (3DGS-MCMC under a
@@ -176,7 +185,9 @@ class SplatTrainer:
         appearance: an appearance.AppearanceConfig to learn one bilateral grid per training image (DESIGN D21); step()
         then takes image=.  Not available with group=.
         pose: a pose.PoseConfig to learn one camera pose correction per training image (DESIGN D22); step() then takes
-        image=, and evaluate() / render() may.  Not available with group=; with appearance=, num_images must agree."""
+        image=, and evaluate() / render() may.  Not available with group=; with appearance=, num_images must agree.
+        depth: a depth.DepthConfig to supervise the rendered inverse depth with per-image priors (DESIGN D23); step()
+        then takes depth=."""
         import torch.distributed as dist
         self.views_per_step = B = int(views_per_step)
         if B < 1:
@@ -191,6 +202,9 @@ class SplatTrainer:
         if pose is not None and appearance is not None and pose.num_images != appearance.num_images:
             raise ValueError(f"appearance= and pose= must name the same training images, got num_images "
                              f"{appearance.num_images} and {pose.num_images}")
+        if depth is not None and not isinstance(depth, DepthConfig):
+            raise ValueError("depth= takes a depth.DepthConfig")
+        self.depth = depth
         self.device = torch.device(device)
         self.cfg = cfg or RefineConfig()
         self.antialiased = bool(antialiased)
@@ -234,6 +248,7 @@ class SplatTrainer:
             self.cam_grads = torch.zeros((2, 4, 4), dtype=torch.float32, device=self.device)  # d/dview, d/dprojmat
         self.projmats = torch.zeros((B, 4, 4), dtype=torch.float32, device=self.device)
         self.losses = torch.zeros((B, 3), dtype=torch.float32, device=self.device)
+        self.depth_losses = torch.zeros(B, dtype=torch.float32, device=self.device)   # D23: per view, unweighted
         self.eval_loss = torch.zeros(3, dtype=torch.float32, device=self.device)    # evaluate()'s result
         self.resolution = None
         self.render_maps = None   # render()'s outputs, sized by the resolution
@@ -274,6 +289,10 @@ class SplatTrainer:
             floats = self.L.gsb_project_camera_partials_floats(n)
             self.cam_blocks = floats // capi.CAMGRAD_TERMS
             self.cam_partials = torch.empty(max(floats, 1), dtype=torch.float32, device=d)
+        if self.depth is not None:   # D23: 1/z where radii > 0, its blend gradient, and the projection's v_depth
+            self.inv_depths = torch.empty(n, dtype=torch.float32, device=d)
+            self.v_inv_depths = torch.empty(n, dtype=torch.float32, device=d)
+            self.v_z = torch.empty(n, dtype=torch.float32, device=d)
 
     def _set_resolution(self, W, H):
         if self.resolution is not None:
@@ -287,6 +306,12 @@ class SplatTrainer:
             self.v_adj = torch.empty((H, W, 3), dtype=torch.float32, device=self.device)
             self.bilagrid_ws = torch.empty(self.L.gsb_bilagrid_workspace_bytes(H, W) + 256, dtype=torch.uint8,
                                            device=self.device)
+        if self.depth is not None:   # D23: the rendered inverse depth, its opacity map, its gradient, the L1's workspace
+            f32, d = torch.float32, self.device
+            self.depth_render = torch.empty((H, W), dtype=f32, device=d)
+            self.depth_alpha = torch.empty((H, W), dtype=f32, device=d)
+            self.v_depth_render = torch.empty((H, W), dtype=f32, device=d)
+            self.depth_ws = torch.empty(self.L.gsb_inverse_depth_l1_workspace_bytes(H, W), dtype=torch.uint8, device=d)
 
     @property
     def n(self):
@@ -329,17 +354,54 @@ class SplatTrainer:
             return [None] * views
         return check_images(image, views, self.num_images)
 
-    def step(self, cam, gt, step, image=None):
+    def _depth_maps(self, depth, views):
+        """step()'s depth= as a list of `views` maps or Nones, each checked for type, dtype, device and rank (step()
+        checks their size against the render resolution)."""
+        if depth is None:
+            return [None] * views
+        if self.depth is None:
+            raise ValueError("depth= needs a trainer constructed with depth=DepthConfig(...)")
+        if isinstance(depth, torch.Tensor):
+            if views == 1:
+                maps = [depth]
+            elif depth.dim() == 3:
+                maps = list(depth.unbind(0))
+            else:
+                raise ValueError(f"depth= must be a [{views},H,W] tensor or a sequence of {views} maps")
+        elif isinstance(depth, (list, tuple)):
+            maps = list(depth)
+        else:
+            raise ValueError("depth= must be a float32 [H,W] CUDA tensor, a sequence of them (or None), or [B,H,W]")
+        if len(maps) != views:
+            raise ValueError(f"depth= must give {views} maps (None for a view without one), got {len(maps)}")
+        for m in maps:
+            if m is None:
+                continue
+            if (not isinstance(m, torch.Tensor) or m.dtype != torch.float32 or m.device != self.device
+                    or m.dim() != 2 or not m.is_contiguous()):
+                raise ValueError(f"every depth map must be a contiguous float32 [H,W] tensor on {self.device}")
+        return maps
+
+    def step(self, cam, gt, step, image=None, depth=None):
         """One training step at `step` (1-based, as opensplat.cpp counts).  At views_per_step = 1: cam is one
         model.Camera, gt one [H,W,3] fp32 CUDA image at this step's render resolution, and the result is the device
         tensor {total, L1, SSIM}.  At B > 1: cam is a sequence of B cameras, gt B images (a sequence or a [B,H,W,3]
         tensor), and the result is the device [B,3] tensor of the views' {total, L1, SSIM}.  The next step overwrites
         the result.  image: with appearance grids or pose corrections, the training image of the view (an int) or of
-        each of the B views (a sequence of B ints); without them it must be None.  Raises ValueError on a wrong number
-        of views, mixed resolutions, a wrong image or a wrong image=."""
+        each of the B views (a sequence of B ints); without them it must be None.  depth: with depth priors (D23), at
+        B = 1 one float32 [H,W] CUDA inverse-depth map at this step's render resolution or None; at B > 1 a sequence of
+        B such maps, any of which may be None, or a [B,H,W] tensor.  Raises ValueError on a wrong number of views,
+        mixed resolutions, a wrong image, a wrong image= or a wrong depth=."""
         pp, B, ap, po = self.pipe, self.views_per_step, self.appearance, self.poses
         images = self._images(image, B)
+        priors = self._depth_maps(depth, B)
         gts = [gt] if B == 1 else gt
+        if any(m is not None for m in priors):
+            _, H, W = view_setups(cam, gts, B, downscale_factor(step, self.num_downscales, self.resolution_schedule))
+            if any(m is not None and tuple(m.shape) != (H, W) for m in priors):
+                raise ValueError(f"every depth map must be [{H},{W}] (this step's render resolution)")
+            # g = w(s) / (H W) in fp64, rounded once: the gradient of the weighted loss w.r.t. a valid pixel of R
+            depth_g = float(depth_weight(self.depth, step) / (H * W))
         # ---- forward, enqueued without a host wait until each view's binning read-back ----
         setups, H, W, use = self._setup_views(cam, gts, B, step, images if po is not None else None)
         if ap is not None:
@@ -349,14 +411,19 @@ class SplatTrainer:
         visible = []
         for b in range(B):
             intr = setups[b][2]
-            self._render_view(b, intr, gts[b], self.losses[b], image=images[b] if ap is not None else None)
+            self._render_view(b, intr, gts[b], self.losses[b], image=images[b] if ap is not None else None,
+                              prior=priors[b])
+            if priors[b] is not None:
+                self._depth_loss(priors[b], depth_g, self.depth_losses[b])
+            elif self.depth is not None:
+                self.depth_losses[b].zero_()
             visible.append(pp.plan.visible > 0)
             # model.cpp:173-174: a lone view that hits nothing trains nothing.  Next to other views, or data-parallel
             # with more than one rank, its backward pass runs and writes zero gradients (no Gaussian has radii > 0):
             # the sum over the views and the divisor B x G stay as they are, and the rank takes the exchange's
             # barriers.
             if B > 1 or visible[b] or self.world > 1:
-                self._backward_view(b, use, intr[0], intr[1], image=images[b])
+                self._backward_view(b, use, intr[0], intr[1], image=images[b], prior=priors[b] is not None)
             # this view's densification statistics (pp.v_xy / pp.radii are overwritten by the next view)
             if self.densifier is not None:
                 self.densifier.accumulate_view(step, pp.v_xy if visible[b] else None, pp.radii, H, W)
@@ -469,10 +536,10 @@ class SplatTrainer:
                                                           P(p["coeffs"]), 0.5, P(self.rgbs_views), s))
         return setups, H, W, use
 
-    def _project_blend(self, b, intr, out_img=None, out_depth=None, out_alpha=None):
+    def _project_blend(self, b, intr, out_img=None, out_depth=None, out_alpha=None, prior=False):
         """View b's projection with the activations from camera slot b (intrinsics `intr`), then binning and the
         clamped blend (the view's one host wait) into the pipeline's image, or into out_img with the depth and opacity
-        maps (render())."""
+        maps (render()).  prior (D23): also 1/z where radii > 0, blended into depth_render."""
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         n, p, tb, H, W = pp.n, pp.p, pp.tb, pp.H, pp.W
         fx, fy, cx, cy = intr
@@ -481,17 +548,21 @@ class SplatTrainer:
             n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmats[b]),
             P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
             P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac), s))
+        if prior:
+            capi.check(L.gsb_inverse_depths(n, P(pp.depths), P(pp.radii), P(self.inv_depths), s))
+            out_depth, out_alpha = self.depth_render, self.depth_alpha
         pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[b], out_img=out_img,
-                      out_depth=out_depth, out_alpha=out_alpha)
+                      out_depth=out_depth, out_alpha=out_alpha, depth_values=self.inv_depths if prior else None)
 
-    def _render_view(self, b, intr, gt, loss, image=None):
+    def _render_view(self, b, intr, gt, loss, image=None, prior=None):
         """View b's forward pass after _setup_views: _project_blend, then the loss against gt into `loss` ({total, L1,
         SSIM}) and its image gradient into the pipeline's v_img.  With a training image (D21) the loss is taken on
         the render sliced through that image's grid, and the slice backward writes v_img and adds 1/B of the grid
-        gradient."""
+        gradient.  prior (D23): the view's depth prior; the blend also renders the inverse depth (_depth_loss takes
+        its loss)."""
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         H, W = pp.H, pp.W
-        self._project_blend(b, intr)
+        self._project_blend(b, intr, prior=prior is not None)
         off = (-self.ssim_ws.data_ptr()) % 256
         if image is None:
             capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(loss),
@@ -507,11 +578,20 @@ class SplatTrainer:
                                                  self.bilagrid_ws.data_ptr() + woff, self.bilagrid_ws.numel() - woff,
                                                  s))
 
-    def _backward_view(self, b, use, fx, fy, image=None):
+    def _depth_loss(self, prior, g, loss):
+        """D23: the unweighted depth loss of the last _render_view into `loss` (a device float) and its gradient, g
+        times the sign on valid pixels, into v_depth_render."""
+        P = capi.ptr
+        H, W = self.pipe.H, self.pipe.W
+        capi.check(self.L.gsb_inverse_depth_l1(H, W, P(self.depth_render), P(prior), g, P(self.v_depth_render),
+                                               P(loss), P(self.depth_ws), self.depth_ws.numel(), capi.stream()))
+
+    def _backward_view(self, b, use, fx, fy, image=None, prior=False):
         """View b's backward pass after its forward pass: rasterize-backward into colour slot b, then projection
         backward into the geometry gradients (view 0 writes them, later views add to them).  With pose corrections
         (D22) the projection backward also reduces the view's camera gradient, which gsb_pose_backward adds, times
-        1/B, to training image `image`'s correction gradient.  Under a group it first
+        1/B, to training image `image`'s correction gradient.  With a depth prior (D23) the blend backward also takes
+        the depth map's gradient, and its 1/z gradient reaches the projection's v_depth.  Under a group it first
         publishes the view's camera centre, read by the peers' multi-view SH backward, and after the last view's
         rasterize-backward starts the exchange's colour half (degrees_to_use `use`).  On a view that hit nothing
         every gradient it writes is zero."""
@@ -519,7 +599,15 @@ class SplatTrainer:
         n, p, g, ex = pp.n, pp.p, pp.g, self.exchange
         if ex is not None:
             ex.set_camera(self.cam_positions[b], b)
-        pp._raster_backward(self.opac, self.v_opac, self.v_rgb_views[b], ops.CLAMP_MAX_ONE)
+        v_depth = None
+        if prior:
+            pp._raster_backward_depth(self.opac, self.v_opac, self.v_rgb_views[b], ops.CLAMP_MAX_ONE,
+                                      self.v_depth_render, self.v_inv_depths)
+            capi.check(L.gsb_inverse_depths_backward(n, P(pp.depths), P(pp.radii), P(self.v_inv_depths), P(self.v_z),
+                                                     capi.stream()))
+            v_depth = self.v_z
+        else:
+            pp._raster_backward(self.opac, self.v_opac, self.v_rgb_views[b], ops.CLAMP_MAX_ONE)
         if ex is not None and ex.overlap and b == self.views_per_step - 1:
             # every colour slot is final: colour pulls + SH expansion start now, on a side stream
             ex.start_colour(degrees_to_use=use, rgbs=self.rgbs_views)
@@ -530,8 +618,8 @@ class SplatTrainer:
             pj = L.gsb_project_backward_activated if b == 0 else L.gsb_project_backward_activated_acc
             opac = self.opac
         args = (n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(opac), P(self.viewmats[b]),
-                P(self.projmats[b]), fx, fy, pp.H, pp.W, P(pp.radii), P(pp.conics), P(pp.v_xy), None, P(pp.v_conic),
-                P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]))
+                P(self.projmats[b]), fx, fy, pp.H, pp.W, P(pp.radii), P(pp.conics), P(pp.v_xy), P(v_depth),
+                P(pp.v_conic), P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]))
         if self.poses is None:
             capi.check(pj(*args, capi.stream()))
             return
