@@ -647,6 +647,59 @@ size_t gsb_knn_workspace_bytes(int n);
 int gsb_knn_mean_dist(int n, const float *xyz, float *mean_dist, void *workspace, size_t workspace_bytes,
                       gsb_stream_t stream);
 
+/* ---- Mip-Splatting's 3-D smoothing filter (DESIGN D24) ------------------------------------------------------------
+ * gsb_project_forward_activated_filter3d: gsb_project_forward_activated (antialiased = 0) or _aa (1) with the filter
+ *   f = filter3d[i] (one float per Gaussian): the covariance is built from sigma_k = sqrtf(s_k s_k + f f) in place of
+ *   s_k = glob_scale expf(a_k), and opacities = sigmoid(logit) * c3 (* comp when antialiased, comp from the filtered
+ *   screen covariance), c3 = (r_0 r_1) r_2, r_k = s_k / sigma_k.  At f = 0 every output equals the unfiltered
+ *   entry point's bit for bit.
+ * gsb_project_backward_activated_filter3d: its exact VJP with filter3d held constant.  opacity_logits are the logits
+ *   (as the _aa backward takes them); accumulate = 1 adds to the four outputs (as _acc), camgrad = 1 also writes the
+ *   camera-gradient partial rows into cam_partials (as gsb_project_backward_activated_camgrad).  At f = 0 the outputs
+ *   equal the unfiltered variant's, up to the sign of a zero.
+ * gsb_filter3d_compute: filter3d [n] from the means [n,3] and num_cameras >= 1 training cameras, a DEVICE array of
+ *   GSB_FILTER3D_CAM_FLOATS floats each: viewmat rows 0..2 (12), fx, fy, cx, cy, W, H (fx > 0).  Camera j sees
+ *   Gaussian i when z > near and -(margin W) <= u <= (1 + margin) W and -(margin H) <= v <= (1 + margin) H, where
+ *   (x, y, z) is the projection's view-space point (tx, ty, tz), u = fx (x / z) + cx and v = fy (y / z) + cy, all fp32
+ *   without contraction; d[i] = the least such z, an unseen Gaussian takes the largest d of the seen ones, and
+ *   f[i] = (d[i] / F) * S with F = max_j fx_j and S = (float)sqrt((double)variance); every f is 0 when no Gaussian
+ *   is seen.  The result does not depend on scheduling (min / max only).  workspace: gsb_filter3d_workspace_bytes(),
+ *   4-byte aligned.  near, margin, variance >= 0 and finite.
+ * gsb_filter3d_bake: the filter baked into a scene at glob_scale 1, in fp64, each output rounded once:
+ *   out_log_scales = log(e^2 + f^2) / 2 with e = exp(a), out_opacity_logits = logit(sigmoid(l) c3).  In place is
+ *   allowed.
+ * gsb_reset_opacity_filter3d: gsb_reset_opacity on the effective opacity sigmoid(l) c3 (c3 the projection's fp32 value
+ *   at glob_scale 1): l = min(l, logit(reset_value / c3)) where reset_value / c3 < 1 (the logit in fp64, rounded once),
+ *   l unchanged where it is >= 1, and min(l, max_logit) -- gsb_reset_opacity's result -- where c3 == 1; the moments,
+ *   when given, are zeroed as there.
+ * None of them allocates; bad flags, sizes and NULL pointers are rejected before any launch; n = 0 is a no-op. */
+#define GSB_FILTER3D_CAM_FLOATS 18
+int gsb_project_forward_activated_filter3d(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                           const float *raw_quats, const float *opacity_logits, const float *filter3d,
+                                           const float *viewmat, const float *projmat, float fx, float fy, float cx,
+                                           float cy, int img_h, int img_w, int tiles_x, int tiles_y,
+                                           float clip_thresh, float *cov3d, float *xys, float *depths, int32_t *radii,
+                                           float *conics, int32_t *num_tiles_hit, float *opacities, int antialiased,
+                                           gsb_stream_t stream);
+int gsb_project_backward_activated_filter3d(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                            const float *raw_quats, const float *opacity_logits,
+                                            const float *filter3d, const float *viewmat, const float *projmat,
+                                            float fx, float fy, int img_h, int img_w, const int32_t *radii,
+                                            const float *conics, const float *v_xy, const float *v_depth,
+                                            const float *v_conic, const float *v_opacity, float *v_mean3d,
+                                            float *v_log_scales, float *v_raw_quats, float *v_opacity_logits,
+                                            int accumulate, int antialiased, int camgrad, float *cam_partials,
+                                            gsb_stream_t stream);
+size_t gsb_filter3d_workspace_bytes(void);
+int gsb_filter3d_compute(int n, const float *means, int num_cameras, const float *cameras, float near, float margin,
+                         float variance, void *workspace, size_t workspace_bytes, float *filter3d,
+                         gsb_stream_t stream);
+int gsb_filter3d_bake(int n, const float *log_scales, const float *opacity_logits, const float *filter3d,
+                      float *out_log_scales, float *out_opacity_logits, gsb_stream_t stream);
+int gsb_reset_opacity_filter3d(int n, float max_logit, float reset_value, const float *log_scales,
+                               const float *filter3d, float *opacities, float *exp_avg, float *exp_avg_sq,
+                               gsb_stream_t stream);
+
 /* ---- Training images (Camera::loadImage / Camera::getImage, input_data.cpp:40-117) --------------------------------
  * Images are 3-channel u8, [h,w,3] row-major and dense.
  * gsb_resize_area_u8 is cv::resize(src, dst, ..., INTER_AREA) of OpenCV 4's CPU code, byte for byte, for dst_h <= src_h and

@@ -30,6 +30,7 @@ SOURCES = {
     "bilagrid.cu": [],
     "pose.cu": [],
     "depth.cu": ["--fmad=false"],
+    "filter3d.cu": ["--fmad=false"],
     "export.cu": ["--fmad=false"],
     "knn.cu": ["--fmad=false"],
     "image.cu": ["--fmad=false"],

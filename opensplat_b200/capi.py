@@ -121,6 +121,21 @@ _SIGS = {
     "gsb_inverse_depth_l1": (_i, [_i, _i, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
     # h, w, factor, src, dst, stream
     "gsb_depth_downscale_mean": (_i, [_i, _i, _i, _vp, _vp, _vp]),
+    # D24: the arguments of gsb_project_forward_activated with filter3d after the logits, then antialiased, stream
+    "gsb_project_forward_activated_filter3d": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _i, _i,
+                                                    _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    # the arguments of gsb_project_backward_activated (logits for opac) with filter3d after the logits, then
+    # accumulate, antialiased, camgrad, cam_partials, stream
+    "gsb_project_backward_activated_filter3d": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
+                                                     _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i,
+                                                     _vp, _vp]),
+    "gsb_filter3d_workspace_bytes": (_sz, []),
+    # n, means, num_cameras, cameras, near, margin, variance, workspace, workspace_bytes, filter3d, stream
+    "gsb_filter3d_compute": (_i, [_i, _vp, _i, _vp, _f, _f, _f, _vp, _sz, _vp, _vp]),
+    # n, log_scales, logits, filter3d, out_log_scales, out_logits, stream
+    "gsb_filter3d_bake": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    # n, max_logit, reset_value, log_scales, filter3d, logits, exp_avg, exp_avg_sq, stream
+    "gsb_reset_opacity_filter3d": (_i, [_i, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_ply_row_floats": (_i, [_i]),
     "gsb_pack_ply_rows": (_i, [_i, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp]),
     "gsb_unpack_ply_rows": (_i, [_i, _i, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp]),
@@ -162,6 +177,7 @@ BILAGRID_X, BILAGRID_Y, BILAGRID_L, BILAGRID_COEFFS = 16, 16, 8, 12   # GSB_BILA
 BILAGRID_FLOATS = BILAGRID_L * BILAGRID_Y * BILAGRID_X * BILAGRID_COEFFS
 POSE_FLOATS = 9   # GSB_POSE_FLOATS
 CAMGRAD_TERMS = 24   # floats per block row of gsb_project_backward_activated_camgrad's partials
+FILTER3D_CAM_FLOATS = 18   # GSB_FILTER3D_CAM_FLOATS
 
 
 # optional symbols (experimental entry points) are bound when present

@@ -72,6 +72,20 @@ __device__ __forceinline__ void load_cam(const float *__restrict__ viewmat,
     for (int i = 0; i < 16; ++i) c.P[i] = __ldg(projmat + i);
 }
 
+// F3D (D24): sigma_k = sqrtf(s_k s_k + f f) from s_k = glob_scale e_k (e_k = expf(a_k)), r_k = s_k / sigma_k and
+// c3 = (r_0 r_1) r_2 -- the one fp32 order of the forward and the backward, so that f = 0 gives sigma = s, r = 1, c3 = 1
+__device__ __forceinline__ void filter3d_scales(float glob_scale, const float (&e)[3], float f, float (&sig)[3],
+                                                float (&r)[3], float &c3) {
+    const float ff = f * f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float s = glob_scale * e[k];
+        sig[k] = sqrtf(s * s + ff);
+        r[k] = s / sig[k];
+    }
+    c3 = r[0] * r[1] * r[2];
+}
+
 // ACT: the parameter activations of Model::forward (model.cpp:148-150,176-177,200) as this kernel's prologue --
 // `scales` holds log-scales (exp here), `quats` the raw quaternions (quat_to_rotmat normalises, as the reference's
 // does, so `quats / quats.norm()` needs no pass of its own), and sigmoid(opacity_logits) is written beside the
@@ -79,7 +93,10 @@ __device__ __forceinline__ void load_cam(const float *__restrict__ viewmat,
 // AA (with ACT only; DESIGN D19): the anti-aliased opacity -- sigmoid(logit) * comp, comp = sqrt(max(0, det0 / det)),
 // det0 the determinant of the screen covariance before the 0.3 px^2 blur and det the one after it, so the blurred
 // Gaussian carries the light of the unblurred one; comp = 0 where radii == 0.  Every other output is the ACT one.
-template <bool ACT, bool AA = false>
+// F3D (with ACT; DESIGN D24): Mip-Splatting's 3-D smoothing filter, f = filter3d[i] -- the covariance is built from
+// sigma_k = sqrtf(s_k s_k + f f) in place of s_k = glob_scale exp(a_k), and the opacity is sigmoid(logit) * c3 (then
+// x comp under AA), c3 = (r_0 r_1) r_2, r_k = s_k / sigma_k.  At f = 0, sigma = s, r = 1 and c3 = 1 exactly.
+template <bool ACT, bool AA = false, bool F3D = false>
 __global__ void __launch_bounds__(PJ_THREADS)
 project_forward_kernel(int n, const float *__restrict__ means3d, const float *__restrict__ scales,
                        float glob_scale, const float *__restrict__ quats,
@@ -88,11 +105,20 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
                        int tiles_x, int tiles_y, float clip_thresh, float *__restrict__ cov3d,
                        float2 *__restrict__ xys, float *__restrict__ depths, int *__restrict__ radii,
                        float *__restrict__ conics, int *__restrict__ num_tiles_hit,
-                       const float *__restrict__ opacity_logits, float *__restrict__ opacities) {
+                       const float *__restrict__ opacity_logits, float *__restrict__ opacities,
+                       const float *__restrict__ filter3d = nullptr) {
     static_assert(ACT || !AA, "the anti-aliased opacity needs the activated projection");
+    static_assert(ACT || !F3D, "the 3-D filter needs the activated projection");
     const int i = blockIdx.x * PJ_THREADS + threadIdx.x;
     if (i >= n) return;
-    if (ACT && !AA) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i]));
+    if (ACT && !AA && !F3D) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i]));
+    float fsig[3] = {0.f, 0.f, 0.f}, fc3 = 1.f;    // F3D: the filtered scales sigma_k and c3
+    if constexpr (F3D) {
+        const float e[3] = {expf(scales[3 * i]), expf(scales[3 * i + 1]), expf(scales[3 * i + 2])};
+        float r[3];
+        filter3d_scales(glob_scale, e, filter3d[i], fsig, r, fc3);
+        if (!AA) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i])) * fc3;
+    }
     float comp = 0.f;
     Cam cam;
     load_cam(viewmat, projmat, cam);
@@ -114,8 +140,9 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
         float R[3][3], M[3][3];
         quat_to_rotmat(q.x, q.y, q.z, q.w, R);
         const float a0 = scales[3 * i], a1 = scales[3 * i + 1], a2 = scales[3 * i + 2];
-        const float s0 = glob_scale * (ACT ? expf(a0) : a0), s1 = glob_scale * (ACT ? expf(a1) : a1),
-                    s2 = glob_scale * (ACT ? expf(a2) : a2);
+        const float s0 = F3D ? fsig[0] : glob_scale * (ACT ? expf(a0) : a0),
+                    s1 = F3D ? fsig[1] : glob_scale * (ACT ? expf(a1) : a1),
+                    s2 = F3D ? fsig[2] : glob_scale * (ACT ? expf(a2) : a2);
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
             M[r][0] = R[r][0] * s0;
@@ -189,7 +216,8 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
             }
         }
     }
-    if (AA) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i])) * comp;
+    if constexpr (AA && F3D) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i])) * fc3 * comp;
+    else if (AA) opacities[i] = 1.f / (1.f + expf(-opacity_logits[i])) * comp;
     float *c3o = cov3d + 6 * (size_t)i;
 #pragma unroll
     for (int k = 0; k < 6; ++k) c3o[k] = c3[k];
@@ -212,7 +240,11 @@ project_forward_kernel(int n, const float *__restrict__ means3d, const float *__
 // v_opacity * o of comp is taken to the blurred covariance and added to vS before the T / J / clamp chain.
 // CAMGRAD (with ACT; DESIGN D22): also the exact VJP w.r.t. viewmat and projmat, summed over the block's Gaussians
 // (camgrad_block_sum) into row blockIdx.x of cam_partials; every other output is the one without CAMGRAD, bit for bit.
-template <bool ACT, bool ACC, bool AA = false, bool CAMGRAD = false>
+// F3D (with ACT; DESIGN D24): VJP of the filtered forward with f = filter3d[i] held constant.  `opacities` holds the
+// logits, as under AA.  d sigma_k / d a_k = s_k r_k, so v_scale gains the factor r_k; the opacity (o c3 [comp]) adds
+// v_opacity * o_eff * (f / sigma_k)^2 to v_scale (written in that form, not 1 - r_k^2, which cancels for the small
+// Gaussians the filter is for), and v_logit = v_opacity * c3 [* comp] * o (1 - o).
+template <bool ACT, bool ACC, bool AA = false, bool CAMGRAD = false, bool F3D = false>
 __global__ void __launch_bounds__(PJ_THREADS)
 project_backward_kernel(int n, const float *__restrict__ means3d, const float *__restrict__ scales,
                         float glob_scale, const float *__restrict__ quats,
@@ -223,8 +255,10 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
                         const float *__restrict__ v_conic, float *__restrict__ v_mean3d,
                         float *__restrict__ v_scale, float4 *__restrict__ v_quat,
                         const float *__restrict__ opacities, const float *__restrict__ v_opacity,
-                        float *__restrict__ v_opacity_logits, float *__restrict__ cam_partials = nullptr) {
+                        float *__restrict__ v_opacity_logits, float *__restrict__ cam_partials = nullptr,
+                        const float *__restrict__ filter3d = nullptr) {
     static_assert(ACT || !AA, "the anti-aliased opacity needs the activated projection");
+    static_assert(ACT || !F3D, "the 3-D filter needs the activated projection");
     static_assert(ACT || !CAMGRAD, "the camera gradient is taken with the activated projection");
     const int i = blockIdx.x * PJ_THREADS + threadIdx.x;
     // CAMGRAD: every thread of the block takes part in the reduction, so none returns early
@@ -234,7 +268,11 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
     for (int k = 0; k < CG_TERMS; ++k) cg[k] = 0.f;
     if (!CAMGRAD || i < n) {
         float comp = 0.f;
-        if (ACT && !AA) {
+        // F3D: f, r_k and c3 as in the forward, and (f / sigma_k)^2 for the opacity's share of v_scale; computed
+        // inside the radii > 0 branch from its exp(a), or on their own where radii == 0
+        float f3 = 0.f, fr[3] = {1.f, 1.f, 1.f}, fc3 = 1.f, fsh[3] = {0.f, 0.f, 0.f};
+        if constexpr (F3D) f3 = filter3d[i];
+        if (ACT && !AA && !F3D) {
             const float o = opacities[i];
             if constexpr (ACC)
                 v_opacity_logits[i] = v_opacity_logits[i] + (v_opacity ? v_opacity[i] * o * (1.f - o) : 0.f);
@@ -282,7 +320,8 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
             quat_to_rotmat(q.x, q.y, q.z, q.w, R);
             const float a[3] = {scales[3 * i], scales[3 * i + 1], scales[3 * i + 2]};
             const float e[3] = {ACT ? expf(a[0]) : a[0], ACT ? expf(a[1]) : a[1], ACT ? expf(a[2]) : a[2]};
-            const float s[3] = {glob_scale * e[0], glob_scale * e[1], glob_scale * e[2]};
+            float s[3] = {glob_scale * e[0], glob_scale * e[1], glob_scale * e[2]};
+            if constexpr (F3D) filter3d_scales(glob_scale, e, f3, s, fr, fc3);
 #pragma unroll
             for (int r = 0; r < 3; ++r)
 #pragma unroll
@@ -324,7 +363,7 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
                     // 0.3 / det^2 [[cyy0^2 + cxy^2 + 0.3 cyy0, -cxy (cxx0 + cyy0 + 0.3)], [.., cxx0^2 + cxy^2 + 0.3 cxx0]]:
                     // the same value without the cancellation of the first form when Sigma0 is small against 0.3 I
                     const float o = 1.f / (1.f + expf(-opacities[i]));
-                    const float k = 0.5f * (v_opacity[i] * o) / comp;
+                    const float k = 0.5f * (v_opacity[i] * (F3D ? o * fc3 : o)) / comp;
                     const float id = 1.f / det;
                     const float a = cyy0 * id, b = cxy * id, c = cxx0 * id, e = 0.3f * id;
                     vS00 = vS00 + k * (0.3f * (a * a + b * b + e * a));
@@ -398,6 +437,7 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
             for (int c = 0; c < 3; ++c) {
                 vs[c] = glob_scale * (R[0][c] * vM[0][c] + R[1][c] * vM[1][c] + R[2][c] * vM[2][c]);
                 if (ACT) vs[c] = vs[c] * e[c];   // d exp(a) = exp(a)
+                if (F3D) vs[c] = vs[c] * fr[c];  // d sigma / d s = r
             }
             float vR[3][3];
 #pragma unroll
@@ -417,12 +457,36 @@ project_backward_kernel(int n, const float *__restrict__ means3d, const float *_
             const float dot = w * gw + x * gx + y * gy + z * gz;
             vq = make_float4((gw - w * dot) * inv, (gx - x * dot) * inv, (gy - y * dot) * inv,
                              (gz - z * dot) * inv);
+            if constexpr (F3D) {
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { const float t = f3 / s[k]; fsh[k] = t * t; }
+            }
+        } else if constexpr (F3D) {
+            const float e[3] = {expf(scales[3 * i]), expf(scales[3 * i + 1]), expf(scales[3 * i + 2])};
+            float sg[3];
+            filter3d_scales(glob_scale, e, f3, sg, fr, fc3);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) { const float t = f3 / sg[k]; fsh[k] = t * t; }
         }
-        if constexpr (AA) {
+        if constexpr (AA && !F3D) {
             float vol = 0.f;
             if (v_opacity) {
                 const float o = 1.f / (1.f + expf(-opacities[i]));
                 vol = v_opacity[i] * comp * o * (1.f - o);
+            }
+            v_opacity_logits[i] = ACC ? v_opacity_logits[i] + vol : vol;
+        }
+        if constexpr (F3D) {
+            float vol = 0.f;
+            if (v_opacity) {
+                const float o = 1.f / (1.f + expf(-opacities[i]));
+                vol = AA ? v_opacity[i] * fc3 * comp * o * (1.f - o) : v_opacity[i] * fc3 * o * (1.f - o);
+                if (f3 > 0.f) {
+                    // d c3 / d a_k = c3 (f / sigma_k)^2: the opacity's share of v_scale, for every Gaussian
+                    const float vo = v_opacity[i] * (AA ? o * fc3 * comp : o * fc3);
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) vs[k] = vs[k] + vo * fsh[k];
+                }
             }
             v_opacity_logits[i] = ACC ? v_opacity_logits[i] + vol : vol;
         }
@@ -465,7 +529,8 @@ camgrad_reduce_kernel(int nblocks, const float *__restrict__ partials, float *__
 }  // namespace
 
 static int project_forward_impl(bool act, bool aa, int n, const float *means3d, const float *scales, float glob_scale,
-                                const float *quats, const float *opacity_logits, const float *viewmat,
+                                const float *quats, const float *opacity_logits, const float *filter3d,
+                                const float *viewmat,
                                 const float *projmat, float fx, float fy, float cx, float cy, int img_h, int img_w,
                                 int tiles_x, int tiles_y, float clip_thresh, float *cov3d, float *xys, float *depths,
                                 int32_t *radii, float *conics, int32_t *num_tiles_hit, float *opacities,
@@ -479,11 +544,13 @@ static int project_forward_impl(bool act, bool aa, int n, const float *means3d, 
     // forward.cu:69-70 evaluates `0.5 * img_size.x / fx` in double and narrows
     const float tan_fovx = (float)(0.5 * (double)img_w / (double)fx);
     const float tan_fovy = (float)(0.5 * (double)img_h / (double)fy);
-#define GSB_PJ_F(A, AA) project_forward_kernel<A, AA><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
+#define GSB_PJ_F(A, AA, F3D) project_forward_kernel<A, AA, F3D><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
         n, means3d, scales, glob_scale, quats, viewmat, projmat, fx, fy, cx, cy, tan_fovx, tan_fovy, img_h, img_w,   \
         tiles_x, tiles_y, clip_thresh, cov3d, reinterpret_cast<float2 *>(xys), depths, radii, conics, num_tiles_hit, \
-        opacity_logits, opacities)
-    if (aa) GSB_PJ_F(true, true); else if (act) GSB_PJ_F(true, false); else GSB_PJ_F(false, false);
+        opacity_logits, opacities, filter3d)
+    if (filter3d) { if (aa) GSB_PJ_F(true, true, true); else GSB_PJ_F(true, false, true); }
+    else if (aa) GSB_PJ_F(true, true, false); else if (act) GSB_PJ_F(true, false, false);
+    else GSB_PJ_F(false, false, false);
 #undef GSB_PJ_F
     GSB_LAUNCH_CHECK();
     return 0;
@@ -495,7 +562,7 @@ extern "C" int gsb_project_forward(int n, const float *means3d, const float *sca
                                    int tiles_x, int tiles_y, float clip_thresh, float *cov3d, float *xys,
                                    float *depths, int32_t *radii, float *conics, int32_t *num_tiles_hit,
                                    gsb_stream_t stream) {
-    return project_forward_impl(false, false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx, fy, cx,
+    return project_forward_impl(false, false, n, means3d, scales, glob_scale, quats, nullptr, nullptr, viewmat, projmat, fx, fy, cx,
                                 cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii, conics,
                                 num_tiles_hit, nullptr, stream);
 }
@@ -507,7 +574,7 @@ extern "C" int gsb_project_forward_activated(int n, const float *means3d, const 
                                              float clip_thresh, float *cov3d, float *xys, float *depths,
                                              int32_t *radii, float *conics, int32_t *num_tiles_hit,
                                              float *opacities, gsb_stream_t stream) {
-    return project_forward_impl(true, false, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, viewmat, projmat,
+    return project_forward_impl(true, false, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, nullptr, viewmat, projmat,
                                 fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii,
                                 conics, num_tiles_hit, opacities, stream);
 }
@@ -517,7 +584,8 @@ static int project_backward_impl(bool act, bool acc, bool aa, int n, const float
                                  const float *projmat, float fx, float fy, int img_h, int img_w,
                                  const int32_t *radii, const float *conics, const float *v_xy, const float *v_depth,
                                  const float *v_conic, const float *v_opacity, float *v_mean3d, float *v_scale,
-                                 float *v_quat, float *v_opacity_logits, float *cam_partials, gsb_stream_t stream) {
+                                 float *v_quat, float *v_opacity_logits, float *cam_partials, gsb_stream_t stream,
+                                 const float *filter3d = nullptr) {
     GSB_CHECK_ARG(n >= 0 && img_h > 0 && img_w > 0);
     if (n == 0) return 0;
     GSB_CHECK_ARG(means3d && scales && quats && viewmat && projmat && radii && conics && v_xy && v_conic &&
@@ -526,17 +594,27 @@ static int project_backward_impl(bool act, bool acc, bool aa, int n, const float
     GSB_CHECK_ARG(((uintptr_t)quats % 16) == 0 && ((uintptr_t)v_quat % 16) == 0 && ((uintptr_t)v_xy % 8) == 0);
     const float tan_fovx = (float)(0.5 * (double)img_w / (double)fx);
     const float tan_fovy = (float)(0.5 * (double)img_h / (double)fy);
-#define GSB_PJ_B(A, ACC, AA, CG) project_backward_kernel<A, ACC, AA, CG><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
+#define GSB_PJ_B5(A, ACC, AA, CG, F3D) project_backward_kernel<A, ACC, AA, CG, F3D><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
         n, means3d, scales, glob_scale, quats, viewmat, projmat, fx, fy, tan_fovx, tan_fovy, img_h, img_w, radii,     \
         conics, reinterpret_cast<const float2 *>(v_xy), v_depth, v_conic, v_mean3d, v_scale,                          \
-        reinterpret_cast<float4 *>(v_quat), opacities, v_opacity, v_opacity_logits, cam_partials)
-    if (cam_partials) {
+        reinterpret_cast<float4 *>(v_quat), opacities, v_opacity, v_opacity_logits, cam_partials, filter3d)
+#define GSB_PJ_B(A, ACC, AA, CG) GSB_PJ_B5(A, ACC, AA, CG, false)
+#define GSB_PJ_BF(ACC, AA, CG) GSB_PJ_B5(true, ACC, AA, CG, true)
+    if (filter3d) {
+        if (cam_partials) {
+            if (aa) { if (acc) GSB_PJ_BF(true, true, true); else GSB_PJ_BF(false, true, true); }
+            else if (acc) GSB_PJ_BF(true, false, true); else GSB_PJ_BF(false, false, true);
+        } else if (aa) { if (acc) GSB_PJ_BF(true, true, false); else GSB_PJ_BF(false, true, false); }
+        else if (acc) GSB_PJ_BF(true, false, false); else GSB_PJ_BF(false, false, false);
+    } else if (cam_partials) {
         if (aa) { if (acc) GSB_PJ_B(true, true, true, true); else GSB_PJ_B(true, false, true, true); }
         else if (acc) GSB_PJ_B(true, true, false, true); else GSB_PJ_B(true, false, false, true);
     } else if (aa) { if (acc) GSB_PJ_B(true, true, true, false); else GSB_PJ_B(true, false, true, false); }
     else if (acc) GSB_PJ_B(true, true, false, false); else if (act) GSB_PJ_B(true, false, false, false);
     else GSB_PJ_B(false, false, false, false);
+#undef GSB_PJ_BF
 #undef GSB_PJ_B
+#undef GSB_PJ_B5
     GSB_LAUNCH_CHECK();
     return 0;
 }
@@ -586,7 +664,7 @@ extern "C" int gsb_project_forward_activated_aa(int n, const float *means3d, con
                                                 float clip_thresh, float *cov3d, float *xys, float *depths,
                                                 int32_t *radii, float *conics, int32_t *num_tiles_hit,
                                                 float *opacities, gsb_stream_t stream) {
-    return project_forward_impl(true, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, viewmat,
+    return project_forward_impl(true, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, nullptr, viewmat,
                                 projmat, fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys,
                                 depths, radii, conics, num_tiles_hit, opacities, stream);
 }
@@ -648,4 +726,43 @@ extern "C" int gsb_project_camera_grad_reduce(int nblocks, const float *partials
     camgrad_reduce_kernel<<<1, CG_TERMS * 32, 0, (cudaStream_t)stream>>>(nblocks, partials, v_viewmat, v_projmat);
     GSB_LAUNCH_CHECK();
     return 0;
+}
+
+// D24: the activated projection with Mip-Splatting's 3-D filter (filter3d [n], one float per Gaussian), plain or
+// anti-aliased.
+extern "C" int gsb_project_forward_activated_filter3d(int n, const float *means3d, const float *log_scales,
+                                                      float glob_scale, const float *raw_quats,
+                                                      const float *opacity_logits, const float *filter3d,
+                                                      const float *viewmat, const float *projmat, float fx, float fy,
+                                                      float cx, float cy, int img_h, int img_w, int tiles_x,
+                                                      int tiles_y, float clip_thresh, float *cov3d, float *xys,
+                                                      float *depths, int32_t *radii, float *conics,
+                                                      int32_t *num_tiles_hit, float *opacities, int antialiased,
+                                                      gsb_stream_t stream) {
+    GSB_CHECK_ARG(antialiased == 0 || antialiased == 1);
+    GSB_CHECK_ARG(n >= 0 && (n == 0 || filter3d));
+    return project_forward_impl(true, antialiased != 0, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
+                                filter3d, viewmat, projmat, fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y,
+                                clip_thresh, cov3d, xys, depths, radii, conics, num_tiles_hit, opacities, stream);
+}
+
+// Its VJP with filter3d held constant, from the opacity logits: written or accumulated, plain or anti-aliased, with
+// or without the camera gradient (camgrad = 1: cam_partials as gsb_project_backward_activated_camgrad's).
+extern "C" int gsb_project_backward_activated_filter3d(int n, const float *means3d, const float *log_scales,
+                                                       float glob_scale, const float *raw_quats,
+                                                       const float *opacity_logits, const float *filter3d,
+                                                       const float *viewmat, const float *projmat, float fx, float fy,
+                                                       int img_h, int img_w, const int32_t *radii,
+                                                       const float *conics, const float *v_xy, const float *v_depth,
+                                                       const float *v_conic, const float *v_opacity, float *v_mean3d,
+                                                       float *v_log_scales, float *v_raw_quats,
+                                                       float *v_opacity_logits, int accumulate, int antialiased,
+                                                       int camgrad, float *cam_partials, gsb_stream_t stream) {
+    GSB_CHECK_ARG((accumulate == 0 || accumulate == 1) && (antialiased == 0 || antialiased == 1) &&
+                  (camgrad == 0 || camgrad == 1));
+    GSB_CHECK_ARG(n >= 0 && (n == 0 || (filter3d && (!camgrad || cam_partials))));
+    return project_backward_impl(true, accumulate != 0, antialiased != 0, n, means3d, log_scales, glob_scale,
+                                 raw_quats, opacity_logits, viewmat, projmat, fx, fy, img_h, img_w, radii, conics,
+                                 v_xy, v_depth, v_conic, v_opacity, v_mean3d, v_log_scales, v_raw_quats,
+                                 v_opacity_logits, camgrad ? cam_partials : nullptr, stream, filter3d);
 }

@@ -624,18 +624,20 @@ class ProjectGaussiansActivated(torch.autograd.Function):
     Gradients come back w.r.t. the raw parameters, and w.r.t. viewMat and projMat when those require grad (DESIGN
     D22: the exact VJP summed over the visible Gaussians, reduced inside the projection backward; row 3 of the
     viewMat gradient and row 2 of the projMat gradient are 0, as the projection does not read them).  C++ twin:
-    gsb::ProjectGaussiansActivated (without the camera gradient)."""
+    gsb::ProjectGaussiansActivated (without the camera gradient).  filter3D (DESIGN D24): an optional [N] float32
+    3-D filter (filter3d.compute_filter3d), held constant: the covariance is built from sqrt(exp(a)^2 globScale^2 + f^2)
+    and the opacity is multiplied by c3; without it the operator runs exactly as before."""
 
     @staticmethod
     def forward(ctx, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat, fx, fy, cx, cy,
-                imgHeight, imgWidth, tileBounds, clipThresh=0.01):
+                imgHeight, imgWidth, tileBounds, clipThresh=0.01, filter3D=None):
         return ProjectGaussiansActivated._forward(ctx, False, means, logScales, globScale, rawQuats, opacityLogits,
                                                   viewMat, projMat, fx, fy, cx, cy, imgHeight, imgWidth, tileBounds,
-                                                  clipThresh)
+                                                  clipThresh, filter3D)
 
     @staticmethod
     def _forward(ctx, aa, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat, fx, fy, cx, cy,
-                 imgHeight, imgWidth, tileBounds, clipThresh):
+                 imgHeight, imgWidth, tileBounds, clipThresh, filter3D=None):
         n = means.shape[0]
         m3, ls, rq = capi.f32(means), capi.f32(logScales), capi.f32(rawQuats)
         ol = capi.f32(opacityLogits).reshape(n)
@@ -648,21 +650,31 @@ class ProjectGaussiansActivated(torch.autograd.Function):
         nth = _empty((n,), torch.int32, m3)
         opac = _empty((n, 1), torch.float32, m3)
         L = capi.lib()
-        capi.check((L.gsb_project_forward_activated_aa if aa else L.gsb_project_forward_activated)(
-            n, capi.ptr(m3), capi.ptr(ls), float(globScale), capi.ptr(rq), capi.ptr(ol), capi.ptr(vm), capi.ptr(pm),
-            float(fx), float(fy), float(cx), float(cy), int(imgHeight), int(imgWidth), tileBounds[0], tileBounds[1],
-            float(clipThresh), capi.ptr(cov3d), capi.ptr(xys), capi.ptr(depths), capi.ptr(radii), capi.ptr(conics),
-            capi.ptr(nth), capi.ptr(opac), capi.stream()))
+        f3 = None
+        if filter3D is not None:
+            # D24: the 3-D filter, a constant [N] float32 (no gradient)
+            if filter3D.dtype != torch.float32 or tuple(filter3D.shape) != (n,) or filter3D.device != m3.device:
+                raise ValueError(f"filter3D must be a float32 [{n}] tensor on the means' device")
+            f3 = filter3D.detach().contiguous()
+        args = (n, capi.ptr(m3), capi.ptr(ls), float(globScale), capi.ptr(rq), capi.ptr(ol))
+        rest = (capi.ptr(vm), capi.ptr(pm), float(fx), float(fy), float(cx), float(cy), int(imgHeight),
+                int(imgWidth), tileBounds[0], tileBounds[1], float(clipThresh), capi.ptr(cov3d), capi.ptr(xys),
+                capi.ptr(depths), capi.ptr(radii), capi.ptr(conics), capi.ptr(nth), capi.ptr(opac))
+        if f3 is None:
+            capi.check((L.gsb_project_forward_activated_aa if aa else L.gsb_project_forward_activated)(
+                *args, *rest, capi.stream()))
+        else:
+            capi.check(L.gsb_project_forward_activated_filter3d(*args, capi.ptr(f3), *rest, int(aa), capi.stream()))
         ctx.meta = (float(globScale), float(fx), float(fy), int(imgHeight), int(imgWidth), tuple(opacityLogits.shape),
                     aa, tuple(viewMat.shape), tuple(projMat.shape))
-        # the plain backward takes sigmoid(logits) from the forward, the anti-aliased one the logits themselves
-        ctx.save_for_backward(m3, ls, rq, vm, pm, radii, conics, ol if aa else opac)
+        # the plain backward takes sigmoid(logits) from the forward, the anti-aliased and filtered ones the logits
+        ctx.save_for_backward(m3, ls, rq, vm, pm, radii, conics, ol if (aa or f3 is not None) else opac, f3)
         ctx.mark_non_differentiable(radii, nth)
         return xys, depths, radii, conics, nth, cov3d, opac
 
     @staticmethod
     def backward(ctx, v_xys, v_depths, v_radii, v_conics, v_numTiles, v_cov3d, v_opac):
-        m3, ls, rq, vm, pm, radii, conics, opac = ctx.saved_tensors
+        m3, ls, rq, vm, pm, radii, conics, opac, f3 = ctx.saved_tensors
         gs, fx, fy, H, W, ol_shape, aa, vm_shape, pm_shape = ctx.meta
         n = m3.shape[0]
         if v_xys is None:
@@ -681,21 +693,29 @@ class ProjectGaussiansActivated(torch.autograd.Function):
                 W, capi.ptr(radii), capi.ptr(conics), capi.ptr(vx), capi.ptr(vd), capi.ptr(vc), capi.ptr(vo),
                 capi.ptr(v_mean), capi.ptr(v_ls), capi.ptr(v_rq), capi.ptr(v_ol))
         v_view = v_proj = None
-        if ctx.needs_input_grad[5] or ctx.needs_input_grad[6]:
+        camgrad = ctx.needs_input_grad[5] or ctx.needs_input_grad[6]
+        if f3 is not None:
+            # D24: opac holds the logits; the filter sits after them in the argument list
+            fargs = args[:6] + (capi.ptr(f3),) + args[6:]
+            part = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, m3) if camgrad else None
+            capi.check(L.gsb_project_backward_activated_filter3d(*fargs, 0, int(aa), int(camgrad), capi.ptr(part),
+                                                                 capi.stream()))
+        if camgrad:
             # D22: the camera gradient, reduced over the Gaussians inside the projection backward
-            part = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, m3)
             v_view = _empty((4, 4), torch.float32, m3)
             v_proj = _empty((4, 4), torch.float32, m3)
-            capi.check(L.gsb_project_backward_activated_camgrad(*args, 0, int(aa), capi.ptr(part), capi.stream()))
+            if f3 is None:
+                part = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, m3)
+                capi.check(L.gsb_project_backward_activated_camgrad(*args, 0, int(aa), capi.ptr(part), capi.stream()))
             capi.check(L.gsb_project_camera_grad_reduce(part.numel() // capi.CAMGRAD_TERMS, capi.ptr(part),
                                                         capi.ptr(v_view), capi.ptr(v_proj), capi.stream()))
             v_view = v_view.reshape(vm_shape) if ctx.needs_input_grad[5] else None
             v_proj = v_proj.reshape(pm_shape) if ctx.needs_input_grad[6] else None
-        else:
+        elif f3 is None:
             capi.check((L.gsb_project_backward_activated_aa if aa else L.gsb_project_backward_activated)(
                 *args, capi.stream()))
-        # 15 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4), viewMat(5), projMat(6)
-        return (v_mean, v_ls, None, v_rq, v_ol.reshape(ol_shape), v_view, v_proj) + (None,) * 8
+        # 16 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4), viewMat(5), projMat(6)
+        return (v_mean, v_ls, None, v_rq, v_ol.reshape(ol_shape), v_view, v_proj) + (None,) * 9
 
 
 class ProjectGaussiansActivatedAntialiased(ProjectGaussiansActivated):
@@ -707,10 +727,10 @@ class ProjectGaussiansActivatedAntialiased(ProjectGaussiansActivated):
 
     @staticmethod
     def forward(ctx, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat, fx, fy, cx, cy,
-                imgHeight, imgWidth, tileBounds, clipThresh=0.01):
+                imgHeight, imgWidth, tileBounds, clipThresh=0.01, filter3D=None):
         return ProjectGaussiansActivated._forward(ctx, True, means, logScales, globScale, rawQuats, opacityLogits,
                                                   viewMat, projMat, fx, fy, cx, cy, imgHeight, imgWidth, tileBounds,
-                                                  clipThresh)
+                                                  clipThresh, filter3D)
 
 
 class SphericalHarmonics(torch.autograd.Function):

@@ -80,7 +80,14 @@ tiles still sorted by z; the colour is the same bits), takes the masked L1 again
 (gsb_inverse_depth_l1, weighted by depth.depth_weight), and its backward adds the depth term to the blend's geometry
 gradients and, through gsb_inverse_depths_backward, to the projection's depth; densification statistics and a pose
 correction's gradient see it too.  A view without one issues exactly the launches of a plain trainer.  The loss
-returned stays the image loss; `depth_losses` holds the unweighted depth loss of each view."""
+returned stays the image loss; `depth_losses` holds the unweighted depth loss of each view.
+
+With Mip-Splatting's 3-D smoothing filter (`filter3d=filter3d.Filter3DConfig(cameras=...)`, DESIGN D24) every
+projection, forward and backward, in step(), evaluate() and render(), takes the per-Gaussian filter f
+(gsb_project_*_activated_filter3d).  f is computed from the training cameras, uploaded once, at construction, after
+every step whose refinement ran and on filter3d.recompute_due's schedule once refinement has stopped; the alpha reset
+clamps the effective opacity, and save() writes the baked scene.  With pose corrections f uses the cameras as given,
+uncorrected.  Under a group every rank computes the same f from the same cameras (no collective)."""
 import ctypes as C
 
 import torch
@@ -91,6 +98,7 @@ from .export import SceneWriter
 from .appearance import Appearance, to_gsplat_order
 from .pose import Poses
 from .depth import DepthConfig, depth_weight
+from .filter3d import Filter3DConfig, bake, camera_table, compute_filter3d, recompute_due
 from .mcmc import MCMCConfig, MCMCRefiner
 from .model import (LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, Camera, camera_setup, downscale_factor,
                     means_learning_rate)
@@ -171,7 +179,7 @@ class SplatTrainer:
     def __init__(self, params, cfg=None, sh_degree=None, sh_degree_interval=1000, num_downscales=0,
                  resolution_schedule=3000, background=(0.6130, 0.0101, 0.3984), device="cuda:0", generator=None,
                  ssim_weight=0.2, m_capacity=None, group=None, views_per_step=1, antialiased=False,
-                 appearance=None, pose=None, depth=None):
+                 appearance=None, pose=None, depth=None, filter3d=None):
         """params: dict with the reference's six tensors (means [n,3], scales [n,3] log, quats [n,4] raw,
         featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
         cfg: densify.RefineConfig (the reference's refinement, the default) or mcmc.MCMCConfig (3DGS-MCMC under a
@@ -187,7 +195,9 @@ class SplatTrainer:
         pose: a pose.PoseConfig to learn one camera pose correction per training image (DESIGN D22); step() then takes
         image=, and evaluate() / render() may.  Not available with group=; with appearance=, num_images must agree.
         depth: a depth.DepthConfig to supervise the rendered inverse depth with per-image priors (DESIGN D23); step()
-        then takes depth=."""
+        then takes depth=.
+        filter3d: a filter3d.Filter3DConfig to train and render with Mip-Splatting's 3-D smoothing filter (DESIGN
+        D24) from its training cameras; save() then writes the baked scene."""
         import torch.distributed as dist
         self.views_per_step = B = int(views_per_step)
         if B < 1:
@@ -204,7 +214,10 @@ class SplatTrainer:
                              f"{appearance.num_images} and {pose.num_images}")
         if depth is not None and not isinstance(depth, DepthConfig):
             raise ValueError("depth= takes a depth.DepthConfig")
+        if filter3d is not None and not isinstance(filter3d, Filter3DConfig):
+            raise ValueError("filter3d= takes a filter3d.Filter3DConfig")
         self.depth = depth
+        self.filter3d_cfg = filter3d
         self.device = torch.device(device)
         self.cfg = cfg or RefineConfig()
         self.antialiased = bool(antialiased)
@@ -262,7 +275,12 @@ class SplatTrainer:
             # symmetric gradient buffer + colour slots + trailers; SplatPipeline.resize_gaussians rebuilds them after a
             # refinement
             pp.exchange = self.exchange = ViewParallelExchange(pp, group=group, views_per_rank=B)
+        if filter3d is not None:   # D24: the training cameras, uploaded once, and the compute's workspace
+            self.f3d_cams = camera_table(filter3d.cameras, self.device)
+            self.f3d_ws = torch.empty(self.L.gsb_filter3d_workspace_bytes(), dtype=torch.uint8, device=self.device)
         self._alloc_gaussian_scratch()
+        if filter3d is not None:
+            self._compute_filter3d()
 
     def _alloc_gaussian_scratch(self):
         """The trainer's per-Gaussian buffers, (re)built at construction and after a refinement."""
@@ -289,6 +307,8 @@ class SplatTrainer:
             floats = self.L.gsb_project_camera_partials_floats(n)
             self.cam_blocks = floats // capi.CAMGRAD_TERMS
             self.cam_partials = torch.empty(max(floats, 1), dtype=torch.float32, device=d)
+        if self.filter3d_cfg is not None:   # D24: the 3-D filter, recomputed after every refinement
+            self.f3d = torch.empty(n, dtype=torch.float32, device=d)
         if self.depth is not None:   # D23: 1/z where radii > 0, its blend gradient, and the projection's v_depth
             self.inv_depths = torch.empty(n, dtype=torch.float32, device=d)
             self.v_inv_depths = torch.empty(n, dtype=torch.float32, device=d)
@@ -337,6 +357,25 @@ class SplatTrainer:
         if self.appearance is None:
             raise ValueError("this trainer has no appearance grids")
         return to_gsplat_order(self.appearance.grids)
+
+    def filter3d(self):
+        """A copy of the 3-D filter, [n] float32 (D24)."""
+        if self.filter3d_cfg is None:
+            raise ValueError("this trainer has no 3-D filter")
+        return self.f3d.clone()
+
+    def _filter3d_of(self, means):
+        """D24: the 3-D filter of `means` from the trainer's cameras, into a new tensor."""
+        c = self.filter3d_cfg
+        return compute_filter3d(means, self.f3d_cams, c.variance, c.near, c.margin)
+
+    def _compute_filter3d(self):
+        """D24: recompute the trainer's filter buffer from the current means."""
+        pp, c = self.pipe, self.filter3d_cfg
+        capi.check(self.L.gsb_filter3d_compute(pp.n, capi.ptr(pp.p["means"]), self.f3d_cams.shape[0],
+                                               capi.ptr(self.f3d_cams), c.near, c.margin, c.variance,
+                                               capi.ptr(self.f3d_ws), self.f3d_ws.numel(), capi.ptr(self.f3d),
+                                               capi.stream()))
 
     def pose_deltas(self):
         """A copy of the pose corrections, [num_images, 9]: translation e[0:3] and 6-D rotation offset e[3:9] per
@@ -446,9 +485,13 @@ class SplatTrainer:
         elif trains:
             # ---- the rest of Model::afterTrain on views into the flat buffers ----
             self._adopt(*self.densifier.finish_step(step, pp.p, flat_views(pp.adam_m, pp.offs),
-                                                    flat_views(pp.adam_v, pp.offs), H, W))
+                                                    flat_views(pp.adam_v, pp.offs), H, W,
+                                                    filter3d=None if self.filter3d_cfg is None else self._filter3d_of))
         else:
             self.last_info = {"refined": False}
+        if self.filter3d_cfg is not None and recompute_due(self.cfg, self.filter3d_cfg, step,
+                                                           self.last_info["refined"]):
+            self._compute_filter3d()
         return self.losses[0] if B == 1 else self.losses
 
     def evaluate(self, cam, gt, step, image=None):
@@ -543,11 +586,14 @@ class SplatTrainer:
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         n, p, tb, H, W = pp.n, pp.p, pp.tb, pp.H, pp.W
         fx, fy, cx, cy = intr
-        project = L.gsb_project_forward_activated_aa if self.antialiased else L.gsb_project_forward_activated
-        capi.check(project(
-            n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]), P(self.viewmats[b]),
-            P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d), P(pp.xys), P(pp.depths),
-            P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac), s))
+        head = (n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]))
+        tail = (P(self.viewmats[b]), P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d),
+                P(pp.xys), P(pp.depths), P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac))
+        if self.filter3d_cfg is not None:     # D24
+            capi.check(L.gsb_project_forward_activated_filter3d(*head, P(self.f3d), *tail, int(self.antialiased), s))
+        else:
+            project = L.gsb_project_forward_activated_aa if self.antialiased else L.gsb_project_forward_activated
+            capi.check(project(*head, *tail, s))
         if prior:
             capi.check(L.gsb_inverse_depths(n, P(pp.depths), P(pp.radii), P(self.inv_depths), s))
             out_depth, out_alpha = self.depth_render, self.depth_alpha
@@ -611,7 +657,7 @@ class SplatTrainer:
         if ex is not None and ex.overlap and b == self.views_per_step - 1:
             # every colour slot is final: colour pulls + SH expansion start now, on a side stream
             ex.start_colour(degrees_to_use=use, rgbs=self.rgbs_views)
-        if self.antialiased:     # D19: the backward recomputes o and comp from the logits
+        if self.antialiased or self.filter3d_cfg is not None:     # D19, D24: the backward recomputes o from the logits
             pj = L.gsb_project_backward_activated_aa if b == 0 else L.gsb_project_backward_activated_aa_acc
             opac = p["opacities"]
         else:
@@ -620,12 +666,19 @@ class SplatTrainer:
         args = (n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(opac), P(self.viewmats[b]),
                 P(self.projmats[b]), fx, fy, pp.H, pp.W, P(pp.radii), P(pp.conics), P(pp.v_xy), P(v_depth),
                 P(pp.v_conic), P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]))
-        if self.poses is None:
-            capi.check(pj(*args, capi.stream()))
+        s, po = capi.stream(), self.poses
+        if self.filter3d_cfg is not None:     # D24: the filter after the logits; accumulate, antialiased, camgrad
+            capi.check(L.gsb_project_backward_activated_filter3d(
+                *args[:6], P(self.f3d), *args[6:], int(b > 0), int(self.antialiased), int(po is not None),
+                P(self.cam_partials) if po is not None else None, s))
+        elif po is None:
+            capi.check(pj(*args, s))
+        else:
+            capi.check(L.gsb_project_backward_activated_camgrad(*args, int(b > 0), int(self.antialiased),
+                                                                P(self.cam_partials), s))
+        if po is None:
             return
-        s, po, cg = capi.stream(), self.poses, self.cam_grads
-        capi.check(L.gsb_project_backward_activated_camgrad(*args, int(b > 0), int(self.antialiased),
-                                                            P(self.cam_partials), s))
+        cg = self.cam_grads
         capi.check(L.gsb_project_camera_grad_reduce(self.cam_blocks, P(self.cam_partials), P(cg[0]), P(cg[1]), s))
         capi.check(L.gsb_pose_backward(P(po.deltas[image]), P(self.base_viewmats[b]), P(self.projs[b]), P(cg[0]),
                                        P(cg[1]), 1.0 / self.views_per_step, P(po.grad[image]), s))
@@ -676,9 +729,15 @@ class SplatTrainer:
 
     # ---- Model::save (model.cpp:496-594) -----------------------------------------------------------------------
     def save(self, filename, step=0, keep_crs=False, scale=1.0, translation=(0.0, 0.0, 0.0), wait=True):
-        """Writes the scene as GaussianModel.save does, packing the rows straight from the flat buffer."""
+        """Writes the scene as GaussianModel.save does, packing the rows straight from the flat buffer.  With the 3-D
+        filter (D24) it writes the baked scene (filter3d.bake): log-scales log(e^2 + f^2) / 2 and logits
+        logit(sigmoid(l) c3), so any 3DGS viewer renders what was trained; loading that file into a filtered trainer
+        would apply the filter a second time."""
         if self.writer is None:
             self.writer = SceneWriter(self.device)
-        self.writer.save(filename, dict(self.pipe.p), step, keep_crs, scale, translation)
+        params = dict(self.pipe.p)
+        if self.filter3d_cfg is not None:
+            params = bake(params, self.f3d)
+        self.writer.save(filename, params, step, keep_crs, scale, translation)
         if wait:
             self.writer.wait()
