@@ -330,7 +330,15 @@ int gsb_bucket_sort_pack(int n, int m_capacity, int len_capacity, const float *d
  *   gsb_rasterize_forward_packed's.
  * gsb_rasterize_backward_depth: gsb_rasterize_backward plus record_depths, v_output_depth [H,W] (NULL == zeros) and
  *   v_depths [n], written completely.  v_output_alpha is the cotangent of out_alpha.  Give it the records, final_Ts
- *   and final_idx of gsb_rasterize_forward_packed_depth (or of gsb_rasterize_forward_packed: they are the same). */
+ *   and final_idx of gsb_rasterize_forward_packed_depth (or of gsb_rasterize_forward_packed: they are the same).
+ * gsb_rasterize_backward_absgrad (DESIGN D25): the arguments of gsb_rasterize_backward_depth plus v_xy_abs [n,2]
+ *   (non-NULL, 8-byte aligned), written completely: per Gaussian the sum over its blended pixels of the absolute value
+ *   of each pixel's contribution to v_xy, component by component (AbsGS's absolute screen-space gradient, which
+ *   does not cancel across the Gaussian's centre as v_xy does).  Depth is on iff v_depths != NULL: then
+ *   record_depths and v_output_depth follow gsb_rasterize_backward_depth's rules, otherwise both must be NULL.  The
+ *   other outputs are bit-identical to those of gsb_rasterize_backward (without depth) or
+ *   gsb_rasterize_backward_depth (with depth); v_xy_abs is bit-reproducible run to run (no atomics).  Allocates
+ *   nothing. */
 size_t gsb_raster_records_bytes(int m);
 size_t gsb_raster_grad_rows_bytes(int m);
 int gsb_pack_records(int m, const int32_t *gaussian_ids_sorted, const int32_t *sorted_index, const float *xys,
@@ -364,6 +372,14 @@ int gsb_rasterize_backward_depth(int img_h, int img_w, int tiles_x, int tiles_y,
                                  float *v_conic, float *v_colors, float *v_opacity, unsigned flags,
                                  const float *record_depths, const float *v_output_depth, float *v_depths,
                                  gsb_stream_t stream);
+int gsb_rasterize_backward_absgrad(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
+                                   const int32_t *tile_bins, const int32_t *tile_order, const float *conics,
+                                   const float *opacities, void *records, const int32_t *cum_tiles_hit,
+                                   const float *background, const float *final_Ts, const int32_t *final_idx,
+                                   const float *v_output, const float *v_output_alpha, void *grad_rows, float *v_xy,
+                                   float *v_conic, float *v_colors, float *v_opacity, unsigned flags,
+                                   const float *record_depths, const float *v_output_depth, float *v_depths,
+                                   float *v_xy_abs, gsb_stream_t stream);
 
 /* ---- Streaming helpers around the path (SURVEY.md 8f "next" rows) ------------------------------
  * gsb_mse_loss_grad: loss = mean((img-target)^2) written to *loss_out (device float; zeroed by the

@@ -71,6 +71,9 @@ _SIGS = {
                                                 _vp, _vp, _vp, _vp]),
     "gsb_rasterize_backward_depth": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                           _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint, _vp, _vp, _vp, _vp]),
+    # D25: the arguments of gsb_rasterize_backward_depth with v_xy_abs before the stream
+    "gsb_rasterize_backward_absgrad": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                            _vp, _vp, _vp, _vp, _vp, _vp, C.c_uint, _vp, _vp, _vp, _vp, _vp]),
     "gsb_bucket_max_tile_len": (_i, []),
     "gsb_bucket_workspace_bytes": (_sz, [_i, _i, _i]),
     "gsb_bucket_tile_ranges": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),

@@ -47,8 +47,17 @@ constexpr int BWD_MIN_BLOCKS = 6;
 // per pair d += z v_depth (nothing is added to Bq's initial value) and a tenth reduced value a_z = sum alpha T v_depth
 // goes to slot 9 of the gradient row.  v_output_depth may be NULL (zeros).
 constexpr int BWD_DEPTH_MIN_BLOCKS = 5;
-template <bool SAT, bool DEPTH>
-__global__ void __launch_bounds__(RK_THREADS, DEPTH ? BWD_DEPTH_MIN_BLOCKS : BWD_MIN_BLOCKS)
+// ABS: AbsGS's absolute screen-space gradient (D25).  Per pair the gradient of the 2-D mean is
+// g = -w (a dx + b dy, b dx + c dy); two more per-lane sums accumulate |w| |a dx + b dy| and |w| |b dx + c dy| and go
+// to slots 10 and 11 of the gradient row.  Everything else is computed as without ABS, in the same order.
+// ABS: 96 registers -> 5 CTAs per SM.  H100 SXM at 700 W, C2: 0.942 ms per launch against 1.009 ms with 4 (101
+// registers); at 6 it spills 48 B.  DEPTH + ABS: 113 registers -> 4 CTAs, the most without a spill (at 5 it spills 8 B;
+// 1.008 against 1.040 ms at C2, equal at C5)
+constexpr int BWD_ABS_MIN_BLOCKS = 5;
+constexpr int BWD_DEPTH_ABS_MIN_BLOCKS = 4;
+template <bool SAT, bool DEPTH, bool ABS>
+__global__ void __launch_bounds__(RK_THREADS, ABS ? (DEPTH ? BWD_DEPTH_ABS_MIN_BLOCKS : BWD_ABS_MIN_BLOCKS)
+                                                  : (DEPTH ? BWD_DEPTH_MIN_BLOCKS : BWD_MIN_BLOCKS))
 rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                           const int2 *__restrict__ tile_bins, const GsbRecord *__restrict__ records,
                           const float *__restrict__ background, const float *__restrict__ final_Ts,
@@ -182,6 +191,9 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 float s0 = 0.f, s1 = 0.f, s2 = 0.f;  // sum w, sum w dy, sum w dy^2 over this lane's pixels
                 float a_r = 0.f, a_g = 0.f, a_b = 0.f;
                 float a_z = 0.f;   // DEPTH only
+                float g_x = 0.f, g_y = 0.f;   // ABS only: sum |w| |a dx + b dy|, sum |w| |b dx + c dy|
+                float adx = 0.f, c2 = 0.f;    // ABS only: a dx and c of the record
+                if (ABS) { adx = (2.f * q1.x) * dx; c2 = 2.f * q1.z; }
                 bool any = false;
                 // slots jlo..jhi inside the y-extent (contiguous); a computed jump to jlo that leaves after jhi (an
                 // A/B measurement chose it over the forward kernel's straight line of per-slot bit tests)
@@ -212,6 +224,10 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 s0 += w;                                                                                  \
                 s1 += wdy;                                                                                \
                 s2 = fmaf(wdy, dy, s2);                                                                   \
+                if (ABS) {                                                                                \
+                    g_x = fmaf(fabsf(w), fabsf(fmaf(q1.y, dy, adx)), g_x);                                \
+                    g_y = fmaf(fabsf(w), fabsf(fmaf(c2, dy, bdx)), g_y);                                  \
+                }                                                                                         \
             }                                                                                             \
         }                                                                                                 \
         if (jhi == j) break;                                                                              \
@@ -230,7 +246,7 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 const int k = __float_as_int(q0.w);
                 float *row = grad_rows + (size_t)k * GSB_GRAD_ROW_FLOATS;
                 if (!__any_sync(0xffffffffu, any)) {
-                    if (lane < (DEPTH ? 10 : 9)) row[lane] = 0.f;
+                    if (lane < (ABS ? 12 : DEPTH ? 10 : 9)) row[lane] = 0.f;
                     continue;
                 }
                 // ---- one cross-lane reduction per (tile, Gaussian): 8 values by halving, 1 by butterfly
@@ -261,7 +277,24 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
                 }
                 v0 += __shfl_xor_sync(0xffffffffu, v0, 2);
                 v0 += __shfl_xor_sync(0xffffffffu, v0, 1);
-                if (DEPTH) {
+                if (ABS) {
+                    // values 8, a_z, g_x, g_y by two halving steps and a butterfly (the sums of the branches below in
+                    // the same order): lanes 0..7 end with value 8, 8..15 with g_x, 16..23 with a_z, 24..31 with g_y
+                    const bool up = lane & 16;
+                    const float t8 = up ? v8 : a_z, k8 = up ? a_z : v8;
+                    const float tg = up ? g_x : g_y, kg = up ? g_y : g_x;
+                    v8 = k8 + __shfl_xor_sync(0xffffffffu, t8, 16);
+                    const float e = kg + __shfl_xor_sync(0xffffffffu, tg, 16);
+                    const bool up8 = lane & 8;
+                    const float t = up8 ? v8 : e, kk = up8 ? e : v8;
+                    v8 = kk + __shfl_xor_sync(0xffffffffu, t, 8);
+#pragma unroll
+                    for (int o = 4; o > 0; o >>= 1) v8 += __shfl_xor_sync(0xffffffffu, v8, o);
+                    // lane l holds the total of value (l >> 2); lanes 1, 9, 17, 25 store values 8, 10, 9, 11
+                    const bool wx = (lane & 7) == 1 && (DEPTH || lane != 17);
+                    if (((lane & 3) == 0) || wx) row[wx ? 8 + ((lane >> 3) & 1) * 2 + (lane >> 4) : (lane >> 2)] =
+                        wx ? v8 : v0;
+                } else if (DEPTH) {
                     // values 8 and 9 by one halving step, then a butterfly within each half: lanes 0..15 end with the
                     // total of value 8 (the same sums in the same order as the butterfly below), lanes 16..31 with 9
                     const bool up = lane & 16;
@@ -291,26 +324,34 @@ rasterize_backward_kernel(int img_h, int img_w, int tiles_x, int num_tiles,
 // Sum each Gaussian's rows (contiguous in the unsorted order), apply the moment -> gradient map
 // (backward.cu:323-329 restated on sums) and write the four gradient tensors:
 //   v_sigma = -w:  v_conic = -1/2 (Sxx, Sxy, Syy),  v_xy = -(a Sx + b Sy, b Sx + c Sy),  v_opacity = S0/opac
-// DEPTH also sums slot 9 into v_depths.
-template <bool DEPTH>
+// DEPTH also sums slot 9 into v_depths, ABS slots 10 and 11 into v_xy_abs.
+template <bool DEPTH, bool ABS>
 __global__ void __launch_bounds__(256)
 reduce_grad_rows_kernel(int n, const int *__restrict__ cum_tiles_hit, const float *__restrict__ grad_rows,
                         const float *__restrict__ conics, const float *__restrict__ opacities,
                         float2 *__restrict__ v_xy, float *__restrict__ v_conic,
-                        float *__restrict__ v_colors, float *__restrict__ v_opacity, float *__restrict__ v_depths) {
+                        float *__restrict__ v_colors, float *__restrict__ v_opacity, float *__restrict__ v_depths,
+                        float2 *__restrict__ v_xy_abs) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= n) return;
     const int k0 = g ? cum_tiles_hit[g - 1] : 0, k1 = cum_tiles_hit[g];
     float a[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     float az = 0.f;   // DEPTH only
+    float ax = 0.f, ay = 0.f;   // ABS only
     for (int k = k0; k < k1; ++k) {
         const float4 *row = reinterpret_cast<const float4 *>(grad_rows + (size_t)k * GSB_GRAD_ROW_FLOATS);
         const float4 r0 = row[0], r1 = row[1];
-        const float r8 = reinterpret_cast<const float *>(row)[8];
         a[0] += r0.x; a[1] += r0.y; a[2] += r0.z; a[3] += r0.w;
         a[4] += r1.x; a[5] += r1.y; a[6] += r1.z; a[7] += r1.w;
-        a[8] += r8;
-        if (DEPTH) az += reinterpret_cast<const float *>(row)[9];
+        if (ABS) {
+            const float4 r2 = row[2];
+            a[8] += r2.x;
+            if (DEPTH) az += r2.y;
+            ax += r2.z; ay += r2.w;
+        } else {
+            a[8] += reinterpret_cast<const float *>(row)[8];
+            if (DEPTH) az += reinterpret_cast<const float *>(row)[9];
+        }
     }
     const float S0 = a[0], Sx = a[1], Sy = a[2], Sxx = a[3], Sxy = a[4], Syy = a[5];
     const float ca = conics[3 * g], cb = conics[3 * g + 1], cc = conics[3 * g + 2];
@@ -320,6 +361,7 @@ reduce_grad_rows_kernel(int n, const int *__restrict__ cum_tiles_hit, const floa
     v_colors[3 * g] = a[6]; v_colors[3 * g + 1] = a[7]; v_colors[3 * g + 2] = a[8];
     v_opacity[g] = (op > 0.f) ? S0 / op : 0.f;
     if (DEPTH) v_depths[g] = az;
+    if (ABS) v_xy_abs[g] = make_float2(ax, ay);
 }
 
 }  // namespace
@@ -328,13 +370,15 @@ extern "C" size_t gsb_raster_grad_rows_bytes(int m) {
     return gsb_align_up((size_t)(m > 0 ? m : 0) * GSB_GRAD_ROW_FLOATS * 4 + 256, 256);
 }
 
-// Body of gsb_rasterize_backward (depth = false) and of gsb_rasterize_backward_depth.
+// Body of gsb_rasterize_backward (depth = false), gsb_rasterize_backward_depth and gsb_rasterize_backward_absgrad
+// (v_xy_abs != NULL).
 static int backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m, const int32_t *tile_bins,
                     const int32_t *tile_order, const float *conics, const float *opacities, void *records,
                     const int32_t *cum_tiles_hit, const float *background, const float *final_Ts,
                     const int32_t *final_idx, const float *v_output, const float *v_output_alpha, void *grad_rows,
                     float *v_xy, float *v_conic, float *v_colors, float *v_opacity, unsigned flags, bool depth,
-                    const float *record_depths, const float *v_output_depth, float *v_depths, gsb_stream_t stream) {
+                    const float *record_depths, const float *v_output_depth, float *v_depths, float *v_xy_abs,
+                    gsb_stream_t stream) {
     GSB_CHECK_ARG(img_h > 0 && img_w > 0 && n >= 0 && m >= 0);
     GSB_CHECK_ARG((flags & ~(unsigned)GSB_RASTER_CLAMP_MAX_ONE) == 0);
     const bool sat = (flags & GSB_RASTER_CLAMP_MAX_ONE) != 0;
@@ -343,7 +387,8 @@ static int backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m
     GSB_CHECK_ARG(tile_bins && conics && opacities && cum_tiles_hit && background && final_Ts && final_idx &&
                   v_output && v_xy && v_conic && v_colors && v_opacity);
     GSB_CHECK_ARG(!depth || (v_depths && (record_depths || m == 0)));
-    GSB_CHECK_ARG(((uintptr_t)v_xy % 8) == 0);
+    GSB_CHECK_ARG(((uintptr_t)v_xy % 8) == 0 && ((uintptr_t)v_xy_abs % 8) == 0);
+    const bool abs = v_xy_abs != nullptr;
     cudaStream_t s = (cudaStream_t)stream;
     if (m > 0) {
         GSB_CHECK_ARG(records && grad_rows && ((uintptr_t)records % 16) == 0 && ((uintptr_t)grad_rows % 16) == 0);
@@ -351,24 +396,37 @@ static int backward(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m
             reinterpret_cast<char *>(records) + gsb_raster_records_bytes(m) - 256);
         GSB_CUDA(cudaMemsetAsync(counters, 0, 256, s));
         const int num_tiles = tiles_x * tiles_y;
-#define GSB_BWD_LAUNCH(S, D)                                                                                    \
-    rasterize_backward_kernel<S, D><<<gsb_blend_grid((const void *)rasterize_backward_kernel<S, D>, num_tiles),  \
-                                      RK_THREADS, 0, s>>>(                                                      \
+#define GSB_BWD_LAUNCH(S, D, A)                                                                                 \
+    rasterize_backward_kernel<S, D, A><<<gsb_blend_grid((const void *)rasterize_backward_kernel<S, D, A>,       \
+                                                        num_tiles), RK_THREADS, 0, s>>>(                        \
         img_h, img_w, tiles_x, num_tiles, reinterpret_cast<const int2 *>(tile_bins),                            \
         reinterpret_cast<const GsbRecord *>(records), background, final_Ts, final_idx, v_output, v_output_alpha, \
         reinterpret_cast<float *>(grad_rows), counters, tile_order, record_depths, v_output_depth)
-        if (depth) {
-            if (sat) GSB_BWD_LAUNCH(true, true); else GSB_BWD_LAUNCH(false, true);
+        if (abs) {
+            if (depth) {
+                if (sat) GSB_BWD_LAUNCH(true, true, true); else GSB_BWD_LAUNCH(false, true, true);
+            } else {
+                if (sat) GSB_BWD_LAUNCH(true, false, true); else GSB_BWD_LAUNCH(false, false, true);
+            }
+        } else if (depth) {
+            if (sat) GSB_BWD_LAUNCH(true, true, false); else GSB_BWD_LAUNCH(false, true, false);
         } else {
-            if (sat) GSB_BWD_LAUNCH(true, false); else GSB_BWD_LAUNCH(false, false);
+            if (sat) GSB_BWD_LAUNCH(true, false, false); else GSB_BWD_LAUNCH(false, false, false);
         }
 #undef GSB_BWD_LAUNCH
     }
-#define GSB_REDUCE_LAUNCH(D)                                                                                    \
-    reduce_grad_rows_kernel<D><<<gsb_div_up(n, 256), 256, 0, s>>>(                                              \
+#define GSB_REDUCE_LAUNCH(D, A)                                                                                 \
+    reduce_grad_rows_kernel<D, A><<<gsb_div_up(n, 256), 256, 0, s>>>(                                           \
         n, cum_tiles_hit, reinterpret_cast<const float *>(grad_rows), conics, opacities,                        \
-        reinterpret_cast<float2 *>(v_xy), v_conic, v_colors, v_opacity, v_depths)
-    if (depth) GSB_REDUCE_LAUNCH(true); else GSB_REDUCE_LAUNCH(false);
+        reinterpret_cast<float2 *>(v_xy), v_conic, v_colors, v_opacity, v_depths,                               \
+        reinterpret_cast<float2 *>(v_xy_abs))
+    if (abs) {
+        if (depth) GSB_REDUCE_LAUNCH(true, true); else GSB_REDUCE_LAUNCH(false, true);
+    } else if (depth) {
+        GSB_REDUCE_LAUNCH(true, false);
+    } else {
+        GSB_REDUCE_LAUNCH(false, false);
+    }
 #undef GSB_REDUCE_LAUNCH
     GSB_LAUNCH_CHECK();
     return 0;
@@ -383,7 +441,7 @@ extern "C" int gsb_rasterize_backward(int img_h, int img_w, int tiles_x, int til
                                       gsb_stream_t stream) {
     return backward(img_h, img_w, tiles_x, tiles_y, n, m, tile_bins, tile_order, conics, opacities, records,
                     cum_tiles_hit, background, final_Ts, final_idx, v_output, v_output_alpha, grad_rows, v_xy, v_conic,
-                    v_colors, v_opacity, flags, false, nullptr, nullptr, nullptr, stream);
+                    v_colors, v_opacity, flags, false, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 extern "C" int gsb_rasterize_backward_depth(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
@@ -396,5 +454,23 @@ extern "C" int gsb_rasterize_backward_depth(int img_h, int img_w, int tiles_x, i
                                             float *v_depths, gsb_stream_t stream) {
     return backward(img_h, img_w, tiles_x, tiles_y, n, m, tile_bins, tile_order, conics, opacities, records,
                     cum_tiles_hit, background, final_Ts, final_idx, v_output, v_output_alpha, grad_rows, v_xy, v_conic,
-                    v_colors, v_opacity, flags, true, record_depths, v_output_depth, v_depths, stream);
+                    v_colors, v_opacity, flags, true, record_depths, v_output_depth, v_depths, nullptr, stream);
+}
+
+extern "C" int gsb_rasterize_backward_absgrad(int img_h, int img_w, int tiles_x, int tiles_y, int n, int m,
+                                              const int32_t *tile_bins, const int32_t *tile_order,
+                                              const float *conics, const float *opacities, void *records,
+                                              const int32_t *cum_tiles_hit, const float *background,
+                                              const float *final_Ts, const int32_t *final_idx, const float *v_output,
+                                              const float *v_output_alpha, void *grad_rows, float *v_xy,
+                                              float *v_conic, float *v_colors, float *v_opacity, unsigned flags,
+                                              const float *record_depths, const float *v_output_depth,
+                                              float *v_depths, float *v_xy_abs, gsb_stream_t stream) {
+    // depth is on iff v_depths is given; without it record_depths and v_output_depth must be NULL too
+    GSB_CHECK_ARG(v_xy_abs != nullptr);
+    GSB_CHECK_ARG(v_depths || (!record_depths && !v_output_depth));
+    return backward(img_h, img_w, tiles_x, tiles_y, n, m, tile_bins, tile_order, conics, opacities, records,
+                    cum_tiles_hit, background, final_Ts, final_idx, v_output, v_output_alpha, grad_rows, v_xy, v_conic,
+                    v_colors, v_opacity, flags, v_depths != nullptr, record_depths, v_output_depth, v_depths, v_xy_abs,
+                    stream);
 }

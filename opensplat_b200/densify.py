@@ -33,6 +33,10 @@ class RefineConfig:
     # DESIGN.md D14), so its moments effectively survive.  True = the evident intent (moments zeroed), False = the
     # reference's effective behaviour (moments kept).
     reset_opacity_moments: bool = True
+    # AbsGS (DESIGN D25, gsplat's DefaultStrategy(absgrad=True)): the statistics take the per-Gaussian sum of each
+    # pixel's |contribution| to the 2-D mean's gradient, component by component, in place of v_xy.  Those sums are
+    # larger than |v_xy|, so raise densify_grad_thresh with it (gsplat: 0.0008).  SplatTrainer only.
+    absgrad: bool = False
 
     @property
     def stop_split_at(self):        # model.hpp:31

@@ -92,6 +92,9 @@ class GaussianModel:
         each Gaussian's opacity is scaled by how much the projection's 0.3 px^2 blur spread it.  The parameters, the
         refinement and the saved files keep the raw opacity."""
         from .mcmc import MCMCConfig
+        if getattr(cfg, "absgrad", False):
+            raise ValueError("GaussianModel's statistics take v_xy from autograd; absgrad (RefineConfig(absgrad=True)) "
+                             "runs in trainer.SplatTrainer")
         if isinstance(cfg, MCMCConfig):
             raise ValueError("GaussianModel refines as the reference does (RefineConfig); the MCMC strategy "
                              "(MCMCConfig) runs in trainer.SplatTrainer")

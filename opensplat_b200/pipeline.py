@@ -178,30 +178,43 @@ class SplatPipeline(BinFrame):
                               self.out_img if out_img is None else out_img, self.final_Ts, self.final_idx, flags,
                               count_visible, out_depth=out_depth, out_alpha=out_alpha, depth_values=depth_values)
 
-    def _raster_backward(self, opacities, v_opacities, v_rgbs, flags):
+    def _raster_backward(self, opacities, v_opacities, v_rgbs, flags, v_xy_abs=None):
         """The blend kernel's backward of the last frame (_bin_blend's), from the gradient of its image in self.v_img
         into self.v_xy / self.v_conic, `v_rgbs` ([n,3]) and `v_opacities` ([n]).  opacities: the ones the blend used;
         flags: the ones it was launched with.  The frame's binning state is read here, so callers need not know it:
         which path produced the frame (only the fast path leaves a tile order), the records and the capacity they
-        were sized with, the per-pixel state of the blend."""
+        were sized with, the per-pixel state of the blend.  v_xy_abs ([n,2], DESIGN D25): also write the absolute
+        screen-space gradient there (gsb_rasterize_backward_absgrad; the other outputs are the same bits)."""
         P = capi.ptr
+        if v_xy_abs is not None:
+            capi.check(self.L.gsb_rasterize_backward_absgrad(
+                self.H, self.W, self.tb[0], self.tb[1], self.n, self.m_raster, P(self.tile_bins),
+                P(self.tile_order) if self._ordered else None, P(self.conics), P(opacities), P(self.records),
+                P(self.cum), P(self.background), P(self.final_Ts), P(self.final_idx), P(self.v_img), None,
+                P(self.grad_rows), P(self.v_xy), P(self.v_conic), P(v_rgbs), P(v_opacities), flags, None, None, None,
+                P(v_xy_abs), capi.stream()))
+            return
         capi.check(self.L.gsb_rasterize_backward(
             self.H, self.W, self.tb[0], self.tb[1], self.n, self.m_raster, P(self.tile_bins),
             P(self.tile_order) if self._ordered else None, P(self.conics), P(opacities), P(self.records), P(self.cum),
             P(self.background), P(self.final_Ts), P(self.final_idx), P(self.v_img), None, P(self.grad_rows),
             P(self.v_xy), P(self.v_conic), P(v_rgbs), P(v_opacities), flags, capi.stream()))
 
-    def _raster_backward_depth(self, opacities, v_opacities, v_rgbs, flags, v_output_depth, v_depths):
+    def _raster_backward_depth(self, opacities, v_opacities, v_rgbs, flags, v_output_depth, v_depths, v_xy_abs=None):
         """_raster_backward of a depth frame (_bin_blend with out_depth): the same outputs plus, from the gradient of
         its depth map in `v_output_depth` ([H,W]), the gradient of the per-Gaussian value it blended into `v_depths`
-        ([n]), through the frame's record_depths.  The opacity map gets no cotangent."""
+        ([n]), through the frame's record_depths.  The opacity map gets no cotangent.  v_xy_abs: as _raster_backward's,
+        with the depth term in each pixel's contribution."""
         P = capi.ptr
-        capi.check(self.L.gsb_rasterize_backward_depth(
-            self.H, self.W, self.tb[0], self.tb[1], self.n, self.m_raster, P(self.tile_bins),
-            P(self.tile_order) if self._ordered else None, P(self.conics), P(opacities), P(self.records), P(self.cum),
-            P(self.background), P(self.final_Ts), P(self.final_idx), P(self.v_img), None, P(self.grad_rows),
-            P(self.v_xy), P(self.v_conic), P(v_rgbs), P(v_opacities), flags, P(self.record_depths),
-            P(v_output_depth), P(v_depths), capi.stream()))
+        args = (self.H, self.W, self.tb[0], self.tb[1], self.n, self.m_raster, P(self.tile_bins),
+                P(self.tile_order) if self._ordered else None, P(self.conics), P(opacities), P(self.records),
+                P(self.cum), P(self.background), P(self.final_Ts), P(self.final_idx), P(self.v_img), None,
+                P(self.grad_rows), P(self.v_xy), P(self.v_conic), P(v_rgbs), P(v_opacities), flags,
+                P(self.record_depths), P(v_output_depth), P(v_depths))
+        if v_xy_abs is not None:
+            capi.check(self.L.gsb_rasterize_backward_absgrad(*args, P(v_xy_abs), capi.stream()))
+        else:
+            capi.check(self.L.gsb_rasterize_backward_depth(*args, capi.stream()))
 
     def backward(self):
         """MSE loss against self.target + the whole backward path; grads land in self.grad_flat."""

@@ -87,7 +87,12 @@ projection, forward and backward, in step(), evaluate() and render(), takes the 
 (gsb_project_*_activated_filter3d).  f is computed from the training cameras, uploaded once, at construction, after
 every step whose refinement ran and on filter3d.recompute_due's schedule once refinement has stopped; the alpha reset
 clamps the effective opacity, and save() writes the baked scene.  With pose corrections f uses the cameras as given,
-uncorrected.  Under a group every rank computes the same f from the same cameras (no collective)."""
+uncorrected.  Under a group every rank computes the same f from the same cameras (no collective).
+
+With AbsGS's absolute gradients (`cfg=densify.RefineConfig(absgrad=True, densify_grad_thresh=0.0008)`, DESIGN D25)
+each view's rasterize-backward is gsb_rasterize_backward_absgrad, which also writes the per-Gaussian sum of each
+pixel's |contribution| to the 2-D mean's gradient (v_xy_abs), and the view's densification statistics take it in
+place of v_xy.  The launch count, every gradient and the Adam step are those of a plain trainer."""
 import ctypes as C
 
 import torch
@@ -184,6 +189,8 @@ class SplatTrainer:
         featuresDc [n,3], featuresRest [n,K-1,3], opacities [n,1] logits), as model.GaussianModel takes them.
         cfg: densify.RefineConfig (the reference's refinement, the default) or mcmc.MCMCConfig (3DGS-MCMC under a
         Gaussian budget, DESIGN D20: no densification statistics are taken, the loss returned stays the image loss).
+        RefineConfig(absgrad=True) (DESIGN D25) feeds the statistics AbsGS's absolute screen-space gradient, written
+        by the blend backward (gsb_rasterize_backward_absgrad) in place of v_xy; nothing else in the step changes.
         m_capacity: initial intersection capacity of the binning buffers (grown on demand).
         group: a process group to train data-parallel over camera views (any size, 1 included); every rank
         constructs the trainer with the same parameters and calls step() with the same step numbers.
@@ -246,6 +253,7 @@ class SplatTrainer:
         # the refinement strategy: the reference's Model::afterTrain (RefineConfig) or 3DGS-MCMC (MCMCConfig, D20)
         self.refiner = MCMCRefiner(self.cfg) if isinstance(self.cfg, MCMCConfig) else None
         self.densifier = None if self.refiner is not None else Densifier(self.cfg, generator=generator, group=group)
+        self._absgrad = self.densifier is not None and getattr(self.cfg, "absgrad", False)
         # the B cameras: views [B,16] | projs [B,16] | centres [B,3], one pinned staging block, one upload per step;
         # with pose corrections (D22) the uploaded views and centres go to base views [B,16] | base centres [B,3]
         # behind them, and the corrected ones are written into the first slots
@@ -309,6 +317,8 @@ class SplatTrainer:
             self.cam_partials = torch.empty(max(floats, 1), dtype=torch.float32, device=d)
         if self.filter3d_cfg is not None:   # D24: the 3-D filter, recomputed after every refinement
             self.f3d = torch.empty(n, dtype=torch.float32, device=d)
+        if self._absgrad:   # D25: the blend's absolute screen-space gradient, the statistics' input
+            self.v_xy_abs = torch.empty((n, 2), dtype=torch.float32, device=d)
         if self.depth is not None:   # D23: 1/z where radii > 0, its blend gradient, and the projection's v_depth
             self.inv_depths = torch.empty(n, dtype=torch.float32, device=d)
             self.v_inv_depths = torch.empty(n, dtype=torch.float32, device=d)
@@ -463,9 +473,11 @@ class SplatTrainer:
             # barriers.
             if B > 1 or visible[b] or self.world > 1:
                 self._backward_view(b, use, intr[0], intr[1], image=images[b], prior=priors[b] is not None)
-            # this view's densification statistics (pp.v_xy / pp.radii are overwritten by the next view)
+            # this view's densification statistics (pp.v_xy / pp.radii are overwritten by the next view); with
+            # absgrad (D25) they take the absolute screen-space gradient instead
             if self.densifier is not None:
-                self.densifier.accumulate_view(step, pp.v_xy if visible[b] else None, pp.radii, H, W)
+                v_xy = self.v_xy_abs if self._absgrad else pp.v_xy
+                self.densifier.accumulate_view(step, v_xy if visible[b] else None, pp.radii, H, W)
         # A step whose views all hit nothing trains nothing; with more than one rank it still takes part in the step
         # (the Adam step every replica takes, the refinement's collectives; see the module docstring).
         trains = any(visible) or self.world > 1
@@ -646,14 +658,15 @@ class SplatTrainer:
         if ex is not None:
             ex.set_camera(self.cam_positions[b], b)
         v_depth = None
+        v_xy_abs = self.v_xy_abs if self._absgrad else None   # D25
         if prior:
             pp._raster_backward_depth(self.opac, self.v_opac, self.v_rgb_views[b], ops.CLAMP_MAX_ONE,
-                                      self.v_depth_render, self.v_inv_depths)
+                                      self.v_depth_render, self.v_inv_depths, v_xy_abs=v_xy_abs)
             capi.check(L.gsb_inverse_depths_backward(n, P(pp.depths), P(pp.radii), P(self.v_inv_depths), P(self.v_z),
                                                      capi.stream()))
             v_depth = self.v_z
         else:
-            pp._raster_backward(self.opac, self.v_opac, self.v_rgb_views[b], ops.CLAMP_MAX_ONE)
+            pp._raster_backward(self.opac, self.v_opac, self.v_rgb_views[b], ops.CLAMP_MAX_ONE, v_xy_abs=v_xy_abs)
         if ex is not None and ex.overlap and b == self.views_per_step - 1:
             # every colour slot is final: colour pulls + SH expansion start now, on a side stream
             ex.start_colour(degrees_to_use=use, rgbs=self.rgbs_views)
