@@ -648,6 +648,18 @@ size_t gsb_ssim_workspace_bytes(int img_h, int img_w);
 int gsb_ssim_l1_loss(int img_h, int img_w, const float *rendered, const float *gt, float ssim_weight,
                      float *v_rendered, float *loss_out, void *workspace, size_t workspace_bytes,
                      gsb_stream_t stream);
+/* gsb_ssim_l1_loss_masked (DESIGN D26): the loss over the used pixels of mask [H,W] u8 (nonzero = used, 0 = ignored).
+ *   With m the mask, N = sum m, x~ = m ? gt : 0 and y~ = m ? rendered : 0 (selected, so non-finite values in ignored
+ *   pixels never reach the result) and S_c the SSIM map of x~ and y~: L1 = sum m |y - x| / 3N, SSIM = sum m S_c / 3N,
+ *   total = (1-w) L1 + w (1 - SSIM); v_rendered is its gradient, exactly 0 on ignored pixels.  N = 0 gives {0, 0, 1}
+ *   and a zero gradient.  With every pixel used and H W <= 2^24, v_rendered equals gsb_ssim_l1_loss's bit for bit and
+ *   loss_out holds the same sums (in both entry points their per-tile float atomics make the last bits of the three
+ *   scalars depend on the order the tiles finish).
+ *   N, the loss and the gradient scales stay on the device (no host read-back).  The workspace is
+ *   gsb_ssim_workspace_bytes(H, W), 256-byte aligned. */
+int gsb_ssim_l1_loss_masked(int img_h, int img_w, const float *rendered, const float *gt, const uint8_t *mask,
+                            float ssim_weight, float *v_rendered, float *loss_out, void *workspace,
+                            size_t workspace_bytes, gsb_stream_t stream);
 
 /* ---- Point-cloud initialisation (Model's constructor, model.hpp:23-57) ---------------------------
  * gsb_knn_mean_dist replaces PointsTensor::scales (kdtree_tensor.cpp:4-22, a nanoflann k-d tree on the CPU):
@@ -732,13 +744,25 @@ int gsb_reset_opacity_filter3d(int n, float max_logit, float reset_value, const 
  *   fixed-point bilinear with BORDER_CONSTANT 0.  An empty ROI is a no-op.
  * gsb_u8_to_f32_views converts num_views images of [h,w,3] u8 (views: a DEVICE array of num_views device addresses,
  *   int64) into out [num_views,h,w,3] float32 = float(u) / 255.0f (IEEE division, as imageToTensor), in one launch.
- *   num_views = 0 is a no-op; at most 65535. */
+ *   num_views = 0 is a no-op; at most 65535.
+ * gsb_resize_area_mask_u8 / gsb_undistort_mask_u8 (DESIGN D26) take a u8 [h,w] loss mask (nonzero = used) through the
+ *   geometry of gsb_resize_area_u8 / gsb_undistort_u8, with the same arguments and checks, and write 0 / 1 bytes: an
+ *   output pixel is 1 iff every source pixel with a nonzero weight in the colour's output pixel is used.  Resize: the
+ *   cell clipped to the image on the integer-scale path (a cell wholly outside it is 0), the entries of OpenCV's
+ *   computeResizeAreaTab (with its 1e-3 cut-offs) on the general path; equal sizes normalise the mask to 0 / 1.
+ *   Undistort: the tap (sx, sy) always, the right taps iff the map's x fraction is nonzero, the bottom taps iff its y
+ *   fraction is; a tap outside the image makes the pixel 0. */
 int gsb_resize_area_u8(int src_h, int src_w, const uint8_t *src, int dst_h, int dst_w, uint8_t *dst, float inv_scale,
                        gsb_stream_t stream);
 int gsb_undistort_u8(int h, int w, const uint8_t *src, float fx, float fy, float cx, float cy, float k1, float k2,
                      float p1, float p2, float k3, float new_fx, float new_fy, float new_cx, float new_cy, int roi_x,
                      int roi_y, int roi_w, int roi_h, uint8_t *dst, gsb_stream_t stream);
 int gsb_u8_to_f32_views(int num_views, const int64_t *views, int h, int w, float *out, gsb_stream_t stream);
+int gsb_resize_area_mask_u8(int src_h, int src_w, const uint8_t *src, int dst_h, int dst_w, uint8_t *dst,
+                            float inv_scale, gsb_stream_t stream);
+int gsb_undistort_mask_u8(int h, int w, const uint8_t *src, float fx, float fy, float cx, float cy, float k1, float k2,
+                          float p1, float p2, float k3, float new_fx, float new_fy, float new_cx, float new_cy,
+                          int roi_x, int roi_y, int roi_w, int roi_h, uint8_t *dst, gsb_stream_t stream);
 
 #ifdef __cplusplus
 }

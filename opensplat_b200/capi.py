@@ -146,6 +146,8 @@ _SIGS = {
     "gsb_pack_splat_rows": (_i, [_i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _f, C.POINTER(C.c_float), _vp, _vp]),
     "gsb_ssim_workspace_bytes": (_sz, [_i, _i]),
     "gsb_ssim_l1_loss": (_i, [_i, _i, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
+    # D26: H, W, rendered, gt, mask, w, v_rendered, loss_out, workspace, workspace_bytes, stream
+    "gsb_ssim_l1_loss_masked": (_i, [_i, _i, _vp, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),
     "gsb_adam_step": (_i, [C.c_longlong, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _vp]),
     # num_segments, segments (host AdamSegment array), param, grad, exp_avg, exp_avg_sq, b1, b2, eps, bc1, bc2, stream
     "gsb_adam_step_segments": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _vp]),
@@ -157,6 +159,10 @@ _SIGS = {
     "gsb_undistort_u8": (_i, [_i, _i, _vp, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _i, _i, _i, _i, _vp,
                               _vp]),
     "gsb_u8_to_f32_views": (_i, [_i, _vp, _i, _i, _vp, _vp]),
+    # D26: the loss masks, with the arguments of the two above
+    "gsb_resize_area_mask_u8": (_i, [_i, _i, _vp, _i, _i, _vp, _f, _vp]),
+    "gsb_undistort_mask_u8": (_i, [_i, _i, _vp, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _f, _i, _i, _i, _i,
+                                   _vp, _vp]),
 }
 
 ADAM_MAX_SEGMENTS = 8   # GSB_ADAM_MAX_SEGMENTS

@@ -17,6 +17,8 @@
 //     point's y shifted by the stripe's first row, cv::invert's closed-form 3x3 inverse), quantised to 1/32 pixel
 //     (CV_16SC2), then remap's fixed-point bilinear (15-bit weights, BORDER_CONSTANT 0) for the ROI pixels only.
 //   gsb_u8_to_f32_views: B stored images -> one float32 [B,H,W,3] at float(u) / 255.0f (IEEE division).
+//   gsb_resize_area_mask_u8 / gsb_undistort_mask_u8 (DESIGN D26): a u8 [h,w] loss mask through the same geometry; an
+//     output pixel is used (1) iff every source pixel with a nonzero weight in its colour is used, else 0.
 #include <float.h>
 #include <math.h>
 
@@ -143,13 +145,8 @@ __device__ __forceinline__ int sat_round_int(double v) {
     return (int)fmin(fmax(rint(v), -2147483648.0), 2147483647.0);
 }
 
-__global__ void __launch_bounds__(IMG_THREADS)
-undistort_kernel(int h, int w, const unsigned char *__restrict__ src, UndistortParams P, int stripe, int roi_x,
-                 int roi_y, int roi_w, int roi_h, unsigned char *__restrict__ dst) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= roi_w * roi_h) return;
-    const int oy = t / roi_w, ox = t - oy * roi_w;
-    const int r = roi_y + oy, j = roi_x + ox;
+// the CV_16SC2 map entry (iu, iv), in 1/32 pixel, of output pixel (row r, column j) of cv::undistort
+__device__ __forceinline__ void undistort_map(const UndistortParams &P, int stripe, int r, int j, int &iu, int &iv) {
     const int ys = (r / stripe) * stripe, i = r - ys;
     // iR = inv(Ar) of the stripe, Ar = [[a,0,c],[0,b,e - ys],[0,0,1]]: cv::invert's closed form, d = 1/det
     const double e = __dsub_rn(P.e, (double)ys);
@@ -172,7 +169,19 @@ undistort_kernel(int h, int w, const unsigned char *__restrict__ src, UndistortP
                                 __dmul_rn(P.p2, xy2));
     const double u = __dadd_rn(__dmul_rn(P.fx, xd), P.u0);
     const double v = __dadd_rn(__dmul_rn(P.fy, yd), P.v0);
-    const int iu = sat_round_int(__dmul_rn(u, 32.0)), iv = sat_round_int(__dmul_rn(v, 32.0));
+    iu = sat_round_int(__dmul_rn(u, 32.0));
+    iv = sat_round_int(__dmul_rn(v, 32.0));
+}
+
+__global__ void __launch_bounds__(IMG_THREADS)
+undistort_kernel(int h, int w, const unsigned char *__restrict__ src, UndistortParams P, int stripe, int roi_x,
+                 int roi_y, int roi_w, int roi_h, unsigned char *__restrict__ dst) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= roi_w * roi_h) return;
+    const int oy = t / roi_w, ox = t - oy * roi_w;
+    const int r = roi_y + oy, j = roi_x + ox;
+    int iu, iv;
+    undistort_map(P, stripe, r, j, iu, iv);
     const int sx = (short)(iu >> 5), sy = (short)(iv >> 5);      // CV_16SC2
     const int ax = iu & 31, ay = iv & 31;
     unsigned char *o = dst + 3 * (size_t)t;
@@ -211,6 +220,59 @@ u8_to_f32_kernel(const long long *__restrict__ views, size_t n_bytes, float *__r
     for (size_t q = 4 * n4 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; q < n_bytes;
          q += (size_t)gridDim.x * blockDim.x)
         dst[q] = __fdiv_rn((float)src[q], 255.f);
+}
+
+// ---- loss masks (DESIGN D26): 1 byte per pixel, nonzero = used; the outputs are 0 / 1 -------------------------------
+// An output pixel is used iff every source pixel INTER_AREA sums into it is used: the entries of area_cell on both
+// axes (the partial first cell, the whole cells, the partial last cell, with OpenCV's 1e-3 cut-offs).
+__global__ void __launch_bounds__(IMG_THREADS)
+resize_area_mask_general_kernel(int sh, int sw, const unsigned char *__restrict__ src, int dh, int dw,
+                                unsigned char *__restrict__ dst, double scale_x, double scale_y) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= dh * dw) return;
+    const int dy = i / dw, dx = i - dy * dw;
+    const AreaCell cx = area_cell(dx, sw, scale_x), cy = area_cell(dy, sh, scale_y);
+    const int x0 = cx.head ? cx.s1 - 1 : cx.s1, x1 = cx.tail ? cx.s2 + 1 : cx.s2;
+    const int y0 = cy.head ? cy.s1 - 1 : cy.s1, y1 = cy.tail ? cy.s2 + 1 : cy.s2;
+    bool used = true;
+    for (int y = y0; y < y1 && used; ++y)
+        for (int x = x0; x < x1; ++x) used = used && src[(size_t)y * sw + x] != 0;
+    dst[i] = used ? 1 : 0;
+}
+
+// the integer-scale fast path: the cell clipped to the image; a cell wholly outside it (OpenCV writes colour 0) is
+// ignored.  isx = isy = 1 is the copy of equal sizes.
+__global__ void __launch_bounds__(IMG_THREADS)
+resize_area_mask_fast_kernel(int sh, int sw, const unsigned char *__restrict__ src, int dh, int dw,
+                             unsigned char *__restrict__ dst, int isx, int isy) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= dh * dw) return;
+    const int dy = i / dw, dx = i - dy * dw;
+    const int y0 = dy * isy, x0 = dx * isx;
+    bool used = y0 < sh && x0 < sw;
+    const int y1 = min(y0 + isy, sh), x1 = min(x0 + isx, sw);
+    for (int y = y0; y < y1 && used; ++y)
+        for (int x = x0; x < x1; ++x) used = used && src[(size_t)y * sw + x] != 0;
+    dst[i] = used ? 1 : 0;
+}
+
+// An output pixel of the ROI is used iff every bilinear tap with a nonzero fixed-point weight lies inside the image
+// and is used: (sx, sy) always, the right taps iff ax > 0, the bottom taps iff ay > 0.  A pixel whose taps all fall
+// outside (colour 0, BORDER_CONSTANT) is ignored.
+__global__ void __launch_bounds__(IMG_THREADS)
+undistort_mask_kernel(int h, int w, const unsigned char *__restrict__ src, UndistortParams P, int stripe, int roi_x,
+                      int roi_y, int roi_w, int roi_h, unsigned char *__restrict__ dst) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= roi_w * roi_h) return;
+    const int oy = t / roi_w, ox = t - oy * roi_w;
+    int iu, iv;
+    undistort_map(P, stripe, roi_y + oy, roi_x + ox, iu, iv);
+    const int sx = (short)(iu >> 5), sy = (short)(iv >> 5);
+    const int xe = (iu & 31) ? sx + 1 : sx, ye = (iv & 31) ? sy + 1 : sy;   // last tap column / row
+    bool used = sx >= 0 && sy >= 0 && xe < w && ye < h;
+    for (int y = sy; y <= ye && used; ++y)
+        for (int x = sx; x <= xe; ++x) used = used && src[(size_t)y * w + x] != 0;
+    dst[t] = used ? 1 : 0;
 }
 
 }  // namespace
@@ -276,6 +338,55 @@ extern "C" int gsb_u8_to_f32_views(int num_views, const int64_t *views, int h, i
     const int blocks = (int)std::min<size_t>((n / 4 + IMG_THREADS - 1) / IMG_THREADS + 1, 1024);
     u8_to_f32_kernel<<<dim3(blocks, num_views), IMG_THREADS, 0, (cudaStream_t)stream>>>(
         (const long long *)views, n, out);
+    GSB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int gsb_resize_area_mask_u8(int src_h, int src_w, const uint8_t *src, int dst_h, int dst_w, uint8_t *dst,
+                                       float inv_scale, gsb_stream_t stream) {
+    GSB_CHECK_ARG(src_h > 0 && src_w > 0 && dst_h > 0 && dst_w > 0);
+    GSB_CHECK_ARG(dst_h <= src_h && dst_w <= src_w);
+    GSB_CHECK_ARG((long long)src_h * src_w <= 0x7fffffffLL / 3);
+    GSB_CHECK_ARG(src && dst && (const void *)src != (const void *)dst);
+    GSB_CHECK_ARG(inv_scale == 0.f || (inv_scale > 0.f && inv_scale <= 1.f));
+    double ix, iy;
+    if (inv_scale == 0.f) {
+        ix = (double)dst_w / src_w;
+        iy = (double)dst_h / src_h;
+    } else {
+        ix = iy = (double)inv_scale;
+        GSB_CHECK_ARG(dst_w == (int)nearbyint(src_w * ix) && dst_h == (int)nearbyint(src_h * iy));
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const int blocks = gsb_div_up(dst_h * dst_w, IMG_THREADS);
+    const double sx = 1.0 / ix, sy = 1.0 / iy;
+    const int isx = (int)nearbyint(sx), isy = (int)nearbyint(sy);
+    if (dst_h == src_h && dst_w == src_w)   // the colour is copied: the mask is normalised to 0 / 1
+        resize_area_mask_fast_kernel<<<blocks, IMG_THREADS, 0, s>>>(src_h, src_w, src, dst_h, dst_w, dst, 1, 1);
+    else if (fabs(sx - isx) < DBL_EPSILON && fabs(sy - isy) < DBL_EPSILON)
+        resize_area_mask_fast_kernel<<<blocks, IMG_THREADS, 0, s>>>(src_h, src_w, src, dst_h, dst_w, dst, isx, isy);
+    else
+        resize_area_mask_general_kernel<<<blocks, IMG_THREADS, 0, s>>>(src_h, src_w, src, dst_h, dst_w, dst, sx, sy);
+    GSB_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int gsb_undistort_mask_u8(int h, int w, const uint8_t *src, float fx, float fy, float cx, float cy,
+                                     float k1, float k2, float p1, float p2, float k3, float new_fx, float new_fy,
+                                     float new_cx, float new_cy, int roi_x, int roi_y, int roi_w, int roi_h,
+                                     uint8_t *dst, gsb_stream_t stream) {
+    GSB_CHECK_ARG(h > 0 && w > 0 && (long long)h * w <= 0x7fffffffLL / 3);
+    GSB_CHECK_ARG(roi_x >= 0 && roi_y >= 0 && roi_w >= 0 && roi_h >= 0 && roi_x + roi_w <= w && roi_y + roi_h <= h);
+    GSB_CHECK_ARG(isfinite(fx) && isfinite(fy) && isfinite(cx) && isfinite(cy) && fx != 0.f && fy != 0.f);
+    GSB_CHECK_ARG(isfinite(new_fx) && isfinite(new_fy) && isfinite(new_cx) && isfinite(new_cy) && new_fx != 0.f &&
+                  new_fy != 0.f);
+    GSB_CHECK_ARG(isfinite(k1) && isfinite(k2) && isfinite(p1) && isfinite(p2) && isfinite(k3));
+    if (roi_w == 0 || roi_h == 0) return 0;
+    GSB_CHECK_ARG(src && dst && (const void *)src != (const void *)dst);
+    const UndistortParams P{fx, fy, cx, cy, k1, k2, p1, p2, k3, new_fx, new_fy, new_cx, new_cy};
+    const int stripe = std::min(std::max(1, 4096 / w), h);
+    undistort_mask_kernel<<<gsb_div_up(roi_w * roi_h, IMG_THREADS), IMG_THREADS, 0, (cudaStream_t)stream>>>(
+        h, w, src, P, stripe, roi_x, roi_y, roi_w, roi_h, dst);
     GSB_LAUNCH_CHECK();
     return 0;
 }

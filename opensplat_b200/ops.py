@@ -784,21 +784,34 @@ class SphericalHarmonicsRgb(torch.autograd.Function):
 
 class MainLoss(torch.autograd.Function):
     """Model::mainLoss (model.cpp:780-784): (1 - w) * L1 + w * (1 - SSIM), fused forward + gradient
-    (gsb_ssim_l1_loss).  rendered, gt: [H,W,3] CUDA tensors.  Returns the scalar loss."""
+    (gsb_ssim_l1_loss).  rendered, gt: [H,W,3] CUDA tensors.  Returns the scalar loss.  mask (DESIGN D26): an optional
+    uint8 or bool [H,W] tensor on rendered's device; the loss is then taken over its nonzero (used) pixels only
+    (gsb_ssim_l1_loss_masked), and the gradient is 0 on the others."""
 
     @staticmethod
-    def forward(ctx, rendered, gt, ssimWeight):
+    def forward(ctx, rendered, gt, ssimWeight, mask=None):
         H, W = rendered.shape[0], rendered.shape[1]
         if rendered.dim() != 3 or rendered.shape[2] != 3 or gt.shape != rendered.shape:
             raise ValueError("rendered and gt must be [H,W,3]")
+        if mask is not None:
+            if (not isinstance(mask, torch.Tensor) or mask.dtype not in (torch.uint8, torch.bool)
+                    or tuple(mask.shape) != (H, W) or mask.device != rendered.device):
+                raise ValueError(f"mask must be a uint8 or bool [{H},{W}] tensor on {rendered.device}")
+            mask = mask.contiguous()
+            mask = mask.view(torch.uint8) if mask.dtype == torch.bool else mask
         L = capi.lib()
         r, g = capi.f32(rendered), capi.f32(gt)
         ws = _ws.get(r.device, "ssim", L.gsb_ssim_workspace_bytes(H, W) + 256)
         off = (-ws.data_ptr()) % 256
         v = torch.empty_like(r)
         out = torch.empty(3, dtype=torch.float32, device=r.device)
-        capi.check(L.gsb_ssim_l1_loss(H, W, capi.ptr(r), capi.ptr(g), float(ssimWeight), capi.ptr(v), capi.ptr(out),
-                                      ws.data_ptr() + off, ws.numel() - off, capi.stream()))
+        if mask is None:
+            capi.check(L.gsb_ssim_l1_loss(H, W, capi.ptr(r), capi.ptr(g), float(ssimWeight), capi.ptr(v),
+                                          capi.ptr(out), ws.data_ptr() + off, ws.numel() - off, capi.stream()))
+        else:
+            capi.check(L.gsb_ssim_l1_loss_masked(H, W, capi.ptr(r), capi.ptr(g), capi.ptr(mask), float(ssimWeight),
+                                                 capi.ptr(v), capi.ptr(out), ws.data_ptr() + off, ws.numel() - off,
+                                                 capi.stream()))
         ctx.save_for_backward(v)
         ctx.parts = out
         return out[0].clone()
@@ -806,7 +819,7 @@ class MainLoss(torch.autograd.Function):
     @staticmethod
     def backward(ctx, v_loss):
         (v,) = ctx.saved_tensors
-        return v * v_loss, None, None
+        return v * v_loss, None, None, None
 
 
 class ActivateGaussians(torch.autograd.Function):

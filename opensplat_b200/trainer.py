@@ -92,7 +92,14 @@ uncorrected.  Under a group every rank computes the same f from the same cameras
 With AbsGS's absolute gradients (`cfg=densify.RefineConfig(absgrad=True, densify_grad_thresh=0.0008)`, DESIGN D25)
 each view's rasterize-backward is gsb_rasterize_backward_absgrad, which also writes the per-Gaussian sum of each
 pixel's |contribution| to the 2-D mean's gradient (v_xy_abs), and the view's densification statistics take it in
-place of v_xy.  The launch count, every gradient and the Adam step are those of a plain trainer."""
+place of v_xy.  The launch count, every gradient and the Adam step are those of a plain trainer.
+
+With per-image loss masks (`step(cam, gt, step, mask=M)`, DESIGN D26; no constructor flag) a view's colour loss is
+gsb_ssim_l1_loss_masked over the pixels where M is nonzero: the images' ignored pixels are read as 0, the loss is
+normalised by the view's own used-pixel count and the ignored pixels' gradient is exactly 0.  With appearance grids the
+mask applies to the loss on the sliced image.  Everything after the loss gradient (densification statistics, absgrad,
+MCMC, pose corrections, the exchange) sees the mask through it; the depth prior keeps its own validity rule.  A view
+without a mask issues exactly the launches of a plain trainer."""
 import ctypes as C
 
 import torch
@@ -431,7 +438,39 @@ class SplatTrainer:
                 raise ValueError(f"every depth map must be a contiguous float32 [H,W] tensor on {self.device}")
         return maps
 
-    def step(self, cam, gt, step, image=None, depth=None):
+    def _masks(self, mask, views, H, W):
+        """step() / evaluate()'s mask= (D26) as a list of `views` u8 [H,W] device masks or Nones (a bool mask is
+        viewed as u8); raises ValueError on a wrong count, type, dtype, device, rank or size."""
+        if mask is None:
+            return [None] * views
+        if isinstance(mask, torch.Tensor):
+            if views == 1:
+                ms = [mask]
+            elif mask.dim() == 3:
+                ms = list(mask.unbind(0))
+            else:
+                raise ValueError(f"mask= must be a [{views},H,W] tensor or a sequence of {views} masks")
+        elif isinstance(mask, (list, tuple)):
+            ms = list(mask)
+        else:
+            raise ValueError("mask= must be a uint8 or bool [H,W] CUDA tensor, a sequence of them (or None), or "
+                             "[B,H,W]")
+        if len(ms) != views:
+            raise ValueError(f"mask= must give {views} masks (None for a view without one), got {len(ms)}")
+        out = []
+        for m in ms:
+            if m is None:
+                out.append(None)
+                continue
+            if (not isinstance(m, torch.Tensor) or m.dtype not in (torch.uint8, torch.bool) or m.device != self.device
+                    or m.dim() != 2 or not m.is_contiguous()):
+                raise ValueError(f"every mask must be a contiguous uint8 or bool [H,W] tensor on {self.device}")
+            if tuple(m.shape) != (H, W):
+                raise ValueError(f"every mask must be [{H},{W}] (this step's render resolution), got {list(m.shape)}")
+            out.append(m.view(torch.uint8) if m.dtype == torch.bool else m)
+        return out
+
+    def step(self, cam, gt, step, image=None, depth=None, mask=None):
         """One training step at `step` (1-based, as opensplat.cpp counts).  At views_per_step = 1: cam is one
         model.Camera, gt one [H,W,3] fp32 CUDA image at this step's render resolution, and the result is the device
         tensor {total, L1, SSIM}.  At B > 1: cam is a sequence of B cameras, gt B images (a sequence or a [B,H,W,3]
@@ -439,20 +478,27 @@ class SplatTrainer:
         the result.  image: with appearance grids or pose corrections, the training image of the view (an int) or of
         each of the B views (a sequence of B ints); without them it must be None.  depth: with depth priors (D23), at
         B = 1 one float32 [H,W] CUDA inverse-depth map at this step's render resolution or None; at B > 1 a sequence of
-        B such maps, any of which may be None, or a [B,H,W] tensor.  Raises ValueError on a wrong number of views,
-        mixed resolutions, a wrong image, a wrong image= or a wrong depth=."""
+        B such maps, any of which may be None, or a [B,H,W] tensor.  mask: a loss mask (D26) in the shapes of depth=,
+        each a uint8 or bool [H,W] CUDA tensor (nonzero = the pixel is used); a view with one takes the masked loss.
+        Raises ValueError on a wrong number of views, mixed resolutions, a wrong image, a wrong image=, a wrong depth=
+        or a wrong mask=."""
         pp, B, ap, po = self.pipe, self.views_per_step, self.appearance, self.poses
         images = self._images(image, B)
         priors = self._depth_maps(depth, B)
         gts = [gt] if B == 1 else gt
+        masks, checked = [None] * B, None
+        if mask is not None or any(m is not None for m in priors):
+            # the step's views, checked before any launch; _setup_views reuses them
+            checked = view_setups(cam, gts, B, downscale_factor(step, self.num_downscales, self.resolution_schedule))
+            _, H, W = checked
+            masks = self._masks(mask, B, H, W)
         if any(m is not None for m in priors):
-            _, H, W = view_setups(cam, gts, B, downscale_factor(step, self.num_downscales, self.resolution_schedule))
             if any(m is not None and tuple(m.shape) != (H, W) for m in priors):
                 raise ValueError(f"every depth map must be [{H},{W}] (this step's render resolution)")
             # g = w(s) / (H W) in fp64, rounded once: the gradient of the weighted loss w.r.t. a valid pixel of R
             depth_g = float(depth_weight(self.depth, step) / (H * W))
         # ---- forward, enqueued without a host wait until each view's binning read-back ----
-        setups, H, W, use = self._setup_views(cam, gts, B, step, images if po is not None else None)
+        setups, H, W, use = self._setup_views(cam, gts, B, step, images if po is not None else None, checked)
         if ap is not None:
             ap.tv()                         # D21: the grids' gradient starts as tv_weight * dTV
         if po is not None:
@@ -461,7 +507,7 @@ class SplatTrainer:
         for b in range(B):
             intr = setups[b][2]
             self._render_view(b, intr, gts[b], self.losses[b], image=images[b] if ap is not None else None,
-                              prior=priors[b])
+                              prior=priors[b], mask=masks[b])
             if priors[b] is not None:
                 self._depth_loss(priors[b], depth_g, self.depth_losses[b])
             elif self.depth is not None:
@@ -506,7 +552,7 @@ class SplatTrainer:
             self._compute_filter3d()
         return self.losses[0] if B == 1 else self.losses
 
-    def evaluate(self, cam, gt, step, image=None):
+    def evaluate(self, cam, gt, step, image=None, mask=None):
         """The loss of one view without training on it (opensplat.cpp:203-207, the --val camera): Model::forward at
         `step`'s downscale factor and SH degree, then mainLoss against gt (a float32 [H,W,3] CUDA image at that
         resolution).  It runs the forward kernels and the loss of a one-view step() (at any views_per_step) and
@@ -516,9 +562,14 @@ class SplatTrainer:
         at another resolution than the last step's reallocates the pixel buffers, and the next step reallocates them
         back, each counted in `pixel_reallocs`; and the binning buffers grow if the view needs more intersections
         than they hold (a step grows them the same way, with no effect on its result).  image: with pose corrections,
-        render at training image `image`'s corrected pose (D22).  Raises ValueError on a wrong image or image=."""
-        setups = self._setup_views(cam, [gt], 1, step, self._view_pose(image))[0]
-        self._render_view(0, setups[0][2], gt, self.eval_loss)
+        render at training image `image`'s corrected pose (D22).  mask: a loss mask as step()'s (D26); only the used
+        pixels of the view are scored.  Raises ValueError on a wrong image, image= or mask=."""
+        masks, checked = [None], None
+        if mask is not None:
+            checked = view_setups(cam, [gt], 1, downscale_factor(step, self.num_downscales, self.resolution_schedule))
+            masks = self._masks(mask, 1, checked[1], checked[2])
+        setups = self._setup_views(cam, [gt], 1, step, self._view_pose(image), checked)[0]
+        self._render_view(0, setups[0][2], gt, self.eval_loss, mask=masks[0])
         return self.eval_loss
 
     def render(self, cam, step, normalize_depth=False, image=None):
@@ -556,15 +607,16 @@ class SplatTrainer:
             raise ValueError("image= in evaluate() and render() needs a trainer constructed with pose=")
         return check_images(image, 1, self.num_images)
 
-    def _setup_views(self, cams, gts, views, step, images=None):
+    def _setup_views(self, cams, gts, views, step, images=None, checked=None):
         """What the forward passes of a step's `views` views share: view_setups at `step`'s downscale factor, the
         render resolution, one upload of the cameras into slots 0..views-1 of the camera block (the last host wait, a
         binning read-back, came after the block's previous upload), `proj @ view` and the SH colours.  One view takes
         the 2-D matmul and the one-view SH forward (see the module docstring).  With `images` (D22: one training image
         per view) each view's camera is uploaded into the base slots and corrected by its image's pose into the
-        working slots before the matmul.  Returns (setups, H, W, use): use is the step's SH degrees_to_use."""
-        setups, H, W = view_setups(cams, gts, views, downscale_factor(step, self.num_downscales,
-                                                                       self.resolution_schedule))
+        working slots before the matmul.  checked: view_setups' result for these arguments when the caller already
+        has it.  Returns (setups, H, W, use): use is the step's SH degrees_to_use."""
+        setups, H, W = checked or view_setups(cams, gts, views, downscale_factor(step, self.num_downscales,
+                                                                                  self.resolution_schedule))
         if (W, H) != self.resolution:
             self._set_resolution(W, H)
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
@@ -612,24 +664,34 @@ class SplatTrainer:
         pp._bin_blend(self.opac, ops.CLAMP_MAX_ONE, count_visible=True, rgbs=self.rgbs_views[b], out_img=out_img,
                       out_depth=out_depth, out_alpha=out_alpha, depth_values=self.inv_depths if prior else None)
 
-    def _render_view(self, b, intr, gt, loss, image=None, prior=None):
+    def _loss(self, rendered, gt, v_out, loss, mask):
+        """The colour loss of `rendered` against gt into `loss` and its gradient into v_out: gsb_ssim_l1_loss, or its
+        masked form over the used pixels of `mask` (D26)."""
+        L, P, H, W = self.L, capi.ptr, self.pipe.H, self.pipe.W
+        off = (-self.ssim_ws.data_ptr()) % 256
+        ws, nbytes = self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off
+        if mask is None:
+            capi.check(L.gsb_ssim_l1_loss(H, W, P(rendered), P(gt), self.ssim_weight, P(v_out), P(loss), ws, nbytes,
+                                          capi.stream()))
+        else:
+            capi.check(L.gsb_ssim_l1_loss_masked(H, W, P(rendered), P(gt), P(mask), self.ssim_weight, P(v_out),
+                                                 P(loss), ws, nbytes, capi.stream()))
+
+    def _render_view(self, b, intr, gt, loss, image=None, prior=None, mask=None):
         """View b's forward pass after _setup_views: _project_blend, then the loss against gt into `loss` ({total, L1,
         SSIM}) and its image gradient into the pipeline's v_img.  With a training image (D21) the loss is taken on
         the render sliced through that image's grid, and the slice backward writes v_img and adds 1/B of the grid
         gradient.  prior (D23): the view's depth prior; the blend also renders the inverse depth (_depth_loss takes
-        its loss)."""
+        its loss).  mask (D26): the view's loss mask; the loss (on the sliced image with a grid) is the masked one."""
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
         H, W = pp.H, pp.W
         self._project_blend(b, intr, prior=prior is not None)
-        off = (-self.ssim_ws.data_ptr()) % 256
         if image is None:
-            capi.check(L.gsb_ssim_l1_loss(H, W, P(pp.out_img), P(gt), self.ssim_weight, P(pp.v_img), P(loss),
-                                          self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off, s))
+            self._loss(pp.out_img, gt, pp.v_img, loss, mask)
             return
         ap = self.appearance
         capi.check(L.gsb_bilagrid_slice_forward(H, W, P(ap.grids[image]), P(pp.out_img), P(self.adj_img), s))
-        capi.check(L.gsb_ssim_l1_loss(H, W, P(self.adj_img), P(gt), self.ssim_weight, P(self.v_adj), P(loss),
-                                      self.ssim_ws.data_ptr() + off, self.ssim_ws.numel() - off, s))
+        self._loss(self.adj_img, gt, self.v_adj, loss, mask)
         woff = (-self.bilagrid_ws.data_ptr()) % 256
         capi.check(L.gsb_bilagrid_slice_backward(H, W, P(ap.grids[image]), P(pp.out_img), P(self.v_adj),
                                                  1.0 / self.views_per_step, P(pp.v_img), P(ap.grad[image]),
