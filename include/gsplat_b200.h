@@ -728,6 +728,34 @@ int gsb_reset_opacity_filter3d(int n, float max_logit, float reset_value, const 
                                const float *filter3d, float *opacities, float *exp_avg, float *exp_avg_sq,
                                gsb_stream_t stream);
 
+/* ---- Fisheye cameras (DESIGN D27) ------------------------------------------------------------------------------------
+ * The activated projection through OpenCV's fisheye model (Kannala-Brandt) in the view frame (x right, y down, +z
+ * forward): t = viewmat (p, 1), theta = atan2(|t.xy|, t.z), theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 +
+ * k4 theta^8), (u, v) = (fx, fy) theta_d / |t.xy| t.xy + (cx, cy) - 0.5.  The EWA covariance takes the full 2x3
+ * Jacobian of (u, v) at t; the 0.3 blur, conic, radius, tile box and the anti-aliased opacity are the pinhole's.  A
+ * Gaussian is culled (as t.z <= clip_thresh culls it) also where theta > theta_lim; theta_lim is the first zero of
+ * d theta_d / d theta in (0, pi/2), else pi/2, in float64 rounded once (model.fisheye_theta_limit).
+ * gsb_project_forward_fisheye: the arguments of gsb_project_forward_activated without projmat, with the distortion
+ *   and theta_lim after cx, cy, and antialiased (0 / 1) before the stream; the same seven outputs.
+ * gsb_project_backward_fisheye: its exact VJP.  opacity_logits are the logits in every mode; accumulate = 1 adds to
+ *   the four outputs; cam_partials != NULL also writes the camera-gradient partial rows of
+ *   gsb_project_backward_activated_camgrad (gsb_project_camera_partials_floats(n) floats) for
+ *   gsb_project_camera_grad_reduce, whose v_projmat is then 0.
+ * Both check fx, fy > 0, finite k1..k4, 0 < theta_lim <= (float)(pi / 2) and the flags. */
+int gsb_project_forward_fisheye(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                const float *raw_quats, const float *opacity_logits, const float *viewmat, float fx,
+                                float fy, float cx, float cy, float k1, float k2, float k3, float k4, float theta_lim,
+                                int img_h, int img_w, int tiles_x, int tiles_y, float clip_thresh, float *cov3d,
+                                float *xys, float *depths, int32_t *radii, float *conics, int32_t *num_tiles_hit,
+                                float *opacities, int antialiased, gsb_stream_t stream);
+int gsb_project_backward_fisheye(int n, const float *means3d, const float *log_scales, float glob_scale,
+                                 const float *raw_quats, const float *opacity_logits, const float *viewmat, float fx,
+                                 float fy, float k1, float k2, float k3, float k4, float theta_lim, int img_h, int img_w,
+                                 const int32_t *radii, const float *conics, const float *v_xy, const float *v_depth,
+                                 const float *v_conic, const float *v_opacity, float *v_mean3d, float *v_log_scales,
+                                 float *v_raw_quats, float *v_opacity_logits, int accumulate, int antialiased,
+                                 float *cam_partials, gsb_stream_t stream);
+
 /* ---- Training images (Camera::loadImage / Camera::getImage, input_data.cpp:40-117) --------------------------------
  * Images are 3-channel u8, [h,w,3] row-major and dense.
  * gsb_resize_area_u8 is cv::resize(src, dst, ..., INTER_AREA) of OpenCV 4's CPU code, byte for byte, for dst_h <= src_h and

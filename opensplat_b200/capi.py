@@ -132,6 +132,14 @@ _SIGS = {
     "gsb_project_backward_activated_filter3d": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _f, _f, _i, _i,
                                                      _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i,
                                                      _vp, _vp]),
+    # D27: n, means, log_scales, glob_scale, raw_quats, logits, viewmat, fx, fy, cx, cy, k1..k4, theta_lim, img_h,
+    # img_w, tiles_x, tiles_y, clip_thresh, 7 outputs, antialiased, stream
+    "gsb_project_forward_fisheye": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _f, _f, _i, _i,
+                                         _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    # n, means, log_scales, glob_scale, raw_quats, logits, viewmat, fx, fy, k1..k4, theta_lim, img_h, img_w, radii,
+    # conics, v_xy, v_depth, v_conic, v_opacity, 4 gradients, accumulate, antialiased, cam_partials, stream
+    "gsb_project_backward_fisheye": (_i, [_i, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _i, _i, _vp,
+                                          _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
     "gsb_filter3d_workspace_bytes": (_sz, []),
     # n, means, num_cameras, cameras, near, margin, variance, workspace, workspace_bytes, filter3d, stream
     "gsb_filter3d_compute": (_i, [_i, _vp, _i, _vp, _f, _f, _f, _vp, _sz, _vp, _vp]),

@@ -39,6 +39,8 @@ class Filter3DConfig:
             raise ValueError("cameras= must be a non-empty sequence of model.Camera")
         if not all(float(c.fx) > 0 and float(c.fy) > 0 and int(c.width) > 0 and int(c.height) > 0 for c in cams):
             raise ValueError("every camera needs fx, fy > 0 and a positive image size")
+        if any(c.model != "pinhole" for c in cams):
+            raise ValueError("the 3-D filter's sampling rate is a pinhole camera's; fisheye cameras are not supported")
         object.__setattr__(self, "cameras", cams)
         for name in ("variance", "near", "margin"):
             v = getattr(self, name)

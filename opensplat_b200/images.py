@@ -29,7 +29,6 @@ import numpy as np
 import torch
 
 from . import capi
-from .model import Camera
 
 UNDISTORT_GRID = 9          # getUndistortRectangles: a 9x9 grid over the image
 UNDISTORT_ITERS = 5         # undistortPoints' default criteria: 5 iterations
@@ -206,7 +205,8 @@ class ImageSet:
             fx, fy, cx, cy = fx * sf, fy * sf, cx * sf, cy * sf
         dist = tuple(f32(v) for v in (cam.k1, cam.k2, cam.p1, cam.p2, cam.k3))
         new_k, roi = None, (0, 0, w, h)
-        if any(d != 0 for d in dist):
+        # a fisheye camera (DESIGN D27) is rendered through its distortion, so its image is not resampled
+        if cam.model == "pinhole" and any(d != 0 for d in dist):
             new_k, roi = get_optimal_new_camera_matrix((fx, fy, cx, cy), dist, (w, h))
             if roi[2] < 1 or roi[3] < 1:
                 raise ValueError(f"the undistorted image of camera {len(self.cameras)} has an empty valid region")
@@ -220,8 +220,7 @@ class ImageSet:
                 mask = m
             img = out
             fx, fy, cx, cy = (f32(v) for v in new_k)
-        self.cameras.append(Camera(img.shape[1], img.shape[0], fx, fy, cx, cy, cam.camToWorld, k1=cam.k1, k2=cam.k2,
-                                   k3=cam.k3, p1=cam.p1, p2=cam.p2))
+        self.cameras.append(cam.replace(width=img.shape[1], height=img.shape[0], fx=fx, fy=fy, cx=cx, cy=cy))
         self.new_k.append(new_k)
         self.roi.append(roi)
         self._levels.append({1: img})

@@ -11,6 +11,7 @@ blend, L1+SSIM loss with gradient, one Adam kernel per tensor, densification sta
 There is no CPU fallback."""
 import math
 
+import numpy as np
 import torch
 
 from . import capi, ops
@@ -30,15 +31,53 @@ def projection_matrix(z_near, z_far, fov_x, fov_y, device):
                          [0.0, 0.0, 1.0, 0.0]], dtype=torch.float32, device=device)
 
 
+CAMERA_MODELS = ("pinhole", "fisheye")
+
+
 class Camera:
     """The fields of the reference's Camera that Model::forward reads (input_data.hpp:12-44), and its distortion
-    coefficients k1, k2, k3, p1, p2, which Camera::loadImage (images.ImageSet) undistorts the image with."""
+    coefficients k1, k2, k3, p1, p2, which Camera::loadImage (images.ImageSet) undistorts the image with.
+    model="fisheye" (DESIGN D27): an OpenCV fisheye (Kannala-Brandt) camera with coefficients k1..k4, which
+    SplatTrainer renders through directly (COLMAP's OPENCV_FISHEYE; RADIAL_FISHEYE is k1, k2 with fx = fy,
+    SIMPLE_RADIAL_FISHEYE k1 alone).  A fisheye camera has p1 = p2 = 0, a pinhole camera k4 = 0."""
 
-    def __init__(self, width, height, fx, fy, cx, cy, cam_to_world, k1=0.0, k2=0.0, k3=0.0, p1=0.0, p2=0.0):
+    def __init__(self, width, height, fx, fy, cx, cy, cam_to_world, k1=0.0, k2=0.0, k3=0.0, p1=0.0, p2=0.0, k4=0.0,
+                 model="pinhole"):
+        if model not in CAMERA_MODELS:
+            raise ValueError(f"Camera model must be one of {CAMERA_MODELS}, got {model!r}")
+        if model == "fisheye" and (float(p1) != 0.0 or float(p2) != 0.0):
+            raise ValueError("a fisheye camera has no tangential distortion (p1 = p2 = 0)")
+        if model == "pinhole" and float(k4) != 0.0:
+            raise ValueError("k4 is a fisheye coefficient; a pinhole camera takes k4 = 0")
         self.width, self.height = int(width), int(height)
         self.fx, self.fy, self.cx, self.cy = float(fx), float(fy), float(cx), float(cy)
         self.camToWorld = torch.as_tensor(cam_to_world, dtype=torch.float32)
         self.k1, self.k2, self.k3, self.p1, self.p2 = float(k1), float(k2), float(k3), float(p1), float(p2)
+        self.k4, self.model = float(k4), model
+
+    def replace(self, **kw):
+        """A copy with the given constructor arguments changed; the model and every coefficient carry over."""
+        a = dict(width=self.width, height=self.height, fx=self.fx, fy=self.fy, cx=self.cx, cy=self.cy,
+                 cam_to_world=self.camToWorld, k1=self.k1, k2=self.k2, k3=self.k3, p1=self.p1, p2=self.p2, k4=self.k4,
+                 model=self.model)
+        a.update(kw)
+        return Camera(**a)
+
+
+def fisheye_theta_limit(k1, k2, k3, k4):
+    """DESIGN D27: the largest incidence angle theta a fisheye camera with coefficients k1..k4 renders, as float32:
+    the first root of d theta_d / d theta = 1 + 3 k1 t^2 + 5 k2 t^4 + 7 k3 t^6 + 9 k4 t^8 in (0, pi/2) if there is
+    one, else pi/2, found in float64 and rounded once.  Beyond it theta_d folds back and the image overlaps itself."""
+    half_pi = 0.5 * math.pi
+    k = [float(v) for v in (k1, k2, k3, k4)]
+    if not all(math.isfinite(v) for v in k):
+        raise ValueError("the fisheye coefficients must be finite")
+    # d theta_d / d theta as a polynomial in x = theta^2, highest power first.  Where it touches 0 without crossing (a
+    # double root, theta_d stops growing there) np.roots returns a conjugate pair whose imaginary parts are about
+    # sqrt(eps) |x| ~ 1e-8 |x|, so a root counts as real up to 1e-6 |x|.
+    c = np.trim_zeros([9.0 * k[3], 7.0 * k[2], 5.0 * k[1], 3.0 * k[0], 1.0], "f")
+    x = [r.real for r in np.roots(c) if abs(r.imag) <= 1e-6 * abs(r) and 0.0 < r.real < half_pi * half_pi]
+    return float(np.float32(math.sqrt(min(x)) if x else half_pi))
 
 
 # learning rates of Model::setupOptimizers (model.cpp:58-70)
@@ -159,6 +198,9 @@ class GaussianModel:
 
     # ---- Model::forward (model.cpp:83-225) ------------------------------------------------------------------
     def forward(self, cam, step):
+        if cam.model != "pinhole":
+            raise ValueError("GaussianModel renders pinhole cameras, as the reference's Model does; fisheye cameras "
+                             "(DESIGN D27) render in trainer.SplatTrainer")
         dev = self.device
         height, width, (fx, fy, cx, cy), view, proj, cam_pos = camera_setup(cam, self.get_downscale_factor(step))
         self.lastHeight, self.lastWidth = height, width

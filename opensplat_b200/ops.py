@@ -733,6 +733,77 @@ class ProjectGaussiansActivatedAntialiased(ProjectGaussiansActivated):
                                                   clipThresh, filter3D)
 
 
+class ProjectGaussiansFisheye(torch.autograd.Function):
+    """ProjectGaussiansActivated through an OpenCV fisheye camera (DESIGN D27, gsb_project_forward_fisheye): the same
+    outputs, with the pixel centre and the EWA Jacobian of the Kannala-Brandt map of the view-space mean.  k: the four
+    distortion coefficients (k1, k2, k3, k4); thetaLim: model.fisheye_theta_limit(*k), beyond which a Gaussian is
+    culled.  antialiased: the opacity of ProjectGaussiansActivatedAntialiased.  Gradients come back w.r.t. the raw
+    parameters, and w.r.t. viewMat when it requires grad (there is no projMat)."""
+
+    @staticmethod
+    def forward(ctx, means, logScales, globScale, rawQuats, opacityLogits, viewMat, fx, fy, cx, cy, k, thetaLim,
+                imgHeight, imgWidth, tileBounds, clipThresh=0.01, antialiased=False):
+        n = means.shape[0]
+        m3, ls, rq = capi.f32(means), capi.f32(logScales), capi.f32(rawQuats)
+        ol = capi.f32(opacityLogits).reshape(n)
+        vm = capi.f32(viewMat)
+        k = tuple(float(x) for x in k)
+        if len(k) != 4:
+            raise ValueError("k takes the four fisheye coefficients (k1, k2, k3, k4)")
+        cov3d = _empty((n, 6), torch.float32, m3)
+        xys = _empty((n, 2), torch.float32, m3)
+        depths = _empty((n,), torch.float32, m3)
+        radii = _empty((n,), torch.int32, m3)
+        conics = _empty((n, 3), torch.float32, m3)
+        nth = _empty((n,), torch.int32, m3)
+        opac = _empty((n, 1), torch.float32, m3)
+        aa = bool(antialiased)
+        capi.check(capi.lib().gsb_project_forward_fisheye(
+            n, capi.ptr(m3), capi.ptr(ls), float(globScale), capi.ptr(rq), capi.ptr(ol), capi.ptr(vm), float(fx),
+            float(fy), float(cx), float(cy), *k, float(thetaLim), int(imgHeight), int(imgWidth), tileBounds[0],
+            tileBounds[1], float(clipThresh), capi.ptr(cov3d), capi.ptr(xys), capi.ptr(depths), capi.ptr(radii),
+            capi.ptr(conics), capi.ptr(nth), capi.ptr(opac), int(aa), capi.stream()))
+        ctx.meta = (float(globScale), float(fx), float(fy), k, float(thetaLim), int(imgHeight), int(imgWidth),
+                    tuple(opacityLogits.shape), aa, tuple(viewMat.shape))
+        ctx.save_for_backward(m3, ls, rq, ol, vm, radii, conics)
+        ctx.mark_non_differentiable(radii, nth)
+        return xys, depths, radii, conics, nth, cov3d, opac
+
+    @staticmethod
+    def backward(ctx, v_xys, v_depths, v_radii, v_conics, v_numTiles, v_cov3d, v_opac):
+        m3, ls, rq, ol, vm, radii, conics = ctx.saved_tensors
+        gs, fx, fy, k, th, H, W, ol_shape, aa, vm_shape = ctx.meta
+        n = m3.shape[0]
+        if v_xys is None:
+            v_xys = torch.zeros_like(m3[:, :2])
+        if v_conics is None:
+            v_conics = torch.zeros_like(conics)
+        v_mean = _empty((n, 3), torch.float32, m3)
+        v_ls = _empty((n, 3), torch.float32, m3)
+        v_rq = _empty((n, 4), torch.float32, m3)
+        v_ol = _empty((n,), torch.float32, m3)
+        vx, vc = capi.f32(v_xys), capi.f32(v_conics)
+        vd = capi.f32(v_depths) if v_depths is not None else None
+        vo = capi.f32(v_opac).reshape(n) if v_opac is not None else None
+        L = capi.lib()
+        camgrad = ctx.needs_input_grad[5]
+        part = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, m3) if camgrad else None
+        capi.check(L.gsb_project_backward_fisheye(
+            n, capi.ptr(m3), capi.ptr(ls), gs, capi.ptr(rq), capi.ptr(ol), capi.ptr(vm), fx, fy, *k, th, H, W,
+            capi.ptr(radii), capi.ptr(conics), capi.ptr(vx), capi.ptr(vd), capi.ptr(vc), capi.ptr(vo),
+            capi.ptr(v_mean), capi.ptr(v_ls), capi.ptr(v_rq), capi.ptr(v_ol), 0, int(aa), capi.ptr(part),
+            capi.stream()))
+        v_view = None
+        if camgrad:
+            v_view = _empty((4, 4), torch.float32, m3)
+            v_proj = _empty((4, 4), torch.float32, m3)
+            capi.check(L.gsb_project_camera_grad_reduce(part.numel() // capi.CAMGRAD_TERMS, capi.ptr(part),
+                                                        capi.ptr(v_view), capi.ptr(v_proj), capi.stream()))
+            v_view = v_view.reshape(vm_shape)
+        # 17 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4), viewMat(5)
+        return (v_mean, v_ls, None, v_rq, v_ol.reshape(ol_shape), v_view) + (None,) * 11
+
+
 class SphericalHarmonics(torch.autograd.Function):
     @staticmethod
     def forward(ctx, degreesToUse, viewDirs, coeffs):

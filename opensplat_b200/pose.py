@@ -15,7 +15,6 @@ from dataclasses import dataclass
 import torch
 
 from . import capi
-from .model import Camera
 
 
 @dataclass
@@ -71,8 +70,7 @@ def adjusted_camera(cam, delta):
     D[:3, :3] = F @ rot6d(e[3:9]) @ F
     D[:3, 3] = F @ e[0:3]
     c2w = torch.as_tensor(cam.camToWorld, dtype=torch.float64) @ D
-    return Camera(cam.width, cam.height, cam.fx, cam.fy, cam.cx, cam.cy, c2w.float(), k1=cam.k1, k2=cam.k2, k3=cam.k3,
-                  p1=cam.p1, p2=cam.p2)
+    return cam.replace(cam_to_world=c2w.float())
 
 
 class Poses:

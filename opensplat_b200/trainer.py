@@ -113,6 +113,7 @@ from .depth import DepthConfig, depth_weight
 from .filter3d import Filter3DConfig, bake, camera_table, compute_filter3d, recompute_due
 from .mcmc import MCMCConfig, MCMCRefiner
 from .model import (LEARNING_RATES, MEANS_LR_INIT, PARAM_NAMES, Camera, camera_setup, downscale_factor,
+                    fisheye_theta_limit,
                     means_learning_rate)
 from .parallel import flat_views
 from .pipeline import SplatPipeline
@@ -211,7 +212,9 @@ class SplatTrainer:
         depth: a depth.DepthConfig to supervise the rendered inverse depth with per-image priors (DESIGN D23); step()
         then takes depth=.
         filter3d: a filter3d.Filter3DConfig to train and render with Mip-Splatting's 3-D smoothing filter (DESIGN
-        D24) from its training cameras; save() then writes the baked scene."""
+        D24) from its training cameras; save() then writes the baked scene.  Not available with fisheye cameras.
+        Cameras: step(), evaluate() and render() take pinhole and fisheye (model.Camera(model="fisheye"), DESIGN D27)
+        cameras, mixed freely within a step; a fisheye view's projection is gsb_project_{forward,backward}_fisheye."""
         import torch.distributed as dist
         self.views_per_step = B = int(views_per_step)
         if B < 1:
@@ -235,6 +238,8 @@ class SplatTrainer:
         self.device = torch.device(device)
         self.cfg = cfg or RefineConfig()
         self.antialiased = bool(antialiased)
+        self.view_fisheye = []     # D27: per view of the last _setup_views, (k1, k2, k3, k4, theta_lim) or None
+        self._theta_lims = {}
         t = {k: torch.as_tensor(params[k]).to(device=self.device, dtype=torch.float32) for k in PARAM_NAMES}
         n, k_bases = t["means"].shape[0], t["featuresRest"].shape[1] + 1
         self.sh_degree = ops.deg_from_sh(k_bases) if sh_degree is None else int(sh_degree)
@@ -617,6 +622,7 @@ class SplatTrainer:
         has it.  Returns (setups, H, W, use): use is the step's SH degrees_to_use."""
         setups, H, W = checked or view_setups(cams, gts, views, downscale_factor(step, self.num_downscales,
                                                                                   self.resolution_schedule))
+        self.view_fisheye = [self._fisheye(c) for c in ([cams] if isinstance(cams, Camera) else cams)]
         if (W, H) != self.resolution:
             self._set_resolution(W, H)
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
@@ -643,6 +649,17 @@ class SplatTrainer:
                                                           P(p["coeffs"]), 0.5, P(self.rgbs_views), s))
         return setups, H, W, use
 
+    def _fisheye(self, cam):
+        """D27: a view's fisheye arguments (k1, k2, k3, k4, theta_lim), None for a pinhole camera."""
+        if cam.model == "pinhole":
+            return None
+        if self.filter3d_cfg is not None:
+            raise ValueError("the 3-D filter (filter3d=) is not available with fisheye cameras")
+        k = (cam.k1, cam.k2, cam.k3, cam.k4)
+        if k not in self._theta_lims:
+            self._theta_lims[k] = fisheye_theta_limit(*k)
+        return k + (self._theta_lims[k],)
+
     def _project_blend(self, b, intr, out_img=None, out_depth=None, out_alpha=None, prior=False):
         """View b's projection with the activations from camera slot b (intrinsics `intr`), then binning and the
         clamped blend (the view's one host wait) into the pipeline's image, or into out_img with the depth and opacity
@@ -653,7 +670,11 @@ class SplatTrainer:
         head = (n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]))
         tail = (P(self.viewmats[b]), P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d),
                 P(pp.xys), P(pp.depths), P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac))
-        if self.filter3d_cfg is not None:     # D24
+        fish = self.view_fisheye[b]
+        if fish is not None:     # D27: no projmat; the distortion after the intrinsics
+            capi.check(L.gsb_project_forward_fisheye(*head, tail[0], *tail[2:6], *fish, *tail[6:],
+                                                     int(self.antialiased), s))
+        elif self.filter3d_cfg is not None:     # D24
             capi.check(L.gsb_project_forward_activated_filter3d(*head, P(self.f3d), *tail, int(self.antialiased), s))
         else:
             project = L.gsb_project_forward_activated_aa if self.antialiased else L.gsb_project_forward_activated
@@ -741,8 +762,12 @@ class SplatTrainer:
         args = (n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(opac), P(self.viewmats[b]),
                 P(self.projmats[b]), fx, fy, pp.H, pp.W, P(pp.radii), P(pp.conics), P(pp.v_xy), P(v_depth),
                 P(pp.v_conic), P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]))
-        s, po = capi.stream(), self.poses
-        if self.filter3d_cfg is not None:     # D24: the filter after the logits; accumulate, antialiased, camgrad
+        s, po, fish = capi.stream(), self.poses, self.view_fisheye[b]
+        if fish is not None:     # D27: the logits in every mode, no projmat; accumulate, antialiased, cam_partials
+            capi.check(L.gsb_project_backward_fisheye(
+                *args[:5], P(p["opacities"]), args[6], fx, fy, *fish, *args[10:], int(b > 0), int(self.antialiased),
+                P(self.cam_partials) if po is not None else None, s))
+        elif self.filter3d_cfg is not None:     # D24: the filter after the logits; accumulate, antialiased, camgrad
             capi.check(L.gsb_project_backward_activated_filter3d(
                 *args[:6], P(self.f3d), *args[6:], int(b > 0), int(self.antialiased), int(po is not None),
                 P(self.cam_partials) if po is not None else None, s))
