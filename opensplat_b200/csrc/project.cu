@@ -17,6 +17,8 @@
 // clamp sub-gradient, which the reference's hand-written CUDA VJP drops (SURVEY.md 8c D8/D11/D12).
 #include "gsb_common.cuh"
 
+#include <type_traits>
+
 namespace {
 
 constexpr int PJ_THREADS = 256;
@@ -672,36 +674,106 @@ camgrad_reduce_kernel(int nblocks, const float *__restrict__ partials, float *__
 
 }  // namespace
 
-static int project_forward_impl(bool act, bool aa, int n, const float *means3d, const float *scales, float glob_scale,
-                                const float *quats, const float *opacity_logits, const float *filter3d,
-                                const float *viewmat,
-                                const float *projmat, float fx, float fy, float cx, float cy, int img_h, int img_w,
-                                int tiles_x, int tiles_y, float clip_thresh, float *cov3d, float *xys, float *depths,
-                                int32_t *radii, float *conics, int32_t *num_tiles_hit, float *opacities,
-                                gsb_stream_t stream, const FishK *fish = nullptr) {
-    GSB_CHECK_ARG(n >= 0 && img_h > 0 && img_w > 0 && tiles_x > 0 && tiles_y > 0);
-    if (n == 0) return 0;
-    GSB_CHECK_ARG(means3d && scales && quats && viewmat && (projmat || fish) && cov3d && xys && depths && radii &&
-                  conics && num_tiles_hit);
-    GSB_CHECK_ARG(!act || (opacity_logits && opacities));
-    GSB_CHECK_ARG(((uintptr_t)quats % 16) == 0 && ((uintptr_t)xys % 8) == 0);
+// A projection mode: the kernels' template flags (ACC and CAMGRAD are the backward's only).
+enum : unsigned { PJ_ACT = 1, PJ_AA = 2, PJ_F3D = 4, PJ_FISH = 8, PJ_ACC = 16, PJ_CAMGRAD = 32 };
+
+static unsigned pj_flag(int on, unsigned flag) { return on ? flag : 0u; }
+
+// The modes the kernels' static_asserts allow: AA, F3D, FISH, ACC and CAMGRAD need ACT, and FISH excludes F3D.  Each
+// launcher checks its call's mode against it and instantiates exactly the modes it allows.
+constexpr bool pj_legal(bool act, bool acc, bool aa, bool camgrad, bool f3d, bool fish) {
+    return (act || !(acc || aa || camgrad || f3d || fish)) && !(f3d && fish);
+}
+
+// f(std::bool_constant<b>...) for the run-time flags b...: the one place a mode becomes template arguments.
+template <class F> static void pj_with_flags(F &&f) { f(); }
+template <class F, class... R> static void pj_with_flags(F &&f, bool b, R... rest) {
+    if (b) pj_with_flags([&](auto... c) { f(std::true_type{}, c...); }, rest...);
+    else pj_with_flags([&](auto... c) { f(std::false_type{}, c...); }, rest...);
+}
+
+// One call of project_forward_kernel as the extern "C" wrappers describe it: the mode (PJ_ACT, PJ_AA, PJ_F3D,
+// PJ_FISH), then the kernel's pointers and scalars.  opacity_logits and opacities are read under ACT, filter3d under
+// F3D and fk under FISH, where projmat is NULL.
+struct ProjectForward {
+    unsigned mode;
+    int n;
+    const float *means3d, *scales;
+    float glob_scale;
+    const float *quats, *opacity_logits, *filter3d, *viewmat, *projmat;
+    float fx, fy, cx, cy;
+    int img_h, img_w, tiles_x, tiles_y;
+    float clip_thresh;
+    float *cov3d, *xys, *depths;
+    int32_t *radii;
+    float *conics;
+    int32_t *num_tiles_hit;
+    float *opacities;
+    FishK fk;
+};
+
+static int project_forward(const ProjectForward &c, gsb_stream_t stream) {
+    const unsigned m = c.mode;
+    GSB_CHECK_ARG(pj_legal(m & PJ_ACT, false, m & PJ_AA, false, m & PJ_F3D, m & PJ_FISH));
+    GSB_CHECK_ARG(c.n >= 0 && c.img_h > 0 && c.img_w > 0 && c.tiles_x > 0 && c.tiles_y > 0);
+    if (c.n == 0) return 0;
+    GSB_CHECK_ARG(c.means3d && c.scales && c.quats && c.viewmat && (c.projmat || (m & PJ_FISH)) && c.cov3d && c.xys &&
+                  c.depths && c.radii && c.conics && c.num_tiles_hit);
+    GSB_CHECK_ARG(!(m & PJ_ACT) || (c.opacity_logits && c.opacities));
+    GSB_CHECK_ARG(((uintptr_t)c.quats % 16) == 0 && ((uintptr_t)c.xys % 8) == 0);
     // forward.cu:69-70 evaluates `0.5 * img_size.x / fx` in double and narrows
-    const float tan_fovx = (float)(0.5 * (double)img_w / (double)fx);
-    const float tan_fovy = (float)(0.5 * (double)img_h / (double)fy);
-#define GSB_PJ_F(A, AA, F3D) project_forward_kernel<A, AA, F3D><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
-        n, means3d, scales, glob_scale, quats, viewmat, projmat, fx, fy, cx, cy, tan_fovx, tan_fovy, img_h, img_w,   \
-        tiles_x, tiles_y, clip_thresh, cov3d, reinterpret_cast<float2 *>(xys), depths, radii, conics, num_tiles_hit, \
-        opacity_logits, opacities, filter3d)
-#define GSB_PJ_FISH(AA) project_forward_kernel<true, AA, false, true><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
-        n, means3d, scales, glob_scale, quats, viewmat, nullptr, fx, fy, cx, cy, tan_fovx, tan_fovy, img_h, img_w,    \
-        tiles_x, tiles_y, clip_thresh, cov3d, reinterpret_cast<float2 *>(xys), depths, radii, conics, num_tiles_hit, \
-        opacity_logits, opacities, nullptr, *fish)
-    if (fish) { if (aa) GSB_PJ_FISH(true); else GSB_PJ_FISH(false); }
-    else if (filter3d) { if (aa) GSB_PJ_F(true, true, true); else GSB_PJ_F(true, false, true); }
-    else if (aa) GSB_PJ_F(true, true, false); else if (act) GSB_PJ_F(true, false, false);
-    else GSB_PJ_F(false, false, false);
-#undef GSB_PJ_FISH
-#undef GSB_PJ_F
+    const float tan_fovx = (float)(0.5 * (double)c.img_w / (double)c.fx);
+    const float tan_fovy = (float)(0.5 * (double)c.img_h / (double)c.fy);
+    pj_with_flags([&](auto act, auto aa, auto f3d, auto fish) {
+        if constexpr (pj_legal(act, false, aa, false, f3d, fish))
+            project_forward_kernel<act, aa, f3d, fish>
+                <<<gsb_div_up(c.n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>(
+                    c.n, c.means3d, c.scales, c.glob_scale, c.quats, c.viewmat, c.projmat, c.fx, c.fy, c.cx, c.cy,
+                    tan_fovx, tan_fovy, c.img_h, c.img_w, c.tiles_x, c.tiles_y, c.clip_thresh, c.cov3d,
+                    reinterpret_cast<float2 *>(c.xys), c.depths, c.radii, c.conics, c.num_tiles_hit, c.opacity_logits,
+                    c.opacities, c.filter3d, c.fk);
+    }, m & PJ_ACT, m & PJ_AA, m & PJ_F3D, m & PJ_FISH);
+    GSB_LAUNCH_CHECK();
+    return 0;
+}
+
+// One call of project_backward_kernel: the mode (PJ_ACT, PJ_ACC, PJ_AA, PJ_CAMGRAD, PJ_F3D, PJ_FISH), then the
+// kernel's pointers and scalars.  `opacities` holds sigmoid(logits) for ACT alone and the logits in every other
+// activated mode; cam_partials is written under CAMGRAD.
+struct ProjectBackward {
+    unsigned mode;
+    int n;
+    const float *means3d, *scales;
+    float glob_scale;
+    const float *quats, *opacities, *filter3d, *viewmat, *projmat;
+    float fx, fy;
+    int img_h, img_w;
+    const int32_t *radii;
+    const float *conics, *v_xy, *v_depth, *v_conic, *v_opacity;
+    float *v_mean3d, *v_scale, *v_quat, *v_opacity_logits, *cam_partials;
+    FishK fk;
+};
+
+static int project_backward(const ProjectBackward &c, gsb_stream_t stream) {
+    const unsigned m = c.mode;
+    GSB_CHECK_ARG(pj_legal(m & PJ_ACT, m & PJ_ACC, m & PJ_AA, m & PJ_CAMGRAD, m & PJ_F3D, m & PJ_FISH));
+    GSB_CHECK_ARG(c.n >= 0 && c.img_h > 0 && c.img_w > 0);
+    if (c.n == 0) return 0;
+    GSB_CHECK_ARG(c.means3d && c.scales && c.quats && c.viewmat && (c.projmat || (m & PJ_FISH)) && c.radii &&
+                  c.conics && c.v_xy && c.v_conic && c.v_mean3d && c.v_scale && c.v_quat);
+    GSB_CHECK_ARG(!(m & PJ_ACT) || (c.opacities && c.v_opacity_logits));
+    GSB_CHECK_ARG(((uintptr_t)c.quats % 16) == 0 && ((uintptr_t)c.v_quat % 16) == 0 && ((uintptr_t)c.v_xy % 8) == 0);
+    const float tan_fovx = (float)(0.5 * (double)c.img_w / (double)c.fx);
+    const float tan_fovy = (float)(0.5 * (double)c.img_h / (double)c.fy);
+    pj_with_flags([&](auto act, auto acc, auto aa, auto camgrad, auto f3d, auto fish) {
+        if constexpr (pj_legal(act, acc, aa, camgrad, f3d, fish))
+            project_backward_kernel<act, acc, aa, camgrad, f3d, fish>
+                <<<gsb_div_up(c.n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>(
+                    c.n, c.means3d, c.scales, c.glob_scale, c.quats, c.viewmat, c.projmat, c.fx, c.fy, tan_fovx,
+                    tan_fovy, c.img_h, c.img_w, c.radii, c.conics, reinterpret_cast<const float2 *>(c.v_xy), c.v_depth,
+                    c.v_conic, c.v_mean3d, c.v_scale, reinterpret_cast<float4 *>(c.v_quat), c.opacities, c.v_opacity,
+                    c.v_opacity_logits, c.cam_partials, c.filter3d, c.fk);
+    }, m & PJ_ACT, m & PJ_ACC, m & PJ_AA, m & PJ_CAMGRAD, m & PJ_F3D, m & PJ_FISH);
     GSB_LAUNCH_CHECK();
     return 0;
 }
@@ -712,9 +784,9 @@ extern "C" int gsb_project_forward(int n, const float *means3d, const float *sca
                                    int tiles_x, int tiles_y, float clip_thresh, float *cov3d, float *xys,
                                    float *depths, int32_t *radii, float *conics, int32_t *num_tiles_hit,
                                    gsb_stream_t stream) {
-    return project_forward_impl(false, false, n, means3d, scales, glob_scale, quats, nullptr, nullptr, viewmat, projmat, fx, fy, cx,
-                                cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii, conics,
-                                num_tiles_hit, nullptr, stream);
+    return project_forward({0, n, means3d, scales, glob_scale, quats, nullptr, nullptr, viewmat, projmat, fx, fy, cx,
+                            cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii, conics,
+                            num_tiles_hit, nullptr}, stream);
 }
 
 extern "C" int gsb_project_forward_activated(int n, const float *means3d, const float *log_scales, float glob_scale,
@@ -724,60 +796,9 @@ extern "C" int gsb_project_forward_activated(int n, const float *means3d, const 
                                              float clip_thresh, float *cov3d, float *xys, float *depths,
                                              int32_t *radii, float *conics, int32_t *num_tiles_hit,
                                              float *opacities, gsb_stream_t stream) {
-    return project_forward_impl(true, false, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, nullptr, viewmat, projmat,
-                                fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii,
-                                conics, num_tiles_hit, opacities, stream);
-}
-
-static int project_backward_impl(bool act, bool acc, bool aa, int n, const float *means3d, const float *scales, float glob_scale,
-                                 const float *quats, const float *opacities, const float *viewmat,
-                                 const float *projmat, float fx, float fy, int img_h, int img_w,
-                                 const int32_t *radii, const float *conics, const float *v_xy, const float *v_depth,
-                                 const float *v_conic, const float *v_opacity, float *v_mean3d, float *v_scale,
-                                 float *v_quat, float *v_opacity_logits, float *cam_partials, gsb_stream_t stream,
-                                 const float *filter3d = nullptr, const FishK *fish = nullptr) {
-    GSB_CHECK_ARG(n >= 0 && img_h > 0 && img_w > 0);
-    if (n == 0) return 0;
-    GSB_CHECK_ARG(means3d && scales && quats && viewmat && (projmat || fish) && radii && conics && v_xy && v_conic &&
-                  v_mean3d && v_scale && v_quat);
-    GSB_CHECK_ARG(!act || (opacities && v_opacity_logits));
-    GSB_CHECK_ARG(((uintptr_t)quats % 16) == 0 && ((uintptr_t)v_quat % 16) == 0 && ((uintptr_t)v_xy % 8) == 0);
-    const float tan_fovx = (float)(0.5 * (double)img_w / (double)fx);
-    const float tan_fovy = (float)(0.5 * (double)img_h / (double)fy);
-#define GSB_PJ_B5(A, ACC, AA, CG, F3D) project_backward_kernel<A, ACC, AA, CG, F3D><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
-        n, means3d, scales, glob_scale, quats, viewmat, projmat, fx, fy, tan_fovx, tan_fovy, img_h, img_w, radii,     \
-        conics, reinterpret_cast<const float2 *>(v_xy), v_depth, v_conic, v_mean3d, v_scale,                          \
-        reinterpret_cast<float4 *>(v_quat), opacities, v_opacity, v_opacity_logits, cam_partials, filter3d)
-#define GSB_PJ_B(A, ACC, AA, CG) GSB_PJ_B5(A, ACC, AA, CG, false)
-#define GSB_PJ_BF(ACC, AA, CG) GSB_PJ_B5(true, ACC, AA, CG, true)
-#define GSB_PJ_BK(ACC, AA, CG) project_backward_kernel<true, ACC, AA, CG, false, true><<<gsb_div_up(n, PJ_THREADS), PJ_THREADS, 0, (cudaStream_t)stream>>>( \
-        n, means3d, scales, glob_scale, quats, viewmat, nullptr, fx, fy, tan_fovx, tan_fovy, img_h, img_w, radii,     \
-        conics, reinterpret_cast<const float2 *>(v_xy), v_depth, v_conic, v_mean3d, v_scale,                          \
-        reinterpret_cast<float4 *>(v_quat), opacities, v_opacity, v_opacity_logits, cam_partials, nullptr, *fish)
-    if (fish) {
-        if (cam_partials) {
-            if (aa) { if (acc) GSB_PJ_BK(true, true, true); else GSB_PJ_BK(false, true, true); }
-            else if (acc) GSB_PJ_BK(true, false, true); else GSB_PJ_BK(false, false, true);
-        } else if (aa) { if (acc) GSB_PJ_BK(true, true, false); else GSB_PJ_BK(false, true, false); }
-        else if (acc) GSB_PJ_BK(true, false, false); else GSB_PJ_BK(false, false, false);
-    } else if (filter3d) {
-        if (cam_partials) {
-            if (aa) { if (acc) GSB_PJ_BF(true, true, true); else GSB_PJ_BF(false, true, true); }
-            else if (acc) GSB_PJ_BF(true, false, true); else GSB_PJ_BF(false, false, true);
-        } else if (aa) { if (acc) GSB_PJ_BF(true, true, false); else GSB_PJ_BF(false, true, false); }
-        else if (acc) GSB_PJ_BF(true, false, false); else GSB_PJ_BF(false, false, false);
-    } else if (cam_partials) {
-        if (aa) { if (acc) GSB_PJ_B(true, true, true, true); else GSB_PJ_B(true, false, true, true); }
-        else if (acc) GSB_PJ_B(true, true, false, true); else GSB_PJ_B(true, false, false, true);
-    } else if (aa) { if (acc) GSB_PJ_B(true, true, true, false); else GSB_PJ_B(true, false, true, false); }
-    else if (acc) GSB_PJ_B(true, true, false, false); else if (act) GSB_PJ_B(true, false, false, false);
-    else GSB_PJ_B(false, false, false, false);
-#undef GSB_PJ_BK
-#undef GSB_PJ_BF
-#undef GSB_PJ_B
-#undef GSB_PJ_B5
-    GSB_LAUNCH_CHECK();
-    return 0;
+    return project_forward({PJ_ACT, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, nullptr, viewmat,
+                            projmat, fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys, depths,
+                            radii, conics, num_tiles_hit, opacities}, stream);
 }
 
 extern "C" int gsb_project_backward(int n, const float *means3d, const float *scales, float glob_scale,
@@ -787,9 +808,9 @@ extern "C" int gsb_project_backward(int n, const float *means3d, const float *sc
                                     const float *v_xy, const float *v_depth, const float *v_conic,
                                     float *v_mean3d, float *v_scale, float *v_quat, gsb_stream_t stream) {
     (void)cov3d; (void)cx; (void)cy;
-    return project_backward_impl(false, false, false, n, means3d, scales, glob_scale, quats, nullptr, viewmat, projmat, fx,
-                                 fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, nullptr, v_mean3d, v_scale,
-                                 v_quat, nullptr, nullptr, stream);
+    return project_backward({0, n, means3d, scales, glob_scale, quats, nullptr, nullptr, viewmat, projmat, fx, fy,
+                             img_h, img_w, radii, conics, v_xy, v_depth, v_conic, nullptr, v_mean3d, v_scale, v_quat,
+                             nullptr, nullptr}, stream);
 }
 
 extern "C" int gsb_project_backward_activated(int n, const float *means3d, const float *log_scales, float glob_scale,
@@ -799,9 +820,9 @@ extern "C" int gsb_project_backward_activated(int n, const float *means3d, const
                                               const float *v_depth, const float *v_conic, const float *v_opacity,
                                               float *v_mean3d, float *v_log_scales, float *v_raw_quats,
                                               float *v_opacity_logits, gsb_stream_t stream) {
-    return project_backward_impl(true, false, false, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
-                                 projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
-                                 v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr, stream);
+    return project_backward({PJ_ACT, n, means3d, log_scales, glob_scale, raw_quats, opacities, nullptr, viewmat,
+                             projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity, v_mean3d,
+                             v_log_scales, v_raw_quats, v_opacity_logits, nullptr}, stream);
 }
 
 // The same VJP added into the four outputs (v += vjp): a trainer's several views of one step summed in place.
@@ -812,9 +833,9 @@ extern "C" int gsb_project_backward_activated_acc(int n, const float *means3d, c
                                                   const float *v_xy, const float *v_depth, const float *v_conic,
                                                   const float *v_opacity, float *v_mean3d, float *v_log_scales,
                                                   float *v_raw_quats, float *v_opacity_logits, gsb_stream_t stream) {
-    return project_backward_impl(true, true, false, n, means3d, log_scales, glob_scale, raw_quats, opacities, viewmat,
-                                 projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
-                                 v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr, stream);
+    return project_backward({PJ_ACT | PJ_ACC, n, means3d, log_scales, glob_scale, raw_quats, opacities, nullptr,
+                             viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
+                             v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr}, stream);
 }
 
 // D19: the activated projection with the anti-aliased opacity, opacities = sigmoid(logits) * comp.
@@ -825,9 +846,9 @@ extern "C" int gsb_project_forward_activated_aa(int n, const float *means3d, con
                                                 float clip_thresh, float *cov3d, float *xys, float *depths,
                                                 int32_t *radii, float *conics, int32_t *num_tiles_hit,
                                                 float *opacities, gsb_stream_t stream) {
-    return project_forward_impl(true, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, nullptr, viewmat,
-                                projmat, fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys,
-                                depths, radii, conics, num_tiles_hit, opacities, stream);
+    return project_forward({PJ_ACT | PJ_AA, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, nullptr,
+                            viewmat, projmat, fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh, cov3d, xys,
+                            depths, radii, conics, num_tiles_hit, opacities}, stream);
 }
 
 // Its VJP, from the opacity logits (the forward's opacities hold sigmoid * comp): written, and added in place.
@@ -839,9 +860,9 @@ extern "C" int gsb_project_backward_activated_aa(int n, const float *means3d, co
                                                  const float *v_depth, const float *v_conic, const float *v_opacity,
                                                  float *v_mean3d, float *v_log_scales, float *v_raw_quats,
                                                  float *v_opacity_logits, gsb_stream_t stream) {
-    return project_backward_impl(true, false, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
-                                 viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic,
-                                 v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr, stream);
+    return project_backward({PJ_ACT | PJ_AA, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, nullptr,
+                             viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity,
+                             v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr}, stream);
 }
 
 extern "C" int gsb_project_backward_activated_aa_acc(int n, const float *means3d, const float *log_scales,
@@ -853,9 +874,9 @@ extern "C" int gsb_project_backward_activated_aa_acc(int n, const float *means3d
                                                      const float *v_opacity, float *v_mean3d, float *v_log_scales,
                                                      float *v_raw_quats, float *v_opacity_logits,
                                                      gsb_stream_t stream) {
-    return project_backward_impl(true, true, true, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
-                                 viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic,
-                                 v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr, stream);
+    return project_backward({PJ_ACT | PJ_ACC | PJ_AA, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
+                             nullptr, viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic,
+                             v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits, nullptr}, stream);
 }
 
 // D22: the activated projection backward (any of the four variants above: accumulate = the _acc form, antialiased =
@@ -875,10 +896,10 @@ extern "C" int gsb_project_backward_activated_camgrad(int n, const float *means3
                                                       int antialiased, float *cam_partials, gsb_stream_t stream) {
     GSB_CHECK_ARG((accumulate == 0 || accumulate == 1) && (antialiased == 0 || antialiased == 1));
     GSB_CHECK_ARG(n >= 0 && (n == 0 || cam_partials));
-    return project_backward_impl(true, accumulate != 0, antialiased != 0, n, means3d, log_scales, glob_scale,
-                                 raw_quats, opacities, viewmat, projmat, fx, fy, img_h, img_w, radii, conics, v_xy,
-                                 v_depth, v_conic, v_opacity, v_mean3d, v_log_scales, v_raw_quats, v_opacity_logits,
-                                 cam_partials, stream);
+    return project_backward({PJ_ACT | PJ_CAMGRAD | pj_flag(accumulate, PJ_ACC) | pj_flag(antialiased, PJ_AA), n,
+                             means3d, log_scales, glob_scale, raw_quats, opacities, nullptr, viewmat, projmat, fx, fy,
+                             img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity, v_mean3d, v_log_scales,
+                             v_raw_quats, v_opacity_logits, cam_partials}, stream);
 }
 
 extern "C" int gsb_project_camera_grad_reduce(int nblocks, const float *partials, float *v_viewmat, float *v_projmat,
@@ -902,9 +923,10 @@ extern "C" int gsb_project_forward_activated_filter3d(int n, const float *means3
                                                       gsb_stream_t stream) {
     GSB_CHECK_ARG(antialiased == 0 || antialiased == 1);
     GSB_CHECK_ARG(n >= 0 && (n == 0 || filter3d));
-    return project_forward_impl(true, antialiased != 0, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
-                                filter3d, viewmat, projmat, fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y,
-                                clip_thresh, cov3d, xys, depths, radii, conics, num_tiles_hit, opacities, stream);
+    return project_forward({PJ_ACT | PJ_F3D | pj_flag(antialiased, PJ_AA), n, means3d, log_scales, glob_scale,
+                            raw_quats, opacity_logits, filter3d, viewmat, projmat, fx, fy, cx, cy, img_h, img_w,
+                            tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii, conics, num_tiles_hit,
+                            opacities}, stream);
 }
 
 // Its VJP with filter3d held constant, from the opacity logits: written or accumulated, plain or anti-aliased, with
@@ -922,10 +944,11 @@ extern "C" int gsb_project_backward_activated_filter3d(int n, const float *means
     GSB_CHECK_ARG((accumulate == 0 || accumulate == 1) && (antialiased == 0 || antialiased == 1) &&
                   (camgrad == 0 || camgrad == 1));
     GSB_CHECK_ARG(n >= 0 && (n == 0 || (filter3d && (!camgrad || cam_partials))));
-    return project_backward_impl(true, accumulate != 0, antialiased != 0, n, means3d, log_scales, glob_scale,
-                                 raw_quats, opacity_logits, viewmat, projmat, fx, fy, img_h, img_w, radii, conics,
-                                 v_xy, v_depth, v_conic, v_opacity, v_mean3d, v_log_scales, v_raw_quats,
-                                 v_opacity_logits, camgrad ? cam_partials : nullptr, stream, filter3d);
+    return project_backward({PJ_ACT | PJ_F3D | pj_flag(accumulate, PJ_ACC) | pj_flag(antialiased, PJ_AA) |
+                                 pj_flag(camgrad, PJ_CAMGRAD),
+                             n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, filter3d, viewmat, projmat,
+                             fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity, v_mean3d,
+                             v_log_scales, v_raw_quats, v_opacity_logits, camgrad ? cam_partials : nullptr}, stream);
 }
 
 // D27: the activated projection through an OpenCV fisheye camera (k1..k4; theta_lim from model.fisheye_theta_limit),
@@ -946,10 +969,10 @@ extern "C" int gsb_project_forward_fisheye(int n, const float *means3d, const fl
                                            float *opacities, int antialiased, gsb_stream_t stream) {
     GSB_CHECK_ARG(antialiased == 0 || antialiased == 1);
     if (const int e = fisheye_check(fx, fy, k1, k2, k3, k4, theta_lim)) return e;
-    const FishK fk = {k1, k2, k3, k4, theta_lim};
-    return project_forward_impl(true, antialiased != 0, n, means3d, log_scales, glob_scale, raw_quats, opacity_logits,
-                                nullptr, viewmat, nullptr, fx, fy, cx, cy, img_h, img_w, tiles_x, tiles_y, clip_thresh,
-                                cov3d, xys, depths, radii, conics, num_tiles_hit, opacities, stream, &fk);
+    return project_forward({PJ_ACT | PJ_FISH | pj_flag(antialiased, PJ_AA), n, means3d, log_scales, glob_scale,
+                            raw_quats, opacity_logits, nullptr, viewmat, nullptr, fx, fy, cx, cy, img_h, img_w,
+                            tiles_x, tiles_y, clip_thresh, cov3d, xys, depths, radii, conics, num_tiles_hit, opacities,
+                            {k1, k2, k3, k4, theta_lim}}, stream);
 }
 
 // Its VJP from the opacity logits: written or accumulated, plain or anti-aliased, and with the camera gradient when
@@ -965,9 +988,10 @@ extern "C" int gsb_project_backward_fisheye(int n, const float *means3d, const f
                                             gsb_stream_t stream) {
     GSB_CHECK_ARG((accumulate == 0 || accumulate == 1) && (antialiased == 0 || antialiased == 1));
     if (const int e = fisheye_check(fx, fy, k1, k2, k3, k4, theta_lim)) return e;
-    const FishK fk = {k1, k2, k3, k4, theta_lim};
-    return project_backward_impl(true, accumulate != 0, antialiased != 0, n, means3d, log_scales, glob_scale,
-                                 raw_quats, opacity_logits, viewmat, nullptr, fx, fy, img_h, img_w, radii, conics,
-                                 v_xy, v_depth, v_conic, v_opacity, v_mean3d, v_log_scales, v_raw_quats,
-                                 v_opacity_logits, cam_partials, stream, nullptr, &fk);
+    return project_backward({PJ_ACT | PJ_FISH | pj_flag(accumulate, PJ_ACC) | pj_flag(antialiased, PJ_AA) |
+                                 pj_flag(cam_partials != nullptr, PJ_CAMGRAD),
+                             n, means3d, log_scales, glob_scale, raw_quats, opacity_logits, nullptr, viewmat, nullptr,
+                             fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity, v_mean3d,
+                             v_log_scales, v_raw_quats, v_opacity_logits, cam_partials, {k1, k2, k3, k4, theta_lim}},
+                            stream);
 }

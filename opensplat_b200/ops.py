@@ -12,6 +12,8 @@ opensplat_b200/csrc/ops; this module is what the parity tests and bench.py drive
 All compute happens in libgsplat_b200.so (hand-written sm_90a CUDA); torch supplies memory, streams
 and the autograd graph.  CPU tensors are rejected -- there is no fallback path.
 """
+from typing import NamedTuple
+
 import torch
 
 from . import capi
@@ -617,6 +619,69 @@ class RasterizeGaussiansDepthClamped(RasterizeGaussiansDepth):
                                            depth_values=depthValues)
 
 
+class ProjectionMode(NamedTuple):
+    """How the activated projection runs: antialiased (D19), filter3d (D24: the [N] float32 3-D filter, held constant)
+    or None, and fisheye (D27: (k1, k2, k3, k4, theta_lim)) or None for a pinhole camera."""
+    antialiased: bool = False
+    filter3d: "torch.Tensor | None" = None
+    fisheye: "tuple | None" = None
+
+
+def project_activated_forward(L, mode, n, means, log_scales, glob_scale, quats, logits, viewmat, projmat, fx, fy, cx,
+                              cy, img_h, img_w, tile_bounds, clip_thresh, out, stream):
+    """The activated projection in `mode` through library L into out = (cov3d, xys, depths, radii, conics,
+    num_tiles_hit, opacities), every buffer a contiguous CUDA tensor.  A fisheye camera does not read projmat."""
+    P = capi.ptr
+    head = (n, P(means), P(log_scales), glob_scale, P(quats), P(logits))
+    tail = (img_h, img_w, tile_bounds[0], tile_bounds[1], clip_thresh) + tuple(P(t) for t in out)
+    if mode.fisheye is not None:
+        capi.check(L.gsb_project_forward_fisheye(*head, P(viewmat), fx, fy, cx, cy, *mode.fisheye, *tail,
+                                                 int(mode.antialiased), stream))
+    elif mode.filter3d is not None:
+        capi.check(L.gsb_project_forward_activated_filter3d(*head, P(mode.filter3d), P(viewmat), P(projmat), fx, fy,
+                                                            cx, cy, *tail, int(mode.antialiased), stream))
+    else:
+        project = L.gsb_project_forward_activated_aa if mode.antialiased else L.gsb_project_forward_activated
+        capi.check(project(*head, P(viewmat), P(projmat), fx, fy, cx, cy, *tail, stream))
+
+
+def project_activated_backward(L, mode, n, means, log_scales, glob_scale, quats, logits, sigmoid, viewmat, projmat,
+                               fx, fy, img_h, img_w, radii, conics, v_xy, v_depth, v_conic, v_opacity, grads, stream,
+                               accumulate=False, cam_grad=None, cam_partials=None):
+    """The VJP of project_activated_forward in `mode` into grads = (v_means, v_log_scales, v_quats, v_logits), written,
+    or added to them under `accumulate`.  sigmoid: the forward's opacities, read only by the pinhole projection without
+    AA or the 3-D filter (every other mode recomputes them from the logits).  v_depth and v_opacity may be None.
+    cam_grad (D22): (v_viewmat, v_projmat), [4,4] each, to receive the camera gradient, or None; cam_partials: its
+    per-block rows, gsb_project_camera_partials_floats(n) floats, allocated here when None."""
+    P = capi.ptr
+    if cam_grad is not None and cam_partials is None:
+        cam_partials = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, means)
+    part = P(cam_partials) if cam_grad is not None else None
+    plain = not mode.antialiased and mode.filter3d is None and mode.fisheye is None
+    head = (n, P(means), P(log_scales), glob_scale, P(quats), P(sigmoid if plain else logits))
+    tail = ((img_h, img_w, P(radii), P(conics), P(v_xy), P(v_depth), P(v_conic), P(v_opacity))
+            + tuple(P(t) for t in grads))
+    acc, aa = int(accumulate), int(mode.antialiased)
+    if mode.fisheye is not None:
+        capi.check(L.gsb_project_backward_fisheye(*head, P(viewmat), fx, fy, *mode.fisheye, *tail, acc, aa, part,
+                                                  stream))
+    elif mode.filter3d is not None:
+        capi.check(L.gsb_project_backward_activated_filter3d(*head, P(mode.filter3d), P(viewmat), P(projmat), fx, fy,
+                                                             *tail, acc, aa, int(cam_grad is not None), part, stream))
+    elif cam_grad is not None:
+        capi.check(L.gsb_project_backward_activated_camgrad(*head, P(viewmat), P(projmat), fx, fy, *tail, acc, aa, part,
+                                                            stream))
+    else:
+        if mode.antialiased:
+            project = L.gsb_project_backward_activated_aa_acc if acc else L.gsb_project_backward_activated_aa
+        else:
+            project = L.gsb_project_backward_activated_acc if acc else L.gsb_project_backward_activated
+        capi.check(project(*head, P(viewmat), P(projmat), fx, fy, *tail, stream))
+    if cam_grad is not None:
+        capi.check(L.gsb_project_camera_grad_reduce(cam_partials.numel() // capi.CAMGRAD_TERMS, part,
+                                                    P(cam_grad[0]), P(cam_grad[1]), stream))
+
+
 class ProjectGaussiansActivated(torch.autograd.Function):
     """ProjectGaussians on the RAW parameters of the model (model.cpp:148-150,200 + 152-165 as one operator):
     `scales` are log-scales (exp fused), `quats` un-normalised (the projection normalises), and the opacity logits
@@ -637,11 +702,18 @@ class ProjectGaussiansActivated(torch.autograd.Function):
 
     @staticmethod
     def _forward(ctx, aa, means, logScales, globScale, rawQuats, opacityLogits, viewMat, projMat, fx, fy, cx, cy,
-                 imgHeight, imgWidth, tileBounds, clipThresh, filter3D=None):
+                 imgHeight, imgWidth, tileBounds, clipThresh, filter3D=None, fisheye=None):
+        """The forward of every activated operator: projMat is None through a fisheye camera."""
         n = means.shape[0]
         m3, ls, rq = capi.f32(means), capi.f32(logScales), capi.f32(rawQuats)
         ol = capi.f32(opacityLogits).reshape(n)
-        vm, pm = capi.f32(viewMat), capi.f32(projMat)
+        vm, pm = capi.f32(viewMat), capi.f32(projMat) if projMat is not None else None
+        f3 = None
+        if filter3D is not None:
+            # D24: the 3-D filter, a constant [N] float32 (no gradient)
+            if filter3D.dtype != torch.float32 or tuple(filter3D.shape) != (n,) or filter3D.device != m3.device:
+                raise ValueError(f"filter3D must be a float32 [{n}] tensor on the means' device")
+            f3 = filter3D.detach().contiguous()
         cov3d = _empty((n, 6), torch.float32, m3)
         xys = _empty((n, 2), torch.float32, m3)
         depths = _empty((n,), torch.float32, m3)
@@ -649,33 +721,20 @@ class ProjectGaussiansActivated(torch.autograd.Function):
         conics = _empty((n, 3), torch.float32, m3)
         nth = _empty((n,), torch.int32, m3)
         opac = _empty((n, 1), torch.float32, m3)
-        L = capi.lib()
-        f3 = None
-        if filter3D is not None:
-            # D24: the 3-D filter, a constant [N] float32 (no gradient)
-            if filter3D.dtype != torch.float32 or tuple(filter3D.shape) != (n,) or filter3D.device != m3.device:
-                raise ValueError(f"filter3D must be a float32 [{n}] tensor on the means' device")
-            f3 = filter3D.detach().contiguous()
-        args = (n, capi.ptr(m3), capi.ptr(ls), float(globScale), capi.ptr(rq), capi.ptr(ol))
-        rest = (capi.ptr(vm), capi.ptr(pm), float(fx), float(fy), float(cx), float(cy), int(imgHeight),
-                int(imgWidth), tileBounds[0], tileBounds[1], float(clipThresh), capi.ptr(cov3d), capi.ptr(xys),
-                capi.ptr(depths), capi.ptr(radii), capi.ptr(conics), capi.ptr(nth), capi.ptr(opac))
-        if f3 is None:
-            capi.check((L.gsb_project_forward_activated_aa if aa else L.gsb_project_forward_activated)(
-                *args, *rest, capi.stream()))
-        else:
-            capi.check(L.gsb_project_forward_activated_filter3d(*args, capi.ptr(f3), *rest, int(aa), capi.stream()))
+        project_activated_forward(capi.lib(), ProjectionMode(aa, f3, fisheye), n, m3, ls, float(globScale), rq, ol, vm,
+                                  pm, float(fx), float(fy), float(cx), float(cy), int(imgHeight), int(imgWidth),
+                                  tileBounds, float(clipThresh), (cov3d, xys, depths, radii, conics, nth, opac),
+                                  capi.stream())
         ctx.meta = (float(globScale), float(fx), float(fy), int(imgHeight), int(imgWidth), tuple(opacityLogits.shape),
-                    aa, tuple(viewMat.shape), tuple(projMat.shape))
-        # the plain backward takes sigmoid(logits) from the forward, the anti-aliased and filtered ones the logits
-        ctx.save_for_backward(m3, ls, rq, vm, pm, radii, conics, ol if (aa or f3 is not None) else opac, f3)
+                    aa, fisheye)
+        ctx.save_for_backward(m3, ls, rq, ol, opac, vm, pm, radii, conics, f3)
         ctx.mark_non_differentiable(radii, nth)
         return xys, depths, radii, conics, nth, cov3d, opac
 
     @staticmethod
     def backward(ctx, v_xys, v_depths, v_radii, v_conics, v_numTiles, v_cov3d, v_opac):
-        m3, ls, rq, vm, pm, radii, conics, opac, f3 = ctx.saved_tensors
-        gs, fx, fy, H, W, ol_shape, aa, vm_shape, pm_shape = ctx.meta
+        m3, ls, rq, ol, opac, vm, pm, radii, conics, f3 = ctx.saved_tensors
+        gs, fx, fy, H, W, ol_shape, aa, fisheye = ctx.meta
         n = m3.shape[0]
         if v_xys is None:
             v_xys = torch.zeros_like(m3[:, :2])
@@ -685,35 +744,15 @@ class ProjectGaussiansActivated(torch.autograd.Function):
         v_ls = _empty((n, 3), torch.float32, m3)
         v_rq = _empty((n, 4), torch.float32, m3)
         v_ol = _empty((n,), torch.float32, m3)
-        vx, vc = capi.f32(v_xys), capi.f32(v_conics)
         vd = capi.f32(v_depths) if v_depths is not None else None
         vo = capi.f32(v_opac).reshape(n) if v_opac is not None else None
-        L = capi.lib()
-        args = (n, capi.ptr(m3), capi.ptr(ls), gs, capi.ptr(rq), capi.ptr(opac), capi.ptr(vm), capi.ptr(pm), fx, fy, H,
-                W, capi.ptr(radii), capi.ptr(conics), capi.ptr(vx), capi.ptr(vd), capi.ptr(vc), capi.ptr(vo),
-                capi.ptr(v_mean), capi.ptr(v_ls), capi.ptr(v_rq), capi.ptr(v_ol))
-        v_view = v_proj = None
-        camgrad = ctx.needs_input_grad[5] or ctx.needs_input_grad[6]
-        if f3 is not None:
-            # D24: opac holds the logits; the filter sits after them in the argument list
-            fargs = args[:6] + (capi.ptr(f3),) + args[6:]
-            part = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, m3) if camgrad else None
-            capi.check(L.gsb_project_backward_activated_filter3d(*fargs, 0, int(aa), int(camgrad), capi.ptr(part),
-                                                                 capi.stream()))
-        if camgrad:
-            # D22: the camera gradient, reduced over the Gaussians inside the projection backward
-            v_view = _empty((4, 4), torch.float32, m3)
-            v_proj = _empty((4, 4), torch.float32, m3)
-            if f3 is None:
-                part = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, m3)
-                capi.check(L.gsb_project_backward_activated_camgrad(*args, 0, int(aa), capi.ptr(part), capi.stream()))
-            capi.check(L.gsb_project_camera_grad_reduce(part.numel() // capi.CAMGRAD_TERMS, capi.ptr(part),
-                                                        capi.ptr(v_view), capi.ptr(v_proj), capi.stream()))
-            v_view = v_view.reshape(vm_shape) if ctx.needs_input_grad[5] else None
-            v_proj = v_proj.reshape(pm_shape) if ctx.needs_input_grad[6] else None
-        elif f3 is None:
-            capi.check((L.gsb_project_backward_activated_aa if aa else L.gsb_project_backward_activated)(
-                *args, capi.stream()))
+        want_view, want_proj = ctx.needs_input_grad[5], ctx.needs_input_grad[6]
+        cam = (_empty((4, 4), torch.float32, m3), _empty((4, 4), torch.float32, m3)) if want_view or want_proj else None
+        project_activated_backward(capi.lib(), ProjectionMode(aa, f3, fisheye), n, m3, ls, gs, rq, ol, opac, vm, pm, fx,
+                                   fy, H, W, radii, conics, capi.f32(v_xys), vd, capi.f32(v_conics), vo,
+                                   (v_mean, v_ls, v_rq, v_ol), capi.stream(), cam_grad=cam)
+        v_view = cam[0].reshape(vm.shape) if want_view else None
+        v_proj = cam[1].reshape(pm.shape) if want_proj else None
         # 16 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4), viewMat(5), projMat(6)
         return (v_mean, v_ls, None, v_rq, v_ol.reshape(ol_shape), v_view, v_proj) + (None,) * 9
 
@@ -743,65 +782,17 @@ class ProjectGaussiansFisheye(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means, logScales, globScale, rawQuats, opacityLogits, viewMat, fx, fy, cx, cy, k, thetaLim,
                 imgHeight, imgWidth, tileBounds, clipThresh=0.01, antialiased=False):
-        n = means.shape[0]
-        m3, ls, rq = capi.f32(means), capi.f32(logScales), capi.f32(rawQuats)
-        ol = capi.f32(opacityLogits).reshape(n)
-        vm = capi.f32(viewMat)
         k = tuple(float(x) for x in k)
         if len(k) != 4:
             raise ValueError("k takes the four fisheye coefficients (k1, k2, k3, k4)")
-        cov3d = _empty((n, 6), torch.float32, m3)
-        xys = _empty((n, 2), torch.float32, m3)
-        depths = _empty((n,), torch.float32, m3)
-        radii = _empty((n,), torch.int32, m3)
-        conics = _empty((n, 3), torch.float32, m3)
-        nth = _empty((n,), torch.int32, m3)
-        opac = _empty((n, 1), torch.float32, m3)
-        aa = bool(antialiased)
-        capi.check(capi.lib().gsb_project_forward_fisheye(
-            n, capi.ptr(m3), capi.ptr(ls), float(globScale), capi.ptr(rq), capi.ptr(ol), capi.ptr(vm), float(fx),
-            float(fy), float(cx), float(cy), *k, float(thetaLim), int(imgHeight), int(imgWidth), tileBounds[0],
-            tileBounds[1], float(clipThresh), capi.ptr(cov3d), capi.ptr(xys), capi.ptr(depths), capi.ptr(radii),
-            capi.ptr(conics), capi.ptr(nth), capi.ptr(opac), int(aa), capi.stream()))
-        ctx.meta = (float(globScale), float(fx), float(fy), k, float(thetaLim), int(imgHeight), int(imgWidth),
-                    tuple(opacityLogits.shape), aa, tuple(viewMat.shape))
-        ctx.save_for_backward(m3, ls, rq, ol, vm, radii, conics)
-        ctx.mark_non_differentiable(radii, nth)
-        return xys, depths, radii, conics, nth, cov3d, opac
+        return ProjectGaussiansActivated._forward(ctx, bool(antialiased), means, logScales, globScale, rawQuats,
+                                                  opacityLogits, viewMat, None, fx, fy, cx, cy, imgHeight, imgWidth,
+                                                  tileBounds, clipThresh, fisheye=k + (float(thetaLim),))
 
     @staticmethod
-    def backward(ctx, v_xys, v_depths, v_radii, v_conics, v_numTiles, v_cov3d, v_opac):
-        m3, ls, rq, ol, vm, radii, conics = ctx.saved_tensors
-        gs, fx, fy, k, th, H, W, ol_shape, aa, vm_shape = ctx.meta
-        n = m3.shape[0]
-        if v_xys is None:
-            v_xys = torch.zeros_like(m3[:, :2])
-        if v_conics is None:
-            v_conics = torch.zeros_like(conics)
-        v_mean = _empty((n, 3), torch.float32, m3)
-        v_ls = _empty((n, 3), torch.float32, m3)
-        v_rq = _empty((n, 4), torch.float32, m3)
-        v_ol = _empty((n,), torch.float32, m3)
-        vx, vc = capi.f32(v_xys), capi.f32(v_conics)
-        vd = capi.f32(v_depths) if v_depths is not None else None
-        vo = capi.f32(v_opac).reshape(n) if v_opac is not None else None
-        L = capi.lib()
-        camgrad = ctx.needs_input_grad[5]
-        part = _empty((L.gsb_project_camera_partials_floats(n),), torch.float32, m3) if camgrad else None
-        capi.check(L.gsb_project_backward_fisheye(
-            n, capi.ptr(m3), capi.ptr(ls), gs, capi.ptr(rq), capi.ptr(ol), capi.ptr(vm), fx, fy, *k, th, H, W,
-            capi.ptr(radii), capi.ptr(conics), capi.ptr(vx), capi.ptr(vd), capi.ptr(vc), capi.ptr(vo),
-            capi.ptr(v_mean), capi.ptr(v_ls), capi.ptr(v_rq), capi.ptr(v_ol), 0, int(aa), capi.ptr(part),
-            capi.stream()))
-        v_view = None
-        if camgrad:
-            v_view = _empty((4, 4), torch.float32, m3)
-            v_proj = _empty((4, 4), torch.float32, m3)
-            capi.check(L.gsb_project_camera_grad_reduce(part.numel() // capi.CAMGRAD_TERMS, capi.ptr(part),
-                                                        capi.ptr(v_view), capi.ptr(v_proj), capi.stream()))
-            v_view = v_view.reshape(vm_shape)
-        # 17 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4), viewMat(5)
-        return (v_mean, v_ls, None, v_rq, v_ol.reshape(ol_shape), v_view) + (None,) * 11
+    def backward(ctx, *grads):
+        # 17 slots; grads for means(0), logScales(1), rawQuats(3), opacityLogits(4), viewMat(5) (slot 6 is fx)
+        return ProjectGaussiansActivated.backward(ctx, *grads)[:6] + (None,) * 11
 
 
 class SphericalHarmonics(torch.autograd.Function):

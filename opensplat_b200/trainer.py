@@ -22,8 +22,8 @@ Several views per step (`views_per_step=B`, with or without a group):
 
 One step body serves every B; B = 1 is the default.  All B views render at the step's one resolution: one upload of
 the B cameras and the SH forward for the B camera centres; then each view runs projection, binning (its own host
-wait), blend, loss, rasterize-backward into its own colour slot, projection backward (the writing kernel for view 0,
-gsb_project_backward_activated_acc after it, so the geometry gradients sum over the views in place) and its
+wait), blend, loss, rasterize-backward into its own colour slot, projection backward (written by view 0 and added
+into by the views after it, so the geometry gradients sum over the views in place) and its
 densification statistics (densify.Densifier.accumulate_view, in view order); then the SH backward of the B colour
 gradients, one segmented Adam launch and the rest of Model::afterTrain (Densifier.finish_step).  Adam sees the mean
 over the B x G views (G ranks, 1 without a group).  The schedules (SH degree, downscale, means learning rate,
@@ -70,7 +70,7 @@ updates every grid.  evaluate(), render() and `image` stay the raw render.
 With per-image pose corrections (`pose=pose.PoseConfig(num_images=...)`, DESIGN D22) every step names its views'
 training images the same way.  Each view's camera is corrected on the device (gsb_pose_apply) between the upload and
 `proj @ view`; the step first writes reg * e into the corrections' gradient, each view's projection backward also
-reduces the camera gradient (gsb_project_backward_activated_camgrad, gsb_project_camera_grad_reduce), which
+reduces the camera gradient (ops.project_activated_backward's cam_grad), which
 gsb_pose_backward takes to 1/B of its image's correction gradient; after the Gaussians' Adam step one Adam step
 updates every correction.  evaluate() and render() take image= to render at that image's corrected pose.
 
@@ -84,7 +84,7 @@ returned stays the image loss; `depth_losses` holds the unweighted depth loss of
 
 With Mip-Splatting's 3-D smoothing filter (`filter3d=filter3d.Filter3DConfig(cameras=...)`, DESIGN D24) every
 projection, forward and backward, in step(), evaluate() and render(), takes the per-Gaussian filter f
-(gsb_project_*_activated_filter3d).  f is computed from the training cameras, uploaded once, at construction, after
+(ops.ProjectionMode.filter3d).  f is computed from the training cameras, uploaded once, at construction, after
 every step whose refinement ran and on filter3d.recompute_due's schedule once refinement has stopped; the alpha reset
 clamps the effective opacity, and save() writes the baked scene.  With pose corrections f uses the cameras as given,
 uncorrected.  Under a group every rank computes the same f from the same cameras (no collective).
@@ -214,7 +214,7 @@ class SplatTrainer:
         filter3d: a filter3d.Filter3DConfig to train and render with Mip-Splatting's 3-D smoothing filter (DESIGN
         D24) from its training cameras; save() then writes the baked scene.  Not available with fisheye cameras.
         Cameras: step(), evaluate() and render() take pinhole and fisheye (model.Camera(model="fisheye"), DESIGN D27)
-        cameras, mixed freely within a step; a fisheye view's projection is gsb_project_{forward,backward}_fisheye."""
+        cameras, mixed freely within a step; a fisheye view projects through ops.ProjectionMode.fisheye."""
         import torch.distributed as dist
         self.views_per_step = B = int(views_per_step)
         if B < 1:
@@ -325,7 +325,6 @@ class SplatTrainer:
             self.geom_ptrs = torch.tensor([pp.grad_flat.data_ptr()], dtype=torch.int64, device=d)
         if self.poses is not None:   # D22: the projection backward's per-block camera-gradient rows
             floats = self.L.gsb_project_camera_partials_floats(n)
-            self.cam_blocks = floats // capi.CAMGRAD_TERMS
             self.cam_partials = torch.empty(max(floats, 1), dtype=torch.float32, device=d)
         if self.filter3d_cfg is not None:   # D24: the 3-D filter, recomputed after every refinement
             self.f3d = torch.empty(n, dtype=torch.float32, device=d)
@@ -660,25 +659,20 @@ class SplatTrainer:
             self._theta_lims[k] = fisheye_theta_limit(*k)
         return k + (self._theta_lims[k],)
 
+    def _projection_mode(self, b):
+        """View b's ops.ProjectionMode: the trainer's anti-aliasing and 3-D filter, and the view's camera model."""
+        return ops.ProjectionMode(self.antialiased, self.f3d if self.filter3d_cfg is not None else None,
+                                  self.view_fisheye[b])
+
     def _project_blend(self, b, intr, out_img=None, out_depth=None, out_alpha=None, prior=False):
         """View b's projection with the activations from camera slot b (intrinsics `intr`), then binning and the
         clamped blend (the view's one host wait) into the pipeline's image, or into out_img with the depth and opacity
         maps (render()).  prior (D23): also 1/z where radii > 0, blended into depth_render."""
         pp, L, P, s = self.pipe, self.L, capi.ptr, capi.stream()
-        n, p, tb, H, W = pp.n, pp.p, pp.tb, pp.H, pp.W
-        fx, fy, cx, cy = intr
-        head = (n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(p["opacities"]))
-        tail = (P(self.viewmats[b]), P(self.projmats[b]), fx, fy, cx, cy, H, W, tb[0], tb[1], 0.01, P(pp.cov3d),
-                P(pp.xys), P(pp.depths), P(pp.radii), P(pp.conics), P(pp.nth), P(self.opac))
-        fish = self.view_fisheye[b]
-        if fish is not None:     # D27: no projmat; the distortion after the intrinsics
-            capi.check(L.gsb_project_forward_fisheye(*head, tail[0], *tail[2:6], *fish, *tail[6:],
-                                                     int(self.antialiased), s))
-        elif self.filter3d_cfg is not None:     # D24
-            capi.check(L.gsb_project_forward_activated_filter3d(*head, P(self.f3d), *tail, int(self.antialiased), s))
-        else:
-            project = L.gsb_project_forward_activated_aa if self.antialiased else L.gsb_project_forward_activated
-            capi.check(project(*head, *tail, s))
+        n, p = pp.n, pp.p
+        ops.project_activated_forward(L, self._projection_mode(b), n, p["means"], p["scales"], 1.0, p["quats"],
+                                      p["opacities"], self.viewmats[b], self.projmats[b], *intr, pp.H, pp.W, pp.tb,
+                                      0.01, (pp.cov3d, pp.xys, pp.depths, pp.radii, pp.conics, pp.nth, self.opac), s)
         if prior:
             capi.check(L.gsb_inverse_depths(n, P(pp.depths), P(pp.radii), P(self.inv_depths), s))
             out_depth, out_alpha = self.depth_render, self.depth_alpha
@@ -753,33 +747,15 @@ class SplatTrainer:
         if ex is not None and ex.overlap and b == self.views_per_step - 1:
             # every colour slot is final: colour pulls + SH expansion start now, on a side stream
             ex.start_colour(degrees_to_use=use, rgbs=self.rgbs_views)
-        if self.antialiased or self.filter3d_cfg is not None:     # D19, D24: the backward recomputes o from the logits
-            pj = L.gsb_project_backward_activated_aa if b == 0 else L.gsb_project_backward_activated_aa_acc
-            opac = p["opacities"]
-        else:
-            pj = L.gsb_project_backward_activated if b == 0 else L.gsb_project_backward_activated_acc
-            opac = self.opac
-        args = (n, P(p["means"]), P(p["scales"]), 1.0, P(p["quats"]), P(opac), P(self.viewmats[b]),
-                P(self.projmats[b]), fx, fy, pp.H, pp.W, P(pp.radii), P(pp.conics), P(pp.v_xy), P(v_depth),
-                P(pp.v_conic), P(self.v_opac), P(g["means"]), P(g["scales"]), P(g["quats"]), P(g["opacities"]))
-        s, po, fish = capi.stream(), self.poses, self.view_fisheye[b]
-        if fish is not None:     # D27: the logits in every mode, no projmat; accumulate, antialiased, cam_partials
-            capi.check(L.gsb_project_backward_fisheye(
-                *args[:5], P(p["opacities"]), args[6], fx, fy, *fish, *args[10:], int(b > 0), int(self.antialiased),
-                P(self.cam_partials) if po is not None else None, s))
-        elif self.filter3d_cfg is not None:     # D24: the filter after the logits; accumulate, antialiased, camgrad
-            capi.check(L.gsb_project_backward_activated_filter3d(
-                *args[:6], P(self.f3d), *args[6:], int(b > 0), int(self.antialiased), int(po is not None),
-                P(self.cam_partials) if po is not None else None, s))
-        elif po is None:
-            capi.check(pj(*args, s))
-        else:
-            capi.check(L.gsb_project_backward_activated_camgrad(*args, int(b > 0), int(self.antialiased),
-                                                                P(self.cam_partials), s))
+        s, po = capi.stream(), self.poses
+        cg, part = (self.cam_grads, self.cam_partials) if po is not None else (None, None)
+        ops.project_activated_backward(L, self._projection_mode(b), n, p["means"], p["scales"], 1.0, p["quats"],
+                                       p["opacities"], self.opac, self.viewmats[b], self.projmats[b], fx, fy, pp.H,
+                                       pp.W, pp.radii, pp.conics, pp.v_xy, v_depth, pp.v_conic, self.v_opac,
+                                       (g["means"], g["scales"], g["quats"], g["opacities"]), s, accumulate=b > 0,
+                                       cam_grad=cg, cam_partials=part)
         if po is None:
             return
-        cg = self.cam_grads
-        capi.check(L.gsb_project_camera_grad_reduce(self.cam_blocks, P(self.cam_partials), P(cg[0]), P(cg[1]), s))
         capi.check(L.gsb_pose_backward(P(po.deltas[image]), P(self.base_viewmats[b]), P(self.projs[b]), P(cg[0]),
                                        P(cg[1]), 1.0 / self.views_per_step, P(po.grad[image]), s))
 
