@@ -23,12 +23,13 @@ import torch
 
 import project_aa_f64 as paa
 import project_f64 as pf
-from project_f64 import C03, F8, R, rexp, rwhere
+from project_f64 import F8, R, rexp
 
 U = pf.U
 U64 = 2.0 ** -53
 C = 2.0
 TREE_DEPTH = 12                       # 5 shuffle levels + 7 sequential warp sums
+CG_ROW = 24                           # the terms of one partial row: viewmat rows 0..2, projmat rows 0, 1, 3
 ALTS = ("left", "columns", "no_fold", "no_JvT", "centre_unmoved")
 
 
@@ -66,80 +67,48 @@ def camgrad_autograd(cam, means, scales, quats, logits, v_xy, v_conic, v_opacity
     return gv.reshape(4, 4).detach(), gp.reshape(4, 4).detach()
 
 
-def _dS(f, kept, o, vo):
-    """The anti-aliased comp term added to vS (project_aa_f64.project's, in the kernel's order)."""
-    comp, pos, _, (cxx0, cxy, cyy0) = paa._comp_tree(f)
-    pos = pos & kept
-    safe = R(torch.where(pos, comp.v, torch.ones_like(comp.v)), comp.b)
-    k = 0.5 * (R(vo) * o) / safe
-    idet = 1.0 / f["det"]
-    ea, eb, ec, ee = cyy0 * idet, cxy * idet, cxx0 * idet, C03 * idet
-    return (pos, k * (C03 * (ea * ea + eb * eb + ee * ea)), k * (C03 * (eb * (ea + ec + ee))),
-            k * (C03 * (ec * ec + eb * eb + ee * ec)))
-
-
-def camgrad_terms(cam, f, v_xy, v_conic, dS, alt=None):
-    """The kernel's 24 terms per Gaussian on R: viewmat rows 0..2, then projmat rows 0, 1, 3 (each 4 floats)."""
-    V = [float(x) for x in cam.V]
-    fx, fy = cam.fx, cam.fy
-    hx, hy, hw = f["h"]
-    rw = f["rw"]
-    vndcx, vndcy = (0.5 * float(cam.W)) * v_xy[0], (0.5 * float(cam.H)) * v_xy[1]
-    vhx, vhy = vndcx * rw, vndcy * rw
-    vhw = -(vndcx * hx + vndcy * hy) * rw * rw
-    A, B, Cc = f["conic"]
-    gA, gB, gC = v_conic[0], 0.5 * v_conic[1], v_conic[2]
-    xg00, xg01 = A * gA + B * gB, A * gB + B * gC
-    xg10, xg11 = B * gA + Cc * gB, B * gB + Cc * gC
-    vS00 = -(xg00 * A + xg01 * B)
-    vS01 = -(xg00 * B + xg01 * Cc)
-    vS11 = -(xg10 * B + xg11 * Cc)
-    mask, d00, d01, d11 = dS
-    vS00 = rwhere(mask, vS00 + d00, vS00)
-    vS01 = rwhere(mask, vS01 - d01, vS01)
-    vS11 = rwhere(mask, vS11 + d11, vS11)
-    T, Cs = f["T"], f["C"]
-    ttx, tty = f["tt"]
-    cqx, cqy = f["cq"]
-    qx, qy = f["q"]
-    rz, rz2 = f["rz"]
-    rz3 = rz2 * rz
-    vST = [[vS00 * T[0][c] + vS01 * T[1][c] for c in range(3)], [vS01 * T[0][c] + vS11 * T[1][c] for c in range(3)]]
-    vT = [[2.0 * (vST[r][0] * Cs[0][c] + vST[r][1] * Cs[1][c] + vST[r][2] * Cs[2][c]) for c in range(3)]
-          for r in range(2)]
-    vJ00 = vT[0][0] * V[0] + vT[0][1] * V[1] + vT[0][2] * V[2]
-    vJ02 = vT[0][0] * V[8] + vT[0][1] * V[9] + vT[0][2] * V[10]
-    vJ11 = vT[1][0] * V[4] + vT[1][1] * V[5] + vT[1][2] * V[6]
-    vJ12 = vT[1][0] * V[8] + vT[1][1] * V[9] + vT[1][2] * V[10]
-    vttx, vtty = -fx * rz2 * vJ02, -fy * rz2 * vJ12
-    vtz = R(torch.zeros_like(rz.v)) + (-fx * rz2 * vJ00 + 2.0 * fx * ttx * rz3 * vJ02 - fy * rz2 * vJ11
-                                       + 2.0 * fy * tty * rz3 * vJ12)
-    vt = []
-    for qq, cq, vtt, lim in ((qx, cqx, vttx, f["lim"][0]), (qy, cqy, vtty, f["lim"][1])):
-        tie = (qq.v == lim) | (qq.v == -lim)
-        clamped = ~((qq.v > -lim) & (qq.v < lim))
-        h = 0.5 * vtt
-        vt.append(rwhere(tie, h, rwhere(clamped, 0.0, vtt)))
-        vtz = rwhere(tie, vtz + cq * h, rwhere(clamped, vtz + cq * vtt, vtz))
-    vt.append(vtz)
-    J00, J11 = fx * rz, fy * rz
-    J02, J12 = -fx * ttx * rz2, -fy * tty * rz2
-    p = f["p"]
+def camgrad_terms(f, p, extra, alt=None):
+    """The kernel's 24 terms per Gaussian on R, viewmat rows 0..2 then projmat rows 0, 1, 3 (each 4 floats), from the
+    forward tree f, the means p and the backward tree's vt, vT, vh (`extra` of project_f64._backward_tree).  Row r of
+    the viewmat gets vt_r (p, 1) plus column c's J^T vT: the pinhole's J00, J11 and (J02, J12), or the fisheye's full
+    J (f["Jf"]), whose projmat rows are 0.  alt "no_JvT": the J^T vT columns dropped."""
+    vt, vT, vh = extra["vt"], extra["vT"], extra["vh"]
     terms = []
     for r in range(3):
         row = [vt[r] * p[c] for c in range(3)] + [vt[r]]
         if alt != "no_JvT":
             for c in range(3):
-                if r == 0:
-                    row[c] = row[c] + J00 * vT[0][c]
+                if "Jf" in f:
+                    Jf = f["Jf"]
+                    row[c] = row[c] + (Jf[0][r] * vT[0][c] + Jf[1][r] * vT[1][c])
+                elif r == 0:
+                    row[c] = row[c] + f["J"][0] * vT[0][c]
                 elif r == 1:
-                    row[c] = row[c] + J11 * vT[1][c]
+                    row[c] = row[c] + f["J"][2] * vT[1][c]
                 else:
-                    row[c] = row[c] + (J02 * vT[0][c] + J12 * vT[1][c])
+                    row[c] = row[c] + (f["J"][1] * vT[0][c] + f["J"][3] * vT[1][c])
         terms += row
-    for vh in (vhx, vhy, vhw):
-        terms += [vh * p[c] for c in range(3)] + [vh]
+    for h in vh:
+        terms += [h * p[c] for c in range(3)] + [h]
     return terms
+
+
+def camgrad_sum(terms, kept):
+    """The kernel's sums of the per-Gaussian terms over `kept`: (G_V, G_P, B_V, B_P), float64 [4,4] each on the terms'
+    device (the bound as in the module docstring; row 3 of G_V and row 2 of G_P are 0 with bound 0)."""
+    n = kept.shape[0]
+    z = torch.zeros((), dtype=F8, device=kept.device)
+    val = torch.stack([torch.where(kept, t.v, z).sum() for t in terms])
+    bsum = torch.stack([torch.where(kept, t.b, z).sum() for t in terms])
+    asum = torch.stack([torch.where(kept, t.v.abs(), z).sum() for t in terms])
+    nb = (n + 255) // 256
+    bound = C * (bsum + gamma(TREE_DEPTH) * (asum + bsum)) + gamma(nb + 5, U64) * (asum + bsum) + U * val.abs()
+    GV, GP, BV, BP = (torch.zeros((4, 4), dtype=F8, device=kept.device) for _ in range(4))
+    GV[:3] = val[:12].reshape(3, 4)
+    BV[:3] = bound[:12].reshape(3, 4)
+    GP[[0, 1, 3]] = val[12:].reshape(3, 4)
+    BP[[0, 1, 3]] = bound[12:].reshape(3, 4)
+    return GV, GP, BV, BP
 
 
 def camgrad_tree(cam, means, scales, quats, logits, v_xy, v_conic, v_opacity=None, aa=False, kept=None, alt=None):
@@ -151,26 +120,16 @@ def camgrad_tree(cam, means, scales, quats, logits, v_xy, v_conic, v_opacity=Non
     vx, vc = pf._t(v_xy, dev).reshape(n, 2), pf._t(v_conic, dev).reshape(n, 3)
     kept = torch.ones(n, dtype=torch.bool) if kept is None else torch.as_tensor(kept).cpu()
     p = [R(m[:, i]) for i in range(3)]
-    f = pf._forward_tree(cam, p, [R(a[:, i]) for i in range(3)], [R(q[:, i]) for i in range(4)], 1.0, True, "cuda")
-    f["p"] = p
+    qr = [R(q[:, i]) for i in range(4)]
+    f = pf._forward_tree(cam, p, [R(a[:, i]) for i in range(3)], qr, 1.0, True, "cuda")
+    dS = None
     if aa and v_opacity is not None:
         o = 1.0 / (1.0 + rexp(-R(ol)))
-        dS = _dS(f, kept, o, pf._t(v_opacity, dev).reshape(n))
-    else:
-        dS = (torch.zeros(n, dtype=torch.bool), 0.0, 0.0, 0.0)
-    terms = camgrad_terms(cam, f, [R(vx[:, 0]), R(vx[:, 1])], [R(vc[:, i]) for i in range(3)], dS, alt)
-    z = torch.zeros((), dtype=F8)
-    val = torch.stack([torch.where(kept, t.v, z).sum() for t in terms])
-    bsum = torch.stack([torch.where(kept, t.b, z).sum() for t in terms])
-    asum = torch.stack([torch.where(kept, t.v.abs(), z).sum() for t in terms])
-    nb = (n + 255) // 256
-    bound = C * (bsum + gamma(TREE_DEPTH) * (asum + bsum)) + gamma(nb + 5, U64) * (asum + bsum) + U * val.abs()
-    GV, GP, BV, BP = (torch.zeros((4, 4), dtype=F8) for _ in range(4))
-    GV[:3] = val[:12].reshape(3, 4)
-    BV[:3] = bound[:12].reshape(3, 4)
-    GP[[0, 1, 3]] = val[12:].reshape(3, 4)
-    BP[[0, 1, 3]] = bound[12:].reshape(3, 4)
-    return GV, GP, BV, BP
+        dS = paa.comp_dS(f, kept, o, pf._t(v_opacity, dev).reshape(n))
+    extra = {}
+    pf._backward_tree(cam, f, qr, 1.0, True, f["conic"], [R(vx[:, 0]), R(vx[:, 1])], R(torch.zeros(n, dtype=F8)),
+                      [R(vc[:, i]) for i in range(3)], dS, extra)
+    return camgrad_sum(camgrad_terms(f, p, extra, alt), kept)
 
 
 # ------------------------------------------------------------------------------------------------ pose chain

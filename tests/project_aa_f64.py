@@ -8,8 +8,8 @@ written map, sigmoid(l) * sqrt(clamp_min(det S0 / det(S0 + 0.3 I), 0)) chained o
 comp = 0 (det0 <= 0) the comp term contributes nothing (the chosen subgradient).
 
 The bound.  `_comp_tree` follows the forward kernel's operations in order (the three sums before the blur from the
-forward tree's T and cov3d, det0, the ratio, sqrtf) and `_backward_tree_aa` the backward kernel's: project_f64's
-_backward_tree with the comp term added to vS before the T / J / clamp chain, evaluated as the kernel does, and
+forward tree's T and cov3d, det0, the ratio, sqrtf) and the backward is project_f64's _backward_tree with the comp
+term `comp_dS` added to vS before the T / J / clamp chain, evaluated as the kernel does, and
 v_logit = ((v comp) o) (1 - o).  The tree's values must equal autograd's, which pins its restatement.
 
 The certificate adds one decision to project_f64's: det0 / det > 0 (the fmaxf), clear of 0 by its bound or exact
@@ -17,7 +17,7 @@ The certificate adds one decision to project_f64's: det0 / det > 0 (the fmaxf), 
 import torch
 
 import project_f64 as pf
-from project_f64 import C03, F8, R, rexp, rwhere, sqrtf
+from project_f64 import C03, F8, R, rexp, sqrtf
 
 ALTS = ("offdiag_full", "comp_eps", "no_comp_in_vlogit", "swap_dets")
 
@@ -44,70 +44,20 @@ def _comp_tree(f, alt=None):
     return R(torch.where(pos, c.v, zero), torch.where(pos, c.b, zero)), pos, ratio, (cxx0, cxy, cyy0)
 
 
-def _backward_tree_aa(cam, f, q, glob_scale, conic, v_xy, v_depth, v_conic, dS):
-    """project_f64._backward_tree (activated) with dS = (d00, d01, d11) added to vS00, vS01, vS11 where given."""
-    V, P = [float(x) for x in cam.V], [float(x) for x in cam.P]
-    fx, fy = cam.fx, cam.fy
-    hx, hy, hw = f["h"]
-    rw = f["rw"]
-    vndcx, vndcy = (0.5 * float(cam.W)) * v_xy[0], (0.5 * float(cam.H)) * v_xy[1]
-    vhx, vhy = vndcx * rw, vndcy * rw
-    vhw = -(vndcx * hx + vndcy * hy) * rw * rw
-    vm = [P[c] * vhx + P[4 + c] * vhy + P[12 + c] * vhw for c in range(3)]
-    vtz = v_depth
-    A, B, Cc = conic
-    gA, gB, gC = v_conic[0], 0.5 * v_conic[1], v_conic[2]
-    xg00, xg01 = A * gA + B * gB, A * gB + B * gC
-    xg10, xg11 = B * gA + Cc * gB, B * gB + Cc * gC
-    vS00 = -(xg00 * A + xg01 * B)
-    vS01 = -(xg00 * B + xg01 * Cc)
-    vS11 = -(xg10 * B + xg11 * Cc)
-    mask, d00, d01, d11 = dS
-    vS00 = rwhere(mask, vS00 + d00, vS00)
-    vS01 = rwhere(mask, vS01 - d01, vS01)
-    vS11 = rwhere(mask, vS11 + d11, vS11)
-    T, Cs, M, Rm, e, s = f["T"], f["C"], f["M"], f["Rm"], f["e"], f["s"]
-    ttx, tty = f["tt"]
-    cqx, cqy = f["cq"]
-    qx, qy = f["q"]
-    rz, rz2 = f["rz"]
-    rz3 = rz2 * rz
-    vST = [[vS00 * T[0][c] + vS01 * T[1][c] for c in range(3)], [vS01 * T[0][c] + vS11 * T[1][c] for c in range(3)]]
-    vV = [[T[0][r] * vST[0][c] + T[1][r] * vST[1][c] for c in range(3)] for r in range(3)]
-    vT = [[2.0 * (vST[r][0] * Cs[0][c] + vST[r][1] * Cs[1][c] + vST[r][2] * Cs[2][c]) for c in range(3)]
-          for r in range(2)]
-    vJ00 = vT[0][0] * V[0] + vT[0][1] * V[1] + vT[0][2] * V[2]
-    vJ02 = vT[0][0] * V[8] + vT[0][1] * V[9] + vT[0][2] * V[10]
-    vJ11 = vT[1][0] * V[4] + vT[1][1] * V[5] + vT[1][2] * V[6]
-    vJ12 = vT[1][0] * V[8] + vT[1][1] * V[9] + vT[1][2] * V[10]
-    vttx, vtty = -fx * rz2 * vJ02, -fy * rz2 * vJ12
-    vtz = vtz + (-fx * rz2 * vJ00 + 2.0 * fx * ttx * rz3 * vJ02 - fy * rz2 * vJ11 + 2.0 * fy * tty * rz3 * vJ12)
-    vt = []
-    for qq, cq, vtt, lim in ((qx, cqx, vttx, f["lim"][0]), (qy, cqy, vtty, f["lim"][1])):
-        tie = (qq.v == lim) | (qq.v == -lim)
-        clamped = ~((qq.v > -lim) & (qq.v < lim))
-        h = 0.5 * vtt
-        vt.append(rwhere(tie, h, rwhere(clamped, 0.0, vtt)))
-        vtz = rwhere(tie, vtz + cq * h, rwhere(clamped, vtz + cq * vtt, vtz))
-    vtx, vty = vt
-    vm = [vm[c] + (V[c] * vtx + V[4 + c] * vty + V[8 + c] * vtz) for c in range(3)]
-    vM = [[2.0 * (vV[r][0] * M[0][c] + vV[r][1] * M[1][c] + vV[r][2] * M[2][c]) for c in range(3)] for r in range(3)]
-    vs = [glob_scale * (Rm[0][c] * vM[0][c] + Rm[1][c] * vM[1][c] + Rm[2][c] * vM[2][c]) * e[c] for c in range(3)]
-    vR = [[vM[r][c] * s[c] for c in range(3)] for r in range(3)]
-    qw_, qx_, qy_, qz_ = q
-    nq = sqrtf(qw_ * qw_ + qx_ * qx_ + qy_ * qy_ + qz_ * qz_)
-    inv = 1.0 / nq
-    w, x, y, z = qw_ * inv, qx_ * inv, qy_ * inv, qz_ * inv
-    gw = 2.0 * (x * (vR[2][1] - vR[1][2]) + y * (vR[0][2] - vR[2][0]) + z * (vR[1][0] - vR[0][1]))
-    gx = 2.0 * (-2.0 * x * (vR[1][1] + vR[2][2]) + y * (vR[1][0] + vR[0][1]) + z * (vR[2][0] + vR[0][2])
-                + w * (vR[2][1] - vR[1][2]))
-    gy = 2.0 * (x * (vR[1][0] + vR[0][1]) - 2.0 * y * (vR[0][0] + vR[2][2]) + z * (vR[2][1] + vR[1][2])
-                + w * (vR[0][2] - vR[2][0]))
-    gz = 2.0 * (x * (vR[2][0] + vR[0][2]) + y * (vR[2][1] + vR[1][2]) - 2.0 * z * (vR[0][0] + vR[1][1])
-                + w * (vR[1][0] - vR[0][1]))
-    dot = w * gw + x * gx + y * gy + z * gz
-    vq = [(gw - w * dot) * inv, (gx - x * dot) * inv, (gy - y * dot) * inv, (gz - z * dot) * inv]
-    return vm, vs, vq
+def comp_dS(f, kept, oe, vo, alt=None):
+    """The comp term the backward kernel adds to vS, (mask, d00, d01, d11) on R: k = 0.5 (v_o oe) / comp, id = 1 / det,
+    (a, b, c, e) = (cyy0, cxy, cxx0, 0.3) id; mask = ratio > 0 on `kept`.  oe: the opacity comp multiplies, sigmoid(l)
+    (times c3 under the 3-D filter).  alt "comp_eps" / "offdiag_full": ALTS."""
+    comp, pos, _, (cxx0, cxy, cyy0) = _comp_tree(f, alt)
+    pos = pos & kept
+    safe = R(torch.where(pos, comp.v, torch.ones_like(comp.v)), comp.b)
+    k = 0.5 * (R(vo) * oe) / (safe + pf.f32(1e-6) if alt == "comp_eps" else safe)
+    idet = 1.0 / f["det"]
+    ea, eb, ec, ee = cyy0 * idet, cxy * idet, cxx0 * idet, C03 * idet
+    d00 = k * (C03 * (ea * ea + eb * eb + ee * ea))
+    d01 = k * (C03 * (eb * (ea + ec + ee)))
+    d11 = k * (C03 * (ec * ec + eb * eb + ee * ec))
+    return pos, d00, (2.0 * d01 if alt == "offdiag_full" else d01), d11
 
 
 # ------------------------------------------------------------------------------------------------ autograd map
@@ -168,7 +118,7 @@ def project_aa(cam, means, scales, quats, opacity_logits, glob_scale=1.0, v_xy=N
     f = pf._forward_tree(cam, [R(m[:, i]) for i in range(3)], [R(a[:, i]) for i in range(3)],
                          [R(q[:, i]) for i in range(4)], glob_scale, True, "cuda")
     kept = out["radii"] > 0
-    comp, pos, ratio, (cxx0, cxy, cyy0) = _comp_tree(f, alt)
+    comp, pos, ratio, _ = _comp_tree(f, alt)
     z = torch.zeros((), dtype=F8, device=dev)
     comp = R(torch.where(kept, comp.v, z), torch.where(kept, comp.b, z))
     pos = pos & kept
@@ -185,21 +135,8 @@ def project_aa(cam, means, scales, quats, opacity_logits, glob_scale=1.0, v_xy=N
     vd = pf._t(v_depth, dev).reshape(n) if v_depth is not None else torch.zeros(n, dtype=F8, device=dev)
     vo = pf._t(v_opacity, dev).reshape(n) if v_opacity is not None else None
     g = vjp_aa(cam, m, a, q, ol, vx, vd, vc, vo, glob_scale, kept)
-    if vo is not None:
-        # the kernel: k = 0.5 (v o) / comp, id = 1 / det, (a, b, c, e) = (cyy0, cxy, cxx0, 0.3) id
-        safe = R(torch.where(pos, comp.v, torch.ones_like(comp.v)), comp.b)
-        k = 0.5 * (R(vo) * o) / (safe + pf.f32(1e-6) if alt == "comp_eps" else safe)
-        idet = 1.0 / f["det"]
-        ea, eb, ec, ee = cyy0 * idet, cxy * idet, cxx0 * idet, C03 * idet
-        d00 = k * (C03 * (ea * ea + eb * eb + ee * ea))
-        d01 = k * (C03 * (eb * (ea + ec + ee)))
-        d11 = k * (C03 * (ec * ec + eb * eb + ee * ec))
-        if alt == "offdiag_full":
-            d01 = 2.0 * d01
-        dS = (pos, d00, d01, d11)
-    else:
-        dS = (torch.zeros_like(pos), 0.0, 0.0, 0.0)
-    vm, vs, vq = _backward_tree_aa(cam, f, [R(q[:, i]) for i in range(4)], glob_scale, f["conic"],
+    dS = comp_dS(f, kept, o, vo, alt) if vo is not None else None
+    vm, vs, vq = pf._backward_tree(cam, f, [R(q[:, i]) for i in range(4)], glob_scale, True, f["conic"],
                                    [R(vx[:, 0]), R(vx[:, 1])], R(vd), [R(vc[:, i]) for i in range(3)], dS)
 
     def stack(rs, mask):

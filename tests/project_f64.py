@@ -165,18 +165,44 @@ def _quat_to_rotmat(qw, qx, qy, qz):
             [2.0 * (x * z - w * y), 2.0 * (y * z + w * x), 1.0 - 2.0 * (x * x + y * y)]]
 
 
-def _forward_tree(cam, p, a, q, glob_scale, act, d3):
-    """project_forward_kernel's tree on R.  p [3] means, a [3] (log-)scales, q [4] raw quaternion, each R over [N]."""
-    V, P = [float(x) for x in cam.V], [float(x) for x in cam.P]
-    px, py, pz = p
-    tx = V[0] * px + V[1] * py + V[2] * pz + V[3]
-    ty = V[4] * px + V[5] * py + V[6] * pz + V[7]
-    tz = V[8] * px + V[9] * py + V[10] * pz + V[11]
+def _filter3d_scales(s, f3):
+    """filter3d_scales of project.cu on R: sigma_k = sqrtf(s_k s_k + f f), r_k = s_k / sigma_k, c3 = (r_0 r_1) r_2."""
+    ff = f3 * f3
+    sig = [sqrtf(x * x + ff) for x in s]
+    fr = [x / g for x, g in zip(s, sig)]
+    return sig, fr, fr[0] * fr[1] * fr[2]
+
+
+def _covariance(q, a, glob_scale, act, f3=None):
+    """R(q / |q|), e (exp of the log-scales under act), s = glob_scale e, and M = R S, cov3d = M M^T on R; with the
+    3-D filter f3 (an R over [N]) S holds sigma_k and the dict also fr (r_k), c3 and f3."""
     Rm = _quat_to_rotmat(*q)
     e = [rexp(x) if act else x for x in a]
     s = [glob_scale * x for x in e]
+    out = dict(Rm=Rm, e=e)
+    if f3 is not None:
+        s, fr, c3 = _filter3d_scales(s, f3)
+        out.update(fr=fr, c3=c3, f3=f3)
     M = [[Rm[r][c] * s[c] for c in range(3)] for r in range(3)]
     C = [[M[r][0] * M[c][0] + M[r][1] * M[c][1] + M[r][2] * M[c][2] for c in range(3)] for r in range(3)]
+    out.update(s=s, M=M, C=C, cov3d=[C[0][0], C[0][1], C[0][2], C[1][1], C[1][2], C[2][2]])
+    return out
+
+
+def _view(V, p):
+    px, py, pz = p
+    return (V[0] * px + V[1] * py + V[2] * pz + V[3], V[4] * px + V[5] * py + V[6] * pz + V[7],
+            V[8] * px + V[9] * py + V[10] * pz + V[11])
+
+
+def _forward_tree(cam, p, a, q, glob_scale, act, d3, f3=None):
+    """project_forward_kernel's tree on R.  p [3] means, a [3] (log-)scales, q [4] raw quaternion, each R over [N];
+    f3: the F3D mode's filter (an R over [N]), or None."""
+    V, P = [float(x) for x in cam.V], [float(x) for x in cam.P]
+    px, py, pz = p
+    tx, ty, tz = _view(V, p)
+    cv = _covariance(q, a, glob_scale, act, f3)
+    C = cv["C"]
     lim_x, lim_y = (cam.lim_x, cam.lim_y) if d3 == "cuda" else (cam.lim_x_cpu, cam.lim_y_cpu)
     qx, qy = tx / tz, ty / tz
     cqx, cqy = rmin(rmax(qx, -lim_x), lim_x), rmin(rmax(qy, -lim_y), lim_y)
@@ -205,15 +231,70 @@ def _forward_tree(cam, p, a, q, glob_scale, act, d3):
     cx, cy = (cam.cx, cam.cy) if d3 == "cuda" else (0.5 * cam.W, 0.5 * cam.H)
     pxc = 0.5 * float(cam.W) * ndcx + cx - 0.5
     pyc = 0.5 * float(cam.H) * ndcy + cy - 0.5
-    cov3d = [C[0][0], C[0][1], C[0][2], C[1][1], C[1][2], C[2][2]]
-    return dict(t=(tx, ty, tz), q=(qx, qy), cq=(cqx, cqy), tt=(ttx, tty), rz=(rz, rz2), T=T, Rm=Rm, e=e, s=s, M=M,
-                C=C, cov3d=cov3d, det=det, conic=conic, r3=r3, h=(hx, hy, hw), rw=rw, xy=(pxc, pyc),
-                lim=(lim_x, lim_y))
+    return dict(cv, t=(tx, ty, tz), q=(qx, qy), cq=(cqx, cqy), tt=(ttx, tty), rz=(rz, rz2), J=(J00, J02, J11, J12),
+                T=T, det=det, conic=conic, r3=r3, h=(hx, hy, hw), rw=rw, xy=(pxc, pyc), lim=(lim_x, lim_y))
 
 
-def _backward_tree(cam, f, q, glob_scale, act, conic, v_xy, v_depth, v_conic):
+def _vS(conic, v_conic, dS=None):
+    """v_Sigma = -X G X from the conic and its cotangent, plus the anti-aliased dS = (mask, d00, d01, d11) where given
+    (project_aa_f64.comp_dS), in the kernel's order."""
+    A, B, Cc = conic
+    gA, gB, gC = v_conic[0], 0.5 * v_conic[1], v_conic[2]
+    xg00, xg01 = A * gA + B * gB, A * gB + B * gC
+    xg10, xg11 = B * gA + Cc * gB, B * gB + Cc * gC
+    vS00 = -(xg00 * A + xg01 * B)
+    vS01 = -(xg00 * B + xg01 * Cc)
+    vS11 = -(xg10 * B + xg11 * Cc)
+    if dS is not None:
+        mask, d00, d01, d11 = dS
+        vS00 = rwhere(mask, vS00 + d00, vS00)
+        vS01 = rwhere(mask, vS01 - d01, vS01)
+        vS11 = rwhere(mask, vS11 + d11, vS11)
+    return vS00, vS01, vS11
+
+
+def _cov2d_chain(T, Cs, vS):
+    """(vV, vT): cov2d = T cov3d T^T taken back to cov3d and to T."""
+    vS00, vS01, vS11 = vS
+    vST = [[vS00 * T[0][c] + vS01 * T[1][c] for c in range(3)], [vS01 * T[0][c] + vS11 * T[1][c] for c in range(3)]]
+    vV = [[T[0][r] * vST[0][c] + T[1][r] * vST[1][c] for c in range(3)] for r in range(3)]
+    vT = [[2.0 * (vST[r][0] * Cs[0][c] + vST[r][1] * Cs[1][c] + vST[r][2] * Cs[2][c]) for c in range(3)]
+          for r in range(2)]
+    return vV, vT
+
+
+def _scale_quat(f, q, glob_scale, act, vV):
+    """(v_scale, v_quat) from vV = d/d cov3d: M = R S, the log-scale's exp under act, and the F3D factor r_k where the
+    forward tree carries the filter (S then holds sigma_k)."""
+    M, Rm, e, s = f["M"], f["Rm"], f["e"], f["s"]
+    vM = [[2.0 * (vV[r][0] * M[0][c] + vV[r][1] * M[1][c] + vV[r][2] * M[2][c]) for c in range(3)] for r in range(3)]
+    vs = [glob_scale * (Rm[0][c] * vM[0][c] + Rm[1][c] * vM[1][c] + Rm[2][c] * vM[2][c]) for c in range(3)]
+    if act:
+        vs = [vs[c] * e[c] for c in range(3)]
+    if "fr" in f:
+        vs = [vs[c] * f["fr"][c] for c in range(3)]
+    vR = [[vM[r][c] * s[c] for c in range(3)] for r in range(3)]
+    qw_, qx_, qy_, qz_ = q
+    nq = sqrtf(qw_ * qw_ + qx_ * qx_ + qy_ * qy_ + qz_ * qz_)
+    inv = 1.0 / nq
+    w, x, y, z = qw_ * inv, qx_ * inv, qy_ * inv, qz_ * inv
+    gw = 2.0 * (x * (vR[2][1] - vR[1][2]) + y * (vR[0][2] - vR[2][0]) + z * (vR[1][0] - vR[0][1]))
+    gx = 2.0 * (-2.0 * x * (vR[1][1] + vR[2][2]) + y * (vR[1][0] + vR[0][1]) + z * (vR[2][0] + vR[0][2])
+                + w * (vR[2][1] - vR[1][2]))
+    gy = 2.0 * (x * (vR[1][0] + vR[0][1]) - 2.0 * y * (vR[0][0] + vR[2][2]) + z * (vR[2][1] + vR[1][2])
+                + w * (vR[0][2] - vR[2][0]))
+    gz = 2.0 * (x * (vR[2][0] + vR[0][2]) + y * (vR[2][1] + vR[1][2]) - 2.0 * z * (vR[0][0] + vR[1][1])
+                + w * (vR[1][0] - vR[0][1]))
+    dot = w * gw + x * gx + y * gy + z * gz
+    vq = [(gw - w * dot) * inv, (gx - x * dot) * inv, (gy - y * dot) * inv, (gz - z * dot) * inv]
+    return vs, vq
+
+
+def _backward_tree(cam, f, q, glob_scale, act, conic, v_xy, v_depth, v_conic, dS=None, extra=None):
     """project_backward_kernel's tree on R, from the forward tree's intermediates (the kernel recomputes the same
-    values in the same order) and the forward's conic (which carries the forward's bound)."""
+    values in the same order) and the forward's conic (which carries the forward's bound).  dS: the anti-aliased
+    term added to vS (project_aa_f64.comp_dS).  extra: a dict that receives vt, vT and vh, the camera gradient's
+    inputs."""
     V, P = [float(x) for x in cam.V], [float(x) for x in cam.P]
     fx, fy = cam.fx, cam.fy
     hx, hy, hw = f["h"]
@@ -223,23 +304,12 @@ def _backward_tree(cam, f, q, glob_scale, act, conic, v_xy, v_depth, v_conic):
     vhw = -(vndcx * hx + vndcy * hy) * rw * rw
     vm = [P[c] * vhx + P[4 + c] * vhy + P[12 + c] * vhw for c in range(3)]
     vtz = v_depth
-    A, B, Cc = conic
-    gA, gB, gC = v_conic[0], 0.5 * v_conic[1], v_conic[2]
-    xg00, xg01 = A * gA + B * gB, A * gB + B * gC
-    xg10, xg11 = B * gA + Cc * gB, B * gB + Cc * gC
-    vS00 = -(xg00 * A + xg01 * B)
-    vS01 = -(xg00 * B + xg01 * Cc)
-    vS11 = -(xg10 * B + xg11 * Cc)
-    T, Cs, M, Rm, e, s = f["T"], f["C"], f["M"], f["Rm"], f["e"], f["s"]
+    vV, vT = _cov2d_chain(f["T"], f["C"], _vS(conic, v_conic, dS))
     ttx, tty = f["tt"]
     cqx, cqy = f["cq"]
     qx, qy = f["q"]
     rz, rz2 = f["rz"]
     rz3 = rz2 * rz
-    vST = [[vS00 * T[0][c] + vS01 * T[1][c] for c in range(3)], [vS01 * T[0][c] + vS11 * T[1][c] for c in range(3)]]
-    vV = [[T[0][r] * vST[0][c] + T[1][r] * vST[1][c] for c in range(3)] for r in range(3)]
-    vT = [[2.0 * (vST[r][0] * Cs[0][c] + vST[r][1] * Cs[1][c] + vST[r][2] * Cs[2][c]) for c in range(3)]
-          for r in range(2)]
     vJ00 = vT[0][0] * V[0] + vT[0][1] * V[1] + vT[0][2] * V[2]
     vJ02 = vT[0][0] * V[8] + vT[0][1] * V[9] + vT[0][2] * V[10]
     vJ11 = vT[1][0] * V[4] + vT[1][1] * V[5] + vT[1][2] * V[6]
@@ -255,24 +325,9 @@ def _backward_tree(cam, f, q, glob_scale, act, conic, v_xy, v_depth, v_conic):
         vtz = rwhere(tie, vtz + cq * h, rwhere(clamped, vtz + cq * vtt, vtz))
     vtx, vty = vt
     vm = [vm[c] + (V[c] * vtx + V[4 + c] * vty + V[8 + c] * vtz) for c in range(3)]
-    vM = [[2.0 * (vV[r][0] * M[0][c] + vV[r][1] * M[1][c] + vV[r][2] * M[2][c]) for c in range(3)] for r in range(3)]
-    vs = [glob_scale * (Rm[0][c] * vM[0][c] + Rm[1][c] * vM[1][c] + Rm[2][c] * vM[2][c]) for c in range(3)]
-    if act:
-        vs = [vs[c] * e[c] for c in range(3)]
-    vR = [[vM[r][c] * s[c] for c in range(3)] for r in range(3)]
-    qw_, qx_, qy_, qz_ = q
-    nq = sqrtf(qw_ * qw_ + qx_ * qx_ + qy_ * qy_ + qz_ * qz_)
-    inv = 1.0 / nq
-    w, x, y, z = qw_ * inv, qx_ * inv, qy_ * inv, qz_ * inv
-    gw = 2.0 * (x * (vR[2][1] - vR[1][2]) + y * (vR[0][2] - vR[2][0]) + z * (vR[1][0] - vR[0][1]))
-    gx = 2.0 * (-2.0 * x * (vR[1][1] + vR[2][2]) + y * (vR[1][0] + vR[0][1]) + z * (vR[2][0] + vR[0][2])
-                + w * (vR[2][1] - vR[1][2]))
-    gy = 2.0 * (x * (vR[1][0] + vR[0][1]) - 2.0 * y * (vR[0][0] + vR[2][2]) + z * (vR[2][1] + vR[1][2])
-                + w * (vR[0][2] - vR[2][0]))
-    gz = 2.0 * (x * (vR[2][0] + vR[0][2]) + y * (vR[2][1] + vR[1][2]) - 2.0 * z * (vR[0][0] + vR[1][1])
-                + w * (vR[1][0] - vR[0][1]))
-    dot = w * gw + x * gx + y * gy + z * gz
-    vq = [(gw - w * dot) * inv, (gx - x * dot) * inv, (gy - y * dot) * inv, (gz - z * dot) * inv]
+    if extra is not None:
+        extra.update(vt=(vtx, vty, vtz), vT=vT, vh=(vhx, vhy, vhw))
+    vs, vq = _scale_quat(f, q, glob_scale, act, vV)
     return vm, vs, vq
 
 
@@ -370,20 +425,17 @@ def _exact32(cam, means):
     return tz.to(F8), (tx / tz).to(F8), (ty / tz).to(F8)
 
 
-def project(cam, means, scales, quats, glob_scale=1.0, act=False, opacity_logits=None, v_xy=None, v_depth=None,
-            v_conic=None, v_opacity=None, d3="cuda", device=None):
-    """The float64 reference of gsb_project_forward[_activated] and, with cotangents, gsb_project_backward[_activated].
-    Inputs are the kernels' fp32 inputs (numpy or torch); everything returned is float64 (radii / num_tiles_hit
-    int64) on `device` (default: that of `means`).  Keys: the forward outputs cov3d, xys, depths, radii, conics,
-    num_tiles_hit (and opacities) with bounds B_<name>; kept (radii > 0); cert; the decisions' own flags
-    (exact_tz, tie_x, tie_y, clamp_x, clamp_y); with v_xy / v_conic given, v_mean3d, v_scale, v_quat (and
-    v_opacity_logits) from autograd, their bounds B_<name>, and re_<name>, the values of the bound's evaluation."""
-    dev = device if device is not None else (means.device if torch.is_tensor(means) else "cpu")
-    m, a, q = _t(means, dev), _t(scales, dev), _t(quats, dev)
-    n = m.shape[0]
-    ol = _t(opacity_logits, dev).reshape(n) if opacity_logits is not None else None
-    f = _forward_tree(cam, [R(m[:, i]) for i in range(3)], [R(a[:, i]) for i in range(3)],
-                      [R(q[:, i]) for i in range(4)], glob_scale, act, d3)
+def stack_masked(rs, mask):
+    """(values, bounds) of a list of R as [N, len] float64, 0 (bound 0) outside mask."""
+    z = torch.zeros((), dtype=F8, device=mask.device)
+    return (torch.stack([torch.where(mask, r.v.to(F8), z) for r in rs], -1),
+            torch.stack([torch.where(mask, r.b.to(F8), z) for r in rs], -1))
+
+
+def forward_outputs(cam, f, m, d3="cuda"):
+    """The forward outputs of a forward tree f (pinhole, any mode): cov3d, xys, depths, radii, conics, num_tiles_hit
+    with bounds B_<name>, kept, cert and the decisions' flags.  m: the means (float64 [N,3])."""
+    dev, n = m.device, m.shape[0]
     tx, ty, tz = f["t"]
     front = tz.v > cam.clip
     tz32, qx32, qy32 = _exact32(cam, m)
@@ -418,18 +470,40 @@ def project(cam, means, scales, quats, glob_scale=1.0, act=False, opacity_logits
     out = dict(kept=kept, front=front, cert=cert, exact_tz=exact_tz,
                tie_x=front & ((qx.v == lim_x) | (qx.v == -lim_x)), tie_y=front & ((qy.v == lim_y) | (qy.v == -lim_y)),
                clamp_x=front & (qx.v.abs() > lim_x), clamp_y=front & (qy.v.abs() > lim_y))
-
-    def stack(rs, mask):
-        v = torch.stack([torch.where(mask, r.v, z) for r in rs], -1)
-        b = torch.stack([torch.where(mask, r.b, z) for r in rs], -1)
-        return v, b
-
+    stack = stack_masked
     out["cov3d"], out["B_cov3d"] = stack(f["cov3d"], front)
     out["conics"], out["B_conics"] = stack(f["conic"], has_conic)
     out["xys"], out["B_xys"] = stack([pxc, pyc], kept)
     out["depths"], out["B_depths"] = torch.where(kept, tz.v, z), torch.where(kept, tz.b, z)
     out["radii"] = torch.where(kept, radius, z).to(torch.int64)
     out["num_tiles_hit"] = torch.where(kept, area, torch.zeros_like(area))
+    return out
+
+
+def project(cam, means, scales, quats, glob_scale=1.0, act=False, opacity_logits=None, v_xy=None, v_depth=None,
+            v_conic=None, v_opacity=None, d3="cuda", device=None):
+    """The float64 reference of gsb_project_forward[_activated] and, with cotangents, gsb_project_backward[_activated].
+    Inputs are the kernels' fp32 inputs (numpy or torch); everything returned is float64 (radii / num_tiles_hit
+    int64) on `device` (default: that of `means`).  Keys: the forward outputs cov3d, xys, depths, radii, conics,
+    num_tiles_hit (and opacities) with bounds B_<name>; kept (radii > 0); cert; the decisions' own flags
+    (exact_tz, tie_x, tie_y, clamp_x, clamp_y); with v_xy / v_conic given, v_mean3d, v_scale, v_quat (and
+    v_opacity_logits) from autograd, their bounds B_<name>, and re_<name>, the values of the bound's evaluation."""
+    dev = device if device is not None else (means.device if torch.is_tensor(means) else "cpu")
+    m, a, q = _t(means, dev), _t(scales, dev), _t(quats, dev)
+    n = m.shape[0]
+    ol = _t(opacity_logits, dev).reshape(n) if opacity_logits is not None else None
+    f = _forward_tree(cam, [R(m[:, i]) for i in range(3)], [R(a[:, i]) for i in range(3)],
+                      [R(q[:, i]) for i in range(4)], glob_scale, act, d3)
+    out = forward_outputs(cam, f, m, d3)
+    tz = f["t"][2]
+    kept = out["kept"]
+    z = torch.zeros((), dtype=F8, device=dev)
+
+    def stack(rs, mask):
+        v = torch.stack([torch.where(mask, r.v, z) for r in rs], -1)
+        b = torch.stack([torch.where(mask, r.b, z) for r in rs], -1)
+        return v, b
+
     if act:
         o = 1.0 / (1.0 + rexp(-R(ol)))
         out["opacities"], out["B_opacities"] = o.v, o.b

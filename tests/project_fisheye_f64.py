@@ -22,7 +22,8 @@ import math
 import numpy as np
 import torch
 
-from project_f64 import (C03, C01, F8, TILE, R, U, _quat_to_rotmat, _trunc_box, f32, rexp, rmax, sqrtf)
+import project_f64 as pf
+from project_f64 import C03, C01, F8, TILE, R, U, _covariance, _trunc_box, _view, f32, rexp, rmax, sqrtf
 
 ATAN2_ULP = 4.0          # device atan2f: 2 ulp <= 4 u |result| (CUDA C Programming Guide, maximum ulp error table)
 RHO = f32(0.1)           # FISH_RHO: the small-r switch
@@ -55,8 +56,11 @@ class FishCam:
         self.tiles_x, self.tiles_y = (self.W + TILE - 1) // TILE, (self.H + TILE - 1) // TILE
 
 
-def _fisheye_terms(k, tx, ty, tz):
-    """fisheye_terms<false> on R: (r, theta, g, h, q, series branch mask, |r - 0.1f t.z| certified)."""
+def _fisheye_terms(k, tx, ty, tz, second=False, alt=None):
+    """fisheye_terms<second> on R: (r, theta, g, h, q, series branch mask, |r - 0.1f t.z| certified), and with
+    `second` w, m and qz, the second derivatives the backward's J VJP needs.  Below the switch the series' first
+    dropped terms are added to the bounds: c5 rho^10 in G, 10 c5 rho^8 in H and 80 c5 rho^6 in W.  alt "series_sign":
+    the sign of H's rho^2 term flipped, for the sensitivity checks."""
     k1, k2, k3, k4 = k
     r2 = tx * tx + ty * ty
     r = sqrtf(r2)
@@ -76,7 +80,8 @@ def _fisheye_terms(k, tx, ty, tz):
     iz2 = iz * iz
     p2 = r2 * iz2
     G = 1.0 + p2 * (c1 + p2 * (c2 + p2 * (c3 + p2 * c4)))
-    H = 2.0 * c1 + p2 * (4.0 * c2 + p2 * (6.0 * c3 + p2 * (8.0 * c4)))
+    Ht = p2 * (4.0 * c2 + p2 * (6.0 * c3 + p2 * (8.0 * c4)))
+    H = 2.0 * c1 - Ht if alt == "series_sign" else 2.0 * c1 + Ht
     c5 = abs(series_c5(k))
     gs, hs = G * iz, H * (iz2 * iz)
     gs = R(gs.v, gs.b + c5 * p2.v ** 5 / tz.v.abs())
@@ -92,21 +97,28 @@ def _fisheye_terms(k, tx, ty, tz):
     d_switch = (r.v - sw.v).abs() > (r.b + sw.b)
     g = R(torch.where(series, gs.v, gd.v), torch.where(series, gs.b, gd.b))
     h = R(torch.where(series, hs.v, hd.v), torch.where(series, hs.b, hd.b))
-    return dict(r=r, theta=theta, g=g, h=h, q=q, series=series, d_switch=d_switch)
+    out = dict(r=r, r2=r2, theta=theta, g=g, h=h, q=q, series=series, d_switch=d_switch)
+    if second:
+        W = 8.0 * c2 + p2 * (24.0 * c3 + p2 * (48.0 * c4))
+        ws = W * ((iz2 * iz2) * iz)
+        ws = R(ws.v, ws.b + 80.0 * c5 * p2.v ** 3 / tz.v.abs() ** 5)
+        ms = (3.0 * hs + r2 * ws) / tz
+        E = 6.0 * kr[0] + t2 * (20.0 * kr[1] + t2 * (42.0 * kr[2] + t2 * (72.0 * kr[3])))
+        md = (E * tz * (theta / rs) - 2.0 * D) / (n2 * n2)
+        wd = (tz * md - 3.0 * hd) / r2s
+        m = R(torch.where(series, ms.v, md.v), torch.where(series, ms.b, md.b))
+        out.update(w=R(torch.where(series, ws.v, wd.v), torch.where(series, ws.b, wd.b)), m=m,
+                   qz=(-(2.0 * q + r2 * m)) / tz)
+    return out
 
 
-def _forward_tree(cam, p, a, q, glob_scale):
+def _forward_tree(cam, p, a, q, glob_scale, second=False, alt=None):
+    """project_forward_kernel<ACT, AA, false, true>'s tree on R (with `second` also the backward's w, m, qz)."""
     V = [float(x) for x in cam.V]
-    px, py, pz = p
-    tx = V[0] * px + V[1] * py + V[2] * pz + V[3]
-    ty = V[4] * px + V[5] * py + V[6] * pz + V[7]
-    tz = V[8] * px + V[9] * py + V[10] * pz + V[11]
-    Rm = _quat_to_rotmat(*q)
-    e = [rexp(x) for x in a]
-    s = [glob_scale * x for x in e]
-    M = [[Rm[r][c] * s[c] for c in range(3)] for r in range(3)]
-    C = [[M[r][0] * M[c][0] + M[r][1] * M[c][1] + M[r][2] * M[c][2] for c in range(3)] for r in range(3)]
-    f = _fisheye_terms(cam.k, tx, ty, tz)
+    tx, ty, tz = _view(V, p)
+    cv = _covariance(q, a, glob_scale, True)
+    C = cv["C"]
+    f = _fisheye_terms(cam.k, tx, ty, tz, second, alt)
     g, h, qq = f["g"], f["h"], f["q"]
     fx, fy = cam.fx, cam.fy
     xy = tx * ty
@@ -127,8 +139,38 @@ def _forward_tree(cam, p, a, q, glob_scale):
     pxc = fx * (g * tx) + cam.cx - 0.5
     pyc = fy * (g * ty) + cam.cy - 0.5
     comp = sqrtf(rmax((cxx0 * cyy0 - cxy * cxy) / det, 0.0))
-    return dict(t=(tx, ty, tz), f=f, cov3d=[C[0][0], C[0][1], C[0][2], C[1][1], C[1][2], C[2][2]], det=det,
-                conic=conic, r3=r3, xy=(pxc, pyc), comp=comp)
+    return dict(cv, t=(tx, ty, tz), f=f, Jf=J, T=T, det=det, conic=conic, r3=r3, xy=(pxc, pyc), comp=comp)
+
+
+def _backward_tree(cam, f, q, glob_scale, conic, v_xy, v_depth, v_conic, dS=None, extra=None, alt=None):
+    """project_backward_kernel<.., FISH>'s tree on R from a forward tree built with `second`: project_f64's vS and
+    cov2d chain and its v_scale / v_quat, and between them the fisheye's J^T (v_u, v_v) plus sum_rc vJ_rc dJ_rc / dt,
+    in the kernel's order.  extra: receives vt, vT and vh (0: no projmat).  alt "no_Jderiv": w, m and qz taken as 0."""
+    V = [float(x) for x in cam.V]
+    fx, fy = cam.fx, cam.fy
+    tx, ty, tz = f["t"]
+    ft, Jf = f["f"], f["Jf"]
+    vV, vT = pf._cov2d_chain(f["T"], f["C"], pf._vS(conic, v_conic, dS))
+    A = [[(fx if r == 0 else fy) * (vT[r][0] * V[4 * c] + vT[r][1] * V[4 * c + 1] + vT[r][2] * V[4 * c + 2])
+          for c in range(3)] for r in range(2)]
+    h, qq = ft["h"], ft["q"]
+    w, m, qz = (R(torch.zeros_like(tz.v)),) * 3 if alt == "no_Jderiv" else (ft["w"], ft["m"], ft["qz"])
+    xx, yy, xy = tx * tx, ty * ty, tx * ty
+    hx, hy, S = h + xx * w, h + yy * w, A[0][1] + A[1][0]
+    qxm, qym, xym = qq + xx * m, qq + yy * m, xy * m
+    vx, vy = v_xy
+    vtx = (Jf[0][0] * vx + Jf[1][0] * vy + A[0][0] * (tx * (2.0 * h + hx)) + S * (ty * hx) + A[1][1] * (tx * hy)
+           - A[0][2] * qxm - A[1][2] * xym)
+    vty = (Jf[0][1] * vx + Jf[1][1] * vy + A[0][0] * (ty * hx) + S * (tx * hy) + A[1][1] * (ty * (2.0 * h + hy))
+           - A[0][2] * xym - A[1][2] * qym)
+    vtz = (v_depth + Jf[0][2] * vx + Jf[1][2] * vy - A[0][0] * qxm - S * xym - A[1][1] * qym
+           - (A[0][2] * tx + A[1][2] * ty) * qz)
+    vm = [V[c] * vtx + V[4 + c] * vty + V[8 + c] * vtz for c in range(3)]
+    if extra is not None:
+        z = R(torch.zeros_like(tz.v))
+        extra.update(vt=(vtx, vty, vtz), vT=vT, vh=(z, z, z))
+    vs, vq = pf._scale_quat(f, q, glob_scale, True, vV)
+    return vm, vs, vq
 
 
 def _t(a, dev):
@@ -187,16 +229,9 @@ def pixel_map(t, k, fx, fy, cx, cy, alt=None):
     return torch.stack([fx * g * tx + cx - half, fy * g * ty + cy - half], -1)
 
 
-def project(cam, means, scales, quats, logits, aa=False, v_xy=None, v_depth=None, v_conic=None, v_opacity=None,
-            device=None):
-    """The float64 reference of gsb_project_forward_fisheye and, with cotangents, of gsb_project_backward_fisheye.
-    Returns the forward outputs (xys, depths, radii, conics, num_tiles_hit, cov3d, opacities) with bounds B_<name>,
-    kept, cert, the decision flags, and with cotangents v_mean3d, v_scale, v_quat, v_opacity_logits (autograd)."""
-    dev = device if device is not None else (means.device if torch.is_tensor(means) else "cpu")
-    m, a, q, ol = _t(means, dev), _t(scales, dev), _t(quats, dev), _t(logits, dev).reshape(-1)
-    n = m.shape[0]
-    f = _forward_tree(cam, [R(m[:, i]) for i in range(3)], [R(a[:, i]) for i in range(3)],
-                      [R(q[:, i]) for i in range(4)], 1.0)
+def forward_outputs(cam, f, n, dev):
+    """The forward outputs of a fisheye forward tree f: cov3d, xys, depths, radii, conics, num_tiles_hit with bounds
+    B_<name>, kept, cert and the decisions' flags (front, in_fov, series)."""
     tx, ty, tz = f["t"]
     th = f["f"]["theta"]
     front = tz.v > cam.clip
@@ -223,10 +258,7 @@ def project(cam, means, scales, quats, logits, aa=False, v_xy=None, v_depth=None
     cert = d_front & (~front | (d_fov & (~in_fov | (f["f"]["d_switch"] & d_det & d_ceil & d_box))))
     z = torch.zeros((), dtype=F8, device=dev)
     out = dict(kept=kept, front=front, in_fov=in_fov, cert=cert, series=vis & f["f"]["series"])
-
-    def stack(rs, mask):
-        return (torch.stack([torch.where(mask, r.v, z) for r in rs], -1),
-                torch.stack([torch.where(mask, r.b, z) for r in rs], -1))
+    stack = pf.stack_masked
 
     out["cov3d"], out["B_cov3d"] = stack(f["cov3d"], vis)
     out["conics"], out["B_conics"] = stack(f["conic"], has_conic)
@@ -234,6 +266,22 @@ def project(cam, means, scales, quats, logits, aa=False, v_xy=None, v_depth=None
     out["depths"], out["B_depths"] = torch.where(kept, tz.v, z), torch.where(kept, tz.b, z)
     out["radii"] = torch.where(kept, radius, z).to(torch.int64)
     out["num_tiles_hit"] = torch.where(kept, area, torch.zeros_like(area))
+    return out
+
+
+def project(cam, means, scales, quats, logits, aa=False, v_xy=None, v_depth=None, v_conic=None, v_opacity=None,
+            device=None):
+    """The float64 reference of gsb_project_forward_fisheye and, with cotangents, of gsb_project_backward_fisheye.
+    Returns the forward outputs (xys, depths, radii, conics, num_tiles_hit, cov3d, opacities) with bounds B_<name>,
+    kept, cert, the decision flags, and with cotangents v_mean3d, v_scale, v_quat, v_opacity_logits (autograd)."""
+    dev = device if device is not None else (means.device if torch.is_tensor(means) else "cpu")
+    m, a, q, ol = _t(means, dev), _t(scales, dev), _t(quats, dev), _t(logits, dev).reshape(-1)
+    n = m.shape[0]
+    f = _forward_tree(cam, [R(m[:, i]) for i in range(3)], [R(a[:, i]) for i in range(3)],
+                      [R(q[:, i]) for i in range(4)], 1.0)
+    out = forward_outputs(cam, f, n, dev)
+    kept = out["kept"]
+    z = torch.zeros((), dtype=F8, device=dev)
     o = 1.0 / (1.0 + rexp(-R(ol)))
     if aa:
         comp = f["comp"]
@@ -257,10 +305,11 @@ def project(cam, means, scales, quats, logits, aa=False, v_xy=None, v_depth=None
     return out
 
 
-def random_fisheye_gaussians(cam, n, seed, frac_axis=0.05, frac_switch=0.1, frac_out=0.08, frac_behind=0.04):
+def random_fisheye_gaussians(cam, n, seed, frac_axis=0.05, frac_switch=0.1, frac_out=0.08, frac_behind=0.04,
+                             px=(0.3, 0.1)):
     """Gaussians in a fisheye camera's view (fp32 means, log-scales, raw quats, logits): directions out to theta_lim,
     some exactly on the axis (t.x = t.y = 0), some either side of the small-r switch rho = 0.1, some beyond theta_lim
-    and some behind the camera; footprints from under a pixel to a tenth of the image."""
+    and some behind the camera; footprints from px[0] pixels to px[1] of the image width."""
     rng = np.random.default_rng(seed)
     tz_dist = np.exp(rng.uniform(np.log(0.5), np.log(20.0), n))
     theta = np.sqrt(rng.uniform(0, 1, n)) * cam.theta_lim * 0.999
@@ -284,7 +333,7 @@ def random_fisheye_gaussians(cam, n, seed, frac_axis=0.05, frac_switch=0.1, frac
     if np.array_equal(cam.V.reshape(4, 4), np.eye(4, dtype=np.float32)):
         means = t
     dist = np.linalg.norm(t, axis=1)
-    px = np.exp(rng.uniform(np.log(0.3), np.log(0.1 * cam.W), (n, 3)))
+    px = np.exp(rng.uniform(np.log(px[0]), np.log(px[1] * cam.W), (n, 3)))
     scales = np.log(px * dist[:, None] / cam.fx)
     quats = rng.standard_normal((n, 4)) * np.exp(rng.uniform(np.log(0.5), np.log(2.0), (n, 1)))
     logits = rng.normal(0, 2, n)
